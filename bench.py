@@ -1,6 +1,7 @@
 """bench.py — image-text pairs/sec, forward+backward, VisualBERT-base (BASELINE.json metric).
 
-    python bench.py --gpus 1 --steps 10 --warmup 3                    # this build (CUDA, sm_100a)
+    python bench.py --gpus 1 --steps 10 --warmup 3                    # this build (CUDA, sm_90a)
+    python bench.py --gpus 1 --steps 10 --warmup 3 --dump-outputs DIR # + what the last timed step computed, as .npy
     python bench.py --impl reference --gpus 1 --steps 3 --warmup 1    # the reference's CPU arithmetic (oracle port)
     python -m torch.distributed.run --nproc-per-node N ... bench.py --gpus N ...
 
@@ -11,9 +12,9 @@ fp32 gradient buffer inside the timed step.
 One step = zero grads -> forward -> loss.backward() (+ all-reduce); the optimizer is excluded on both the GPU
 and the CPU side, as BASELINE.md §2 specifies for this metric.
 
-Printed JSON (one line, rank 0): the driver contract plus
-  roofline      dominant kernel family (gemm_tcgen05_kernel): algorithmic FLOPs / CUDA-event kernel time measured
-                live inside the timed steps (vb_profile_*), against MEASURED_PEAKS.json bf16_tflops_sustained
+Printed JSON (one line, rank 0): the benchmark result plus
+  roofline      dominant kernel family (gemm_wgmma_kernel): algorithmic FLOPs / CUDA-event kernel time measured
+                live inside the timed steps (vb_profile_*), against the H100 SXM data-sheet dense BF16 rate
   step_roofline the whole step: hot-path algorithmic FLOPs per pair (SURVEY.md §8d, heads excluded) x pairs/s
   cpu_baseline  the oracle (CPU restatement of the reference, oracle/vb_oracle.py) on a bounded sample
   e2e           same step through the public API with inputs in pinned HOST memory (H2D + loss D2H inside)
@@ -45,17 +46,12 @@ def hot_path_flops_per_pair(c):
 
 
 def load_peaks():
-    path = os.path.join(ROOT, "MEASURED_PEAKS.json")
-    if os.path.exists(path):
-        with open(path) as f:
-            p = json.load(f)
-        return dict(bf16_sustained=p.get("bf16_tflops_sustained", 1400.0), bf16_burst=p.get("bf16_tflops", 1590.0),
-                    hbm=p.get("hbm_gbs", 6650.0), source="measured (MEASURED_PEAKS.json)")
-    return dict(bf16_sustained=1400.0, bf16_burst=1590.0, hbm=6650.0, source="fallback (B200_PROFILING.md)")
+    """NVIDIA's H100 SXM data sheet (dense, 700 W): a ceiling to divide by, not a rate this card was seen to reach."""
+    return dict(bf16=989.0, hbm=3350.0, source="H100 SXM data sheet (dense BF16, 700 W)")
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons sampled DURING the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons sampled DURING the timed region (read-only queries)."""
     Q = ("clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,"
          "clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
 
@@ -226,6 +222,7 @@ def run_ours(args):
     h2d_bytes = sum(v.numel() * v.element_size() for v in resident.values() if torch.is_tensor(v))
 
     lscale = sync.loss_scale()   # 1 / world: the mean over ranks is folded into the loss, no divide pass over the buffer
+    last = {}
 
     def step(batch):
         sync.zero()
@@ -234,6 +231,7 @@ def run_ours(args):
         sync.allreduce(prescaled=True)
         if opt is not None:
             opt.step()
+        last["out"] = out
         return out["loss"]
 
     def barrier():
@@ -265,6 +263,9 @@ def run_ours(args):
         clk.mark()
         ms_total = timed(lambda: step(resident), args.steps)
         launches = _lib.launch_count() - n0
+        if args.dump_outputs and rank == 0:
+            dump_outputs(args.dump_outputs, last["out"], sync.flat)
+        last.clear()
         # ---- roofline pass: the SAME K steps again with a CUDA-event pair around every launch of the library ----
         _lib.profile_read()
         _lib.profile_enable(True)
@@ -365,7 +366,7 @@ def run_ours(args):
             ms2 = timed(step2, k2) / k2
             others[name] = {"workload": workload_name(oc), "per_gpu_batch": oc["B"], "global_batch": world * oc["B"],
                             "seq_len": oc["T"] + oc["V"], "ms_per_step": ms2, "value": world * oc["B"] / (ms2 * 1e-3), "unit": UNIT,
-                            "step_roofline_frac": (oc["B"] / (ms2 * 1e-3)) * hot_path_flops_per_pair(oc) / 1e12 / load_peaks()["bf16_sustained"],
+                            "step_roofline_frac": (oc["B"] / (ms2 * 1e-3)) * hot_path_flops_per_pair(oc) / 1e12 / load_peaks()["bf16"],
                             "steps": k2}
             del m2, s2, res2, pf2
             torch.cuda.empty_cache()
@@ -384,13 +385,6 @@ def run_ours(args):
     F = hot_path_flops_per_pair(c)
     step_tf = (value / world) * F / 1e12
     kern_ms = {k: round(v["ms"] / args.steps, 3) for k, v in prof.items()}
-    traffic, traffic_src = None, None
-    for tname in ("r02b_traffic.json", "r02_traffic.json"):   # newest committed capture first
-        tj = os.path.join(os.path.dirname(os.path.abspath(__file__)), "profiles", tname)
-        if os.path.exists(tj) and args.config == "cfg2" and B == 256:  # the ncu capture is of this workload only
-            tr = json.load(open(tj))
-            traffic, traffic_src = tr["gemm_dram_bytes_per_launch_avg"], f"profiles/{tname} ({tr['source']})"
-            break
     line = {
         "metric": METRIC, "value": value, "unit": UNIT, "n_gpus": world, "steps": args.steps, "warmup": max(args.warmup, 3),
         "ms_per_step": ms_step, "higher_is_better": True, "scaling": "weak", "vs_baseline": None, "dtype": "bf16",
@@ -400,22 +394,19 @@ def run_ours(args):
                    "step": "zero_grad + forward (MLM+NSP heads) + backward" + (" + 1 NCCL all-reduce (flat fp32 grads)" if world > 1 else "")
                            + ("; + fused BertAdam step (--optimizer; NOT the BASELINE metric)" if had_opt
                               else "; optimizer excluded (BASELINE.md §2)"),
-                   "l2": "per-step working set (>12 GB of activations) is >> the 126 MB L2; no explicit flush needed"},
+                   "l2": "per-step working set (>12 GB of activations) is >> the 50 MB L2; no explicit flush needed"},
         "clocks": clk.summary(),
         "gpu_launches": int(launches),
-        "roofline": {"bound": "tensor", "kernel": "gemm_tcgen05_2cta_kernel (all 12 GEMMs/layer fwd+dgrad+wgrad, projection, MLM decoder)",
-                     "achieved": gemm_tf, "peak": peaks["bf16_sustained"], "unit": "TFLOP/s",
-                     "frac": gemm_tf / peaks["bf16_sustained"], "traffic": traffic,
-                     "traffic_note": ("NOT measured in this run: DRAM read+write bytes per GEMM launch from the committed ncu capture "
-                                      "(ncu --set full, mean over one layer's 12 GEMM launches), "
-                                      + traffic_src) if traffic else "no ncu capture for this workload",
+        "roofline": {"bound": "tensor", "kernel": "gemm_wgmma_kernel (all 12 GEMMs/layer fwd+dgrad+wgrad, projection, MLM decoder)",
+                     "achieved": gemm_tf, "peak": peaks["bf16"], "unit": "TFLOP/s",
+                     "frac": gemm_tf / peaks["bf16"],
                      "flops_per_launch": g["work"] / max(1, g["launches"]),
-                     "of": peaks["source"] + " bf16_tflops_sustained", "launches_per_step": g["launches"] / args.steps,
+                     "of": peaks["source"], "launches_per_step": g["launches"] / args.steps,
                      "kernel_ms_per_step": round(g["ms"] / args.steps, 3),
                      "measured": f"per-launch CUDA events over a second pass of the same {args.steps} steps "
                                  f"({ms_profiled:.2f} ms/step with the events enabled)"},
-        "step_roofline": {"flops_per_pair": F, "achieved": step_tf, "peak": peaks["bf16_sustained"], "unit": "TFLOP/s",
-                          "frac": step_tf / peaks["bf16_sustained"],
+        "step_roofline": {"flops_per_pair": F, "achieved": step_tf, "peak": peaks["bf16"], "unit": "TFLOP/s",
+                          "frac": step_tf / peaks["bf16"],
                           "note": "hot-path algorithmic FLOPs (SURVEY.md §8d, heads and recompute not credited) over the whole step"},
         "kernel_ms_per_step": kern_ms,
         "e2e": {"value": e2e_value, "unit": UNIT, "ms_per_step": ms_e2e, "h2d_bytes_per_step": int(h2d_bytes),
@@ -436,10 +427,43 @@ def run_ours(args):
     return 0
 
 
+def dump_outputs(path, out, flat_grads, max_elems=1 << 21):
+    """What the last timed step handed its caller, as DIR/<name>.npy (float32; scalars and indices float64): every tensor of
+    the output dict and the gradients of all parameters (the flat buffer of FlatGradSync). Tensors above `max_elems`
+    elements are written as a fixed seeded sample of rows (logits) or elements (gradients), together with the indices of
+    the sample, so that two builds of the project compare entry for entry (about 32 MB in all)."""
+    import numpy as np
+    os.makedirs(path, exist_ok=True)
+    gen = torch.Generator().manual_seed(0)
+    arrays = {}
+    for k in sorted(out.keys()):
+        with torch.no_grad():
+            v = out[k]   # lazily computed entries (the MLM logits) are materialised here, outside the timed steps
+        if not torch.is_tensor(v):
+            continue
+        v = v.detach()
+        if v.numel() == 1:
+            arrays[k] = np.float64(v.double().item())
+            continue
+        if v.numel() > max_elems:   # [..., C]: a seeded sample of whole rows
+            rows = v.reshape(-1, v.shape[-1])
+            n = max(1, max_elems // rows.shape[1])
+            idx = torch.randperm(rows.shape[0], generator=gen)[:n].sort().values
+            arrays[k + "_sample_rows"] = idx.numpy().astype(np.float64)
+            v = rows[idx.to(rows.device)]
+        arrays[k] = v.float().cpu().numpy()
+    idx = torch.randperm(flat_grads.numel(), generator=gen)[:min(flat_grads.numel(), max_elems)].sort().values
+    arrays["grads_sample_index"] = idx.numpy().astype(np.float64)
+    arrays["grads_sample"] = flat_grads[idx.to(flat_grads.device)].float().cpu().numpy()
+    arrays["grads_norm"] = np.float64(flat_grads.double().norm().item())
+    for k, a in arrays.items():
+        np.save(os.path.join(path, k + ".npy"), a)
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
-    ap.add_argument("--steps", type=int, default=10)
+    ap.add_argument("--steps", type=int, default=10, help="timed steps (at least 1)")
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--impl", default="ours", choices=["ours", "reference"])
     ap.add_argument("--config", default="cfg2", choices=sorted(synthetic.CONFIGS))
@@ -450,7 +474,11 @@ def main():
                     help="also time BASELINE.json configs[2..4] at their per-GPU batch (always on for N > 1)")
     ap.add_argument("--optimizer", action="store_true",
                     help="also run the fused BertAdam step every step (SURVEY §8f rank 2; the BASELINE metric excludes it)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write what the last timed step computed (output dict, gradients) to DIR/<name>.npy")
     args = ap.parse_args()
+    if args.steps < 1:
+        ap.error("--steps must be at least 1")
     if args.impl == "reference":
         return run_reference(args)
     return run_ours(args)

@@ -1,5 +1,5 @@
 /*
- * vbert_b200.h — C ABI of libvbert_b200.so: the VisualBERT encoder hot path as sm_100a kernels.
+ * vbert_b200.h — C ABI of libvbert_b200.so: the VisualBERT encoder hot path as sm_90a (H100) kernels.
  *
  * Drop-in boundary (SURVEY.md §8b): every entry point takes plain device pointers, sizes and a
  * cudaStream_t (passed as void*); no torch types, no allocation of persistent state, re-entrant.
@@ -34,13 +34,13 @@ int64_t vb_launch_count(void);
  * vb_profile_read synchronises the device and returns, per category, the summed kernel time [ms], the
  * algorithmic work (FLOPs for the tensor-core kernels, bytes for the HBM-bound ones) and the number of launches
  * since the previous read; arrays of VB_PROFILE_CATEGORIES entries:
- * 0 gemm fwd, 1 gemm dgrad, 2 gemm wgrad (all gemm_tcgen05_kernel), 3 attention fwd, 4 attention dQ,
+ * 0 gemm fwd, 1 gemm dgrad, 2 gemm wgrad (all gemm_wgmma_kernel), 3 attention fwd, 4 attention dQ,
  * 5 attention dK/dV, 6 layernorm fwd, 7 layernorm bwd, 8 column sums, 9 embedding, 10 other. */
 #define VB_PROFILE_CATEGORIES 11
 void vb_profile_enable(int on);
 int vb_profile_read(double* ms, double* work, int64_t* launches);
 
-/* ---- GEMM core (tcgen05.mma + TMA + TMEM) ------------------------------------------------ */
+/* ---- GEMM core (wgmma + TMA + mbarrier) --------------------------------------------------- */
 /* epilogue selectors */
 #define VB_EPI_NONE 0
 #define VB_EPI_GELU 1  /* u = acc + bias: aux_out = gelu(u), D = gelu'(u)   — M.py:56-61, 302-305 */
@@ -213,7 +213,7 @@ int vb_layer_bwd(const vb_layer_desc* d, const void* x_in, const vb_layer_acts* 
  * layer slot (order: qkv, ctx, lse, pre1, mean1, rstd1, x1, u, g, pre2, mean2, rstd2, keep_mask, y) and returns the
  * slot stride; layer l's buffer i sits at arena + l * stride + offsets[i]; total size = n_layers * stride. The same
  * arena pointer is handed to forward and backward (PyTorch owns it; the library allocates nothing). One call replaces
- * the Python loop of M.py:365-368 and its per-layer allocations: host time per step drops from ~5 ms to ~0.2 ms, and the
+ * the Python loop of M.py:365-368 and its per-layer allocations: host time per step drops to a few calls, and the
  * recurring pointers make the library's tensor-map cache hit.
  * descs[l].seed / dropouts / layer_index are honoured per layer; descs is a HOST array. */
 #define VB_ENCODER_ARENA_BUFFERS 14

@@ -1,7 +1,7 @@
 """Generate tests/golden/*.npz from the UNMODIFIED reference (uclanlp/visualbert) — TEST INFRASTRUCTURE.
 
-Runs only in the build container, where the reference is mounted read-only at /root/reference:
-    python oracle/make_golden.py
+Needs a checkout of the reference (read only); VB_REFERENCE names its directory:
+    VB_REFERENCE=/path/to/visualbert-checkout python oracle/make_golden.py
 Imports visualbert/pytorch_pretrained_bert/modeling.py with the two shims of SURVEY.md §8c
 (stub boto3/botocore; Tensor.cuda -> identity on CPU), loads seeded weights
 (visualbert_b200.synthetic.init_state_dict) into the reference's TrainVisualBERTObjective, runs
@@ -19,7 +19,7 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 from visualbert_b200 import synthetic  # noqa: E402
 
-REF = "/root/reference/visualbert"
+REF = os.path.join(os.environ.get("VB_REFERENCE", "."), "visualbert")
 
 CASES = {
     # BASELINE.json configs[0]: VisualBERT-base 2-layer, batch 4, 36 regions (2048-d) + 20 tokens

@@ -7,8 +7,8 @@ import this module, and only as the checker. The product path (visualbert_b200) 
 
 Parity pinning: the reference repo holds NO tests, golden vectors or known-answer fixtures for this
 path (SURVEY.md §4, §8c), so the oracle is pinned against outputs of the reference itself, generated
-in the build container by oracle/make_golden.py (which imports the unmodified reference from
-/root/reference) and committed under tests/golden/. tests/test_oracle_golden.py checks this module
+by oracle/make_golden.py (which imports the unmodified reference from a checkout named by
+VB_REFERENCE) and committed under tests/golden/. tests/test_oracle_golden.py checks this module
 against those fixtures on every CPU test run.
 
 State is a dict name -> tensor using the reference's state_dict keys (SURVEY.md §8b), e.g.

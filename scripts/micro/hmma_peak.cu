@@ -1,5 +1,5 @@
 // Microbenchmark: peak throughput of warp-level mma.sync.m16n8k16 (bf16 -> fp32) on this GPU, as a function of
-// resident warps per SM and independent accumulators per warp. Build: nvcc -gencode arch=compute_100a,code=sm_100a -O3
+// resident warps per SM and independent accumulators per warp. Build: nvcc -gencode arch=compute_90a,code=sm_90a -O3
 #include <cstdio>
 #include <cuda_runtime.h>
 template <int ACC>

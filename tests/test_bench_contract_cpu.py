@@ -1,5 +1,5 @@
 """bench.py contract checks that need no GPU: the reference arm (`--impl reference`, the oracle port timed on host
-cores) prints ONE JSON line with the keys the driver reads; per-GPU batch of the configs BASELINE.json quotes as 8-GPU
+cores) prints ONE JSON line with the result keys; per-GPU batch of the configs BASELINE.json quotes as 8-GPU
 global batches."""
 import json
 import os

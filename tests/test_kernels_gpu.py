@@ -149,13 +149,11 @@ def test_gemm_dropout_statistics_and_determinism():
     assert abs(D1.float().mean().item() - D0.float().mean().item()) < 0.02 * D0.float().abs().mean().item()
 
 
-@pytest.mark.parametrize("env", [{"VB_GEMM_TMA_STORE": "0"}, {"VB_GEMM_TMA_STORE": "1"}, {"VB_GEMM_QUAD": "1"},
-                                 {"VB_GEMM_QUAD": "1", "VB_GEMM_TMA_STORE": "0"}, {"VB_GEMM_QUAD": "2"}, {"VB_GEMM_GP_TILED": "0"},
-                                 {"VB_GEMM_2CTA": "0"}])
+@pytest.mark.parametrize("env", [{"VB_GEMM_GP_TILED": "0"}, {"VB_GEMM_TILE_ORDER": "0"}, {"VB_PDL": "0"}])
 def test_gemm_kernel_variants(env):
-    """The GEMM picks its kernel per launch (CTA-pair / quad cluster with multicast B / single CTA; epilogue storing from
-    registers or through staged TMA stores). Each family must pass the same checks: the variants are forced through the
-    library's environment switches, read once per process, so the GEMM tests rerun in a subprocess."""
+    """The GEMM picks per launch the layout of gelu'(u) (row-major or tile-native) and the order of its tiles, and its
+    kernels are launched with or without programmatic dependent launch. Each choice must pass the same checks: they are
+    forced through the library's environment switches, read once per process, so the GEMM tests rerun in a subprocess."""
     import os, subprocess, sys
     root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
     r = subprocess.run([sys.executable, "-m", "pytest", os.path.join(root, "tests", "test_kernels_gpu.py"), "-m", "gpu", "-q",
@@ -285,15 +283,15 @@ def test_attention_dropout_consistent_between_fwd_and_bwd():
     assert abs(ctx.float().mean().item() - ref.mean().item()) < 5e-3
 
 
-@pytest.mark.parametrize("impl", ["head", "staged"])
+@pytest.mark.parametrize("impl", ["head", "staged", "head_recompute"])
 def test_attention_alternative_implementations(impl):
-    """The whole-head mma.sync kernels and the generic staged kernels must agree with the default tcgen05 kernels
-    (selected per process through VB_ATTN_FWD_IMPL / VB_ATTN_STAGED, so each runs in a subprocess)."""
+    """The whole-head mma.sync kernels (the fallback of the default wgmma kernels; `head_recompute`: their backward variant
+    that recomputes P instead of keeping it in shared memory) and the generic staged kernels must pass the same checks.
+    They are forced per process through the library's environment switches, so each runs in a subprocess."""
     import os, subprocess, sys
     env = dict(os.environ)
-    env["VB_ATTN_FWD_IMPL"] = impl
-    if impl == "staged":
-        env["VB_ATTN_STAGED"] = "1"
+    env.update({"head": {"VB_ATTN_HEAD": "1"}, "staged": {"VB_ATTN_STAGED": "1"},
+                "head_recompute": {"VB_ATTN_HEAD": "1", "VB_ATTN_BWD_PS": "0"}}[impl])
     root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
     r = subprocess.run([sys.executable, "-m", "pytest", os.path.join(root, "tests", "test_kernels_gpu.py"), "-m", "gpu", "-q",
                         "-k", "attention_fwd_bwd or attention_dropout or attention_fully"], env=env, capture_output=True, text=True,

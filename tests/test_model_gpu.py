@@ -1,4 +1,4 @@
-"""End-to-end parity of the CUDA path (visualbert_b200.TrainVisualBERTObjective -> C ABI -> sm_100a kernels) against
+"""End-to-end parity of the CUDA path (visualbert_b200.TrainVisualBERTObjective -> C ABI -> sm_90a kernels) against
 (a) the committed reference outputs in tests/golden/ (generated from the unmodified reference, fp32 CPU) and
 (b) the oracle (oracle/vb_oracle.py) run in fp32 on the same seeded weights and batches.
 
@@ -329,8 +329,8 @@ def test_data_updating_optimizer_is_seen_by_the_compute_weights():
 def test_full_depth_base_model_parity_at_benchmark_shape():
     """VERDICT r1 item 6a: the goldens stop at 3 layers — the 12-layer, H=768, S=164 stack of the headline number is
     compared here with the fp32 oracle on the device (B=16, ragged masks): loss, last hidden state, pooled output and
-    gradients of tensors at the bottom, middle and top of the stack. Measured on B200 (bf16 compute, 12 layers): loss 4e-6
-    relative, last hidden 1.7e-2 of max, pooled 2.3e-2, worst gradient relative error 1.6e-2; the bounds are ~2x that."""
+    gradients of tensors at the bottom, middle and top of the stack (bf16 compute, 12 layers); the bounds are about twice
+    the errors of the bf16 arithmetic."""
     from visualbert_b200 import BertConfig, TrainVisualBERTObjective, synthetic
     dev = torch.device("cuda:0")
     cfg = synthetic.bert_config_dict(12, 768, 12, 3072, vocab=8192)

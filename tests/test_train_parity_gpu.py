@@ -5,7 +5,7 @@ The library's dropout is a pure function of (seed, stream, element index) — `d
 csrc/vb_common.cuh — and the attention-probability bits are written to the keep-mask buffer by the forward. This test
 regenerates the hidden-state masks with a torch restatement of that hash, reads the attention bits back, runs the
 reference math with those masks and compares the layer output, the input gradient and every parameter gradient.
-It covers what eval-mode parity cannot: the forward/backward mask agreement of the tcgen05 attention kernels, the
+It covers what eval-mode parity cannot: the forward/backward mask agreement of the attention kernels, the
 GEMM-epilogue dropout, and the mask REGENERATION in the LayerNorm backward (dx_drop).
 """
 import ctypes

@@ -7,7 +7,7 @@ import ctypes
 import os
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
-# VB_LIB_PATH: load another build of the same library (A/B timing of kernel variants on one GPU box, scripts/build_variant.sh)
+# VB_LIB_PATH: load another build of the same library (A/B timing of kernel variants on one GPU, scripts/build_variant.sh)
 LIB_PATH = os.environ.get("VB_LIB_PATH") or os.path.join(_HERE, "lib", "libvbert_b200.so")
 
 ABI_VERSION = 2   # == VB_ABI_VERSION of include/vbert_b200.h (tests/test_abi.py keeps the two in step)

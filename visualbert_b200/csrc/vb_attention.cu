@@ -13,8 +13,8 @@
 // Backward recomputes P from the saved log-sum-exp: kernel A (per query block) produces dQ and the
 // row term D = rowsum(dO * O); kernel B (per key block) produces dK and dV. No atomics, deterministic.
 //
-// Tensor-core path here is warp-level mma.sync (m16n8k16, bf16 -> fp32); the tcgen05 budget of the
-// layer is spent in vb_gemm.cu where > 96 % of the FLOPs are.
+// Tensor-core path here is warp-level mma.sync (m16n8k16, bf16 -> fp32); the wgmma kernel of the
+// layer is in vb_gemm.cu, where > 96 % of the FLOPs are.
 #include "vb_attention.cuh"
 
 namespace vb {
@@ -434,6 +434,17 @@ static bool staged_only() {
     return v == 1;
 }
 
+// VB_ATTN_HEAD=1 forces the whole-head mma.sync kernels where the wgmma kernels would run (testing / tuning)
+static bool head_only() {
+    static int v = -1;
+    if (v < 0) { const char* e = getenv("VB_ATTN_HEAD"); v = (e != nullptr && atoi(e) != 0) ? 1 : 0; }
+    return v == 1;
+}
+// The wgmma kernels serve seq <= 192 (every reference config), the whole-head mma.sync kernels seq <= 256, the staged kernels
+// any length. Both fused paths take pre-drawn dropout bits and a pre-computed D = rowsum(dO * O).
+static bool head_path(int S) { return !staged_only() && (S + kBlk - 1) / kBlk <= kMaxSub; }
+static bool wgmma_path(const AttnParams& p) { return head_path(p.S) && !head_only() && attn_wgmma_supported(p); }
+
 static int fill_params(AttnParams& p, const void* qkv, const float* mask_bias, void* ctx, float* lse,
                        const void* dctx, void* dqkv, float* drow, void* keep, int B, int S, int A, int H,
                        float dropout_p, unsigned long long seed, unsigned stream_id) {
@@ -470,22 +481,19 @@ long long attn_keep_bytes(int B, int S, int A) {
 }
 
 // Draws the attention-dropout keep bits of a layer on the library's SIDE stream, so that the ALU-only mask kernel (no memory
-// traffic, 32 registers, no shared memory) shares the SMs with the QKV projection GEMM instead of running alone for 35 us:
+// traffic, 32 registers, no shared memory) shares the SMs with the QKV projection GEMM instead of running alone:
 // call it right after enqueuing that GEMM with an event recorded on `main` BEFORE the GEMM (the bits depend on (seed, stream)
 // only). Returns 1 when the bits are on their way (`main` already waits for them: pass mask_ready = true to attn_fwd), 0 when
 // the caller's attn_fwd will draw them itself (no dropout, another attention implementation, not opted in), < 0 on error.
-// OPT-IN (VB_MASK_OVERLAP=1): measured r02 on one box, 2 x 2 bench runs: 28.59 / 28.57 ms without, 28.87 / 28.56 ms with — the GEMM
-// slows down by what the mask kernel saves (its epilogue warps share the schedulers), so the default stays the plain sequence.
+// OPT-IN (VB_MASK_OVERLAP=1): the GEMM shares its SMs with the mask kernel, so whether it pays off depends on the GPU; the
+// default is the plain sequence.
 int attn_mask_async(void* keep, int B, int S, int A, int H, float dropout_p, unsigned long long seed, unsigned stream_id,
                     cudaEvent_t before_gemm, cudaStream_t main) {
     static const int off = [] { const char* e = getenv("VB_MASK_OVERLAP"); return (e != nullptr && atoi(e) == 1) ? 0 : 1; }();
     if (off || dropout_p <= 0.f || keep == nullptr) return 0;
-    const char* e = getenv("VB_ATTN_FWD_IMPL");
-    if ((e != nullptr && e[0] != 't') || staged_only()) return 0;
+    if (!head_path(S)) return 0;
     AttnParams p;
     if (fill_params(p, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, keep, B, S, A, H, dropout_p, seed, stream_id)) return -1;
-    p.qkv = reinterpret_cast<const bf16*>(keep);   // only the alignment of qkv is looked at below; the mask kernel never reads it
-    if (!attn_fwd_tc_supported(p)) return 0;
     static cudaStream_t side[kMaxDevices] = {nullptr};
     static cudaEvent_t done[kMaxDevices] = {nullptr};
     const int dev = current_device();
@@ -511,22 +519,8 @@ int attn_fwd(const void* qkv, const float* mask_bias, void* ctx, float* lse, voi
     int rc = fill_params(p, qkv, mask_bias, ctx, lse, nullptr, nullptr, nullptr, keep, B, S, A, H, dropout_p, seed, stream_id);
     if (rc) return rc;
     dim3 grid((S + kBlk - 1) / kBlk, A, B);
-    // implementation choice (VB_ATTN_FWD_IMPL = tc | head | staged): the tcgen05 / TMEM / TMA kernel is the default
-    // for seq <= 192 (every reference config), the persistent whole-head mma.sync kernel covers seq <= 256, the
-    // staged kernel any length.
-    static int impl = -1;
-    if (impl < 0) {
-        const char* e = getenv("VB_ATTN_FWD_IMPL");
-        impl = e == nullptr ? 0 : (e[0] == 't' ? 0 : (e[0] == 's' ? 2 : 1));
-    }
-    if (impl == 0 && !staged_only() && attn_fwd_tc_supported(p)) {
-        if (!mask_ready) {
-            rc = attn_keep_mask(p, static_cast<int>(grid.x), st);
-            if (rc) return rc;
-        }
-        return attn_fwd_tc(p, st);
-    }
-    if (impl <= 1 && static_cast<int>(grid.x) <= kMaxSub && !staged_only()) return attn_fwd_head(p, static_cast<int>(grid.x), st);
+    if (wgmma_path(p)) return attn_fwd_wgmma(p, st, mask_ready);
+    if (head_path(S)) return attn_fwd_head(p, static_cast<int>(grid.x), st, mask_ready);
     const int nsub = static_cast<int>(grid.x) < kMaxSub ? static_cast<int>(grid.x) : kMaxSub;
     const int smem = (1 + 2 * nsub) * kTileBytes;
     static int configured[kMaxDevices] = {0};
@@ -541,22 +535,8 @@ int attn_fwd(const void* qkv, const float* mask_bias, void* ctx, float* lse, voi
 
 static int g_bwd_minb = 3;
 
-static int bwd_impl() {   // VB_ATTN_BWD_IMPL = tc | head | staged
-    static int bimpl = -1;
-    if (bimpl < 0) {
-        const char* e = getenv("VB_ATTN_BWD_IMPL");
-        bimpl = e == nullptr ? 0 : (e[0] == 't' ? 0 : (e[0] == 's' ? 2 : 1));
-    }
-    return bimpl;
-}
-
 bool attn_bwd_takes_delta(const void* qkv, const void* dctx, void* dqkv, int B, int S, int A, int H) {
-    if (bwd_impl() != 0 || staged_only() || B <= 0 || S <= 0 || A <= 0 || H != A * kHd) return false;
-    AttnParams p;
-    memset(&p, 0, sizeof(p));
-    p.qkv = static_cast<const bf16*>(qkv); p.dctx = static_cast<const bf16*>(dctx); p.dqkv = static_cast<bf16*>(dqkv);
-    p.B = B; p.S = S; p.A = A; p.H = H;
-    return attn_bwd_tc_supported(p);
+    return B > 0 && S > 0 && A > 0 && H == A * kHd && head_path(S);
 }
 
 int attn_bwd(const void* qkv, const float* mask_bias, const void* ctx, const float* lse, const void* keep,
@@ -578,16 +558,8 @@ int attn_bwd(const void* qkv, const float* mask_bias, const void* ctx, const flo
         env_read = true;
     }
     dim3 grid((S + kBlk - 1) / kBlk, A, B);
-    // VB_ATTN_BWD_IMPL = tc | head | staged: tcgen05 kernel by default (seq <= 192), then the whole-head mma.sync kernel
-    const int bimpl = bwd_impl();
-    if (bimpl == 0 && !staged_only() && attn_bwd_tc_supported(p)) {
-        if (!delta_ready) {   // D = rowsum(dO * O) — unless the GEMM that produced dO already wrote it (vb_gemm_args.delta_out)
-            rc = attn_delta(p, st);
-            if (rc) return rc;
-        }
-        return attn_bwd_tc(p, st);
-    }
-    if (bimpl <= 1 && static_cast<int>(grid.x) <= kMaxSub && !staged_only()) return attn_bwd_head(p, static_cast<int>(grid.x), st);
+    if (wgmma_path(p)) return attn_bwd_wgmma(p, st, delta_ready);
+    if (head_path(S)) return attn_bwd_head(p, static_cast<int>(grid.x), st, delta_ready);
     const int nsub = static_cast<int>(grid.x) < kMaxSub ? static_cast<int>(grid.x) : kMaxSub;
     {   // algorithmic work of the backward = 2x forward (recompute not credited), split evenly over the two kernels
         ProfScope ps(st, PROF_ATTN_DQ, 4.0 * B * A * S * S * kHd, 1);

@@ -1,5 +1,6 @@
 // vb_attention.cuh — device helpers shared by the attention kernels (vb_attention.cu: staged kernels for any
-// sequence length; vb_attention_head.cu: persistent whole-head kernels for seq <= 256).
+// sequence length; vb_attention_head.cu: persistent whole-head mma.sync kernels for seq <= 256; vb_attention_wgmma.cu:
+// wgmma / TMA kernels for seq <= 192, the default).
 #pragma once
 #include <stdlib.h>
 
@@ -261,17 +262,17 @@ __device__ __forceinline__ void store_acc(bf16* base, long long ld, int row0, in
 
 constexpr int kMaxSub = 4;  // 64-row tiles per resident stage
 
-// whole-head persistent kernels (vb_attention_head.cu); nkb = ceil(S / 64) <= kMaxSub
-int attn_fwd_head(const AttnParams& p, int nkb, cudaStream_t st);
-int attn_bwd_head(const AttnParams& p, int nkb, cudaStream_t st);
+// whole-head persistent kernels (vb_attention_head.cu); nkb = ceil(S / 64) <= kMaxSub.
+// mask_ready: the keep bits were already drawn (attn_mask_async); delta_ready: p.drow already holds D = rowsum(dO * O)
+// (written by the epilogue of the GEMM that produced dO, vb_gemm_args.delta_out).
+int attn_fwd_head(const AttnParams& p, int nkb, cudaStream_t st, bool mask_ready);
+int attn_bwd_head(const AttnParams& p, int nkb, cudaStream_t st, bool delta_ready);
 int attn_keep_mask(const AttnParams& p, int nkb, cudaStream_t st);
 int attn_delta(const AttnParams& p, cudaStream_t st);
-// tcgen05 / TMEM / TMA backward (vb_attention_bwd_tc.cu), seq <= 192; needs p.drow = D (attn_delta)
-bool attn_bwd_tc_supported(const AttnParams& p);
-int attn_bwd_tc(const AttnParams& p, cudaStream_t st);
-// tcgen05 / TMEM / TMA forward (vb_attention_tc.cu), seq <= 192
-bool attn_fwd_tc_supported(const AttnParams& p);
-int attn_fwd_tc(const AttnParams& p, cudaStream_t st);
-int make_tmap_3d(CUtensorMap* m, const void* ptr, int S, int B, int ld, int box_rows);
+// wgmma / TMA / mbarrier kernels (vb_attention_wgmma.cu), seq <= 192: the default where supported
+bool attn_wgmma_supported(const AttnParams& p);
+int attn_fwd_wgmma(const AttnParams& p, cudaStream_t st, bool mask_ready);
+int attn_bwd_wgmma(const AttnParams& p, cudaStream_t st, bool delta_ready);
+int make_tmap_bf16(CUtensorMap* m, const void* ptr, uint64_t inner, uint64_t outer, uint64_t ld_elems, uint32_t box_outer);
 
 }  // namespace vb

@@ -1,8 +1,8 @@
-// vb_attention_head.cu — persistent whole-head attention kernels for seq <= 256 (every reference config).
+// vb_attention_head.cu — persistent whole-head mma.sync attention kernels for seq <= 256 (the fallback of the wgmma
+// kernels in vb_attention_wgmma.cu: 192 < seq <= 256, or VB_ATTN_HEAD=1).
 //
 // The staged kernels in vb_attention.cu launch one short-lived CTA per (batch, head, 64-query block): each
-// re-loads the head's K/V and spends most of its ~10 us life waiting for that load (measured: 23-30 % of the
-// mma.sync peak). Here one CTA owns a whole (batch, head): NW = ceil(S/16) warps, each with 16 query rows
+// re-loads the head's K/V and spends much of its short life waiting for that load. Here one CTA owns a whole (batch, head): NW = ceil(S/16) warps, each with 16 query rows
 // (and, in backward, 16 key rows); Q/K/V (and dO) tiles are loaded ONCE per head with cp.async, and the CTA is
 // persistent — it walks over heads and prefetches the next head's tiles into the second shared-memory buffer
 // while computing the current one, so the tensor pipe never waits for HBM/L2 latency.
@@ -30,11 +30,11 @@ __device__ __forceinline__ void load_rows(uint32_t tiles, const bf16* base, long
 
 // ------------------------------------------------------------------------------------------------
 // attention-probability dropout mask: one thread per 64-bit word (query row, 64-key block), 16 counter hashes -> 64 keep
-// decisions of 8 random bits each (keep iff value >= thresh8). Drawing the bits inside the attention kernels cost 65 us
-// per layer at the benchmark shape; this kernel has nothing else to do and runs at full issue rate (~20 us).
+// decisions of 8 random bits each (keep iff value >= thresh8). Drawing the bits inside the attention kernels made them
+// slower than this separate pass, which has nothing else to do and runs at full issue rate.
 // Two layouts are written: keep[(bh * np64 + q) * nkb + kb] (bit = key % 64; rows = queries: forward kernels, mma.sync
-// backward) and the transpose keepT[(bh * np64 + key) * nkb + qb] (bit = query % 64; rows = keys: the tcgen05 backward,
-// whose TMEM lanes are keys). A block is one 64 x 64 bit tile; the transpose is 64 warp ballots per 32 rows.
+// backward) and the transpose keepT[(bh * np64 + key) * nkb + qb] (bit = query % 64; rows = keys: for a backward
+// that walks keys). A block is one 64 x 64 bit tile; the transpose is 64 warp ballots per 32 rows.
 // ------------------------------------------------------------------------------------------------
 __global__ void __launch_bounds__(64)
 attn_keep_mask_kernel(unsigned long long* __restrict__ keep, unsigned long long* __restrict__ keepT, int nkb, int np64, int S,
@@ -656,9 +656,9 @@ int attn_keep_mask(const AttnParams& p, int nkb, cudaStream_t st) {
     return 0;
 }
 
-int attn_fwd_head(const AttnParams& p, int nkb, cudaStream_t st) {
+int attn_fwd_head(const AttnParams& p, int nkb, cudaStream_t st, bool mask_ready) {
     const int nw = (p.S + 15) / 16;
-    int rc = attn_keep_mask(p, nkb, st);
+    int rc = mask_ready ? 0 : attn_keep_mask(p, nkb, st);
     if (rc) return rc;
     if (nw <= 4) rc = launch_fwd<4>(p, nkb, st);
     else if (nw <= 8) rc = launch_fwd<8>(p, nkb, st);
@@ -701,7 +701,7 @@ static int bwd_ps_smem(const AttnParams& p, int nkb, int* colsP) {
         const char* e = getenv("VB_ATTN_BWD_PS");
         enabled = (e && e[0] == '0') ? 0 : 1;
     }
-    const int max_smem = 227 * 1024;  // sm_100a opt-in limit per block (the library targets this arch only)
+    const int max_smem = 227 * 1024;  // sm_90a opt-in limit per block (the library targets this arch only)
     if (!enabled) return 0;
     *colsP = (p.S + 15) / 16 * 16;
     const int smem = 4 * nkb * kTileBytes + 2 * 3 * nkb * kBlk * 4 + 2 * (*colsP) * ((*colsP) * 2 + 16);
@@ -717,8 +717,8 @@ int attn_delta(const AttnParams& p, cudaStream_t st) {
     return 0;
 }
 
-int attn_bwd_head(const AttnParams& p, int nkb, cudaStream_t st) {
-    {
+int attn_bwd_head(const AttnParams& p, int nkb, cudaStream_t st, bool delta_ready) {
+    if (!delta_ready) {
         int rc0 = attn_delta(p, st);
         if (rc0) return rc0;
     }

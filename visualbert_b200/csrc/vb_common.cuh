@@ -1,6 +1,6 @@
-// vb_common.cuh — sm_100a device primitives shared by every kernel in libvbert_b200.
+// vb_common.cuh — sm_90a device primitives shared by every kernel in libvbert_b200.
 //
-// Thin inline-PTX wrappers (mbarrier, TMA, tcgen05/TMEM) plus small math helpers.
+// Thin inline-PTX wrappers (mbarrier, TMA, wgmma) plus small math helpers.
 // No CUTLASS/CuTe dependency: the descriptors are built by hand (see vb_gemm.cu).
 #pragma once
 
@@ -38,7 +38,7 @@ enum { PROF_GEMM_FWD = 0, PROF_GEMM_DGRAD = 1, PROF_GEMM_WGRAD = 2, PROF_ATTN_FW
        PROF_LN_FWD = 6, PROF_LN_BWD = 7, PROF_COLSUM = 8, PROF_EMBED = 9, PROF_OTHER = 10, PROF_NCAT = 11 };
 // ---- programmatic dependent launch (PDL) -------------------------------------------------------------------
 // Hot-path kernels are launched with cudaLaunchAttributeProgrammaticStreamSerialization: the next kernel's CTAs may be
-// scheduled, and run their on-chip prologue (barrier init, TMEM allocation, tensor-map prefetch), while the previous
+// scheduled, and run their on-chip prologue (barrier init, tensor-map prefetch), while the previous
 // kernel's last CTAs drain. Every such kernel calls pdl_trigger() on entry and pdl_wait() BEFORE its first global
 // memory access (griddepcontrol.wait returns once the preceding grid has completed and its writes are visible).
 // VB_PDL=0 in the environment turns the attribute off (plain stream order).
@@ -58,26 +58,6 @@ inline cudaError_t launch_pdl(void (*kernel)(KArgs...), dim3 grid, dim3 block, s
     attr[0].val.programmaticStreamSerializationAllowed = 1;
     cfg.attrs = attr;
     cfg.numAttrs = pdl_enabled() ? 1 : 0;
-    return cudaLaunchKernelEx(&cfg, kernel, static_cast<KArgs>(args)...);
-}
-// same, for a kernel launched as clusters of `cluster` CTAs along x (cluster size chosen at launch, not at compile time)
-template <typename... KArgs, typename... Args>
-inline cudaError_t launch_pdl_cluster(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t st, int cluster,
-                                      Args&&... args) {
-    cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = grid;
-    cfg.blockDim = block;
-    cfg.dynamicSmemBytes = smem;
-    cfg.stream = st;
-    cudaLaunchAttribute attr[2];
-    attr[0].id = cudaLaunchAttributeClusterDimension;
-    attr[0].val.clusterDim.x = cluster;
-    attr[0].val.clusterDim.y = 1;
-    attr[0].val.clusterDim.z = 1;
-    attr[1].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    attr[1].val.programmaticStreamSerializationAllowed = 1;
-    cfg.attrs = attr;
-    cfg.numAttrs = pdl_enabled() ? 2 : 1;
     return cudaLaunchKernelEx(&cfg, kernel, static_cast<KArgs>(args)...);
 }
 #endif
@@ -269,22 +249,6 @@ __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
     }
 }
 
-// UMMA shared-memory descriptor split in two 32-bit halves: only the 14-bit start-address field (bits 0-13, in 16-byte
-// units) changes between the MMAs of a tile, so stepping through k is ONE 32-bit add on the low half — the MMA-issuing
-// thread is a single thread whose instruction latency is exposed, every instruction saved there shortens the pipeline.
-struct UmmaDesc {
-    uint32_t lo, hi;
-    __device__ __forceinline__ uint64_t at(uint32_t byte_off) const {
-        return (static_cast<uint64_t>(hi) << 32) | static_cast<uint64_t>(lo + (byte_off >> 4));
-    }
-};
-__device__ __forceinline__ UmmaDesc make_umma_desc_sw128(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
-    UmmaDesc d;
-    d.lo = ((saddr & 0x3FFFFu) >> 4) | (((lbo_bytes >> 4) & 0x3FFFu) << 16);
-    d.hi = ((sbo_bytes >> 4) & 0x3FFFu) | (1u << 14) | (2u << 29);   // version 1 (bit 46), SWIZZLE_128B (bits 61-63)
-    return d;
-}
-
 // ---------------------------------------------------------------------------------------------
 // TMA (cp.async.bulk.tensor) — 2-D tiled load, completion on an mbarrier
 // ---------------------------------------------------------------------------------------------
@@ -301,176 +265,79 @@ __device__ __forceinline__ void tma_load_2d(uint32_t smem_dst, const CUtensorMap
 }
 
 // ---------------------------------------------------------------------------------------------
-// tcgen05 / TMEM
+// wgmma (warpgroup MMA, sm_90a)
 // ---------------------------------------------------------------------------------------------
-__device__ __forceinline__ void tcgen05_fence_before() {
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
+// Shared-memory matrix descriptor, 128-byte swizzle: start address, leading / stride byte offsets (16-byte units).
+//  K-major  tile [rows][64]: 8-row groups are 1024 B apart (SBO); LBO unused.
+//  MN-major tile [atoms of 64 along MN][64 k-rows][64]: 8 k-rows = 1024 B (SBO), next 64-wide MN atom = 8192 B (LBO).
+__device__ __forceinline__ uint64_t wgmma_desc_sw128(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
+    return static_cast<uint64_t>((saddr & 0x3FFFFu) >> 4) | (static_cast<uint64_t>((lbo_bytes >> 4) & 0x3FFFu) << 16) |
+           (static_cast<uint64_t>((sbo_bytes >> 4) & 0x3FFFu) << 32) | (1ull << 62);
 }
-__device__ __forceinline__ void tcgen05_fence_after() {
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-}
-// whole warp; writes the TMEM base address (lane<<16 | column) to *smem_dst
-__device__ __forceinline__ void tmem_alloc(uint32_t smem_dst, uint32_t ncols) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_dst),
-                 "r"(ncols)
-                 : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols)
-                 : "memory");
-}
-// D[tmem] (+)= A[smem desc] * B[smem desc]; issued by ONE thread on behalf of the CTA.
-__device__ __forceinline__ void umma_bf16(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc,
-                                          uint32_t idesc, uint32_t accumulate) {
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// D[64 x 128] (+)= A[64 x 16] * B[16 x 128], bf16 in, fp32 accumulators in registers of the warpgroup.
+// TA / TB = 1: the operand is MN-major in shared memory (transposed read), 0: K-major.
+// Fragment of thread t (warp w = t / 32, lane l): d[4 j + 2 i + c] = D[16 w + l / 4 + 8 i][8 j + 2 (l % 4) + c].
+template <int TA, int TB>
+__device__ __forceinline__ void wgmma_m64n128k16(float (&d)[64], uint64_t a_desc, uint64_t b_desc, uint32_t accumulate) {
     asm volatile(
         "{\n"
         ".reg .pred p;\n"
-        "setp.ne.b32 p, %4, 0;\n"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n"
-        "}\n" ::"r"(d_tmem),
-        "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate)
-        : "memory");
+        "setp.ne.b32 p, %66, 0;\n"
+        "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, "
+        "%64, %65, p, 1, 1, %67, %68;\n"
+        "}\n"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+          "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+          "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+          "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
+          "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
+          "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
+          "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
+          "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+        : "l"(a_desc), "l"(b_desc), "r"(accumulate), "n"(TA), "n"(TB));
 }
-// mbarrier arrives when all previously issued tcgen05.mma of this thread have completed
-// (implies tcgen05.fence::before_thread_sync).
-__device__ __forceinline__ void umma_commit(uint32_t bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar)
-                 : "memory");
-}
-// ---- cta_group::2 (CTA pair) variants -------------------------------------------------------------
-__device__ __forceinline__ uint32_t cluster_ctarank() {
-    uint32_t r;
-    asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-    return r;
-}
-__device__ __forceinline__ void cluster_sync_all() {
-    asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory");
-    asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-// arrive on the mbarrier at the same shared-memory offset in CTA `cta` of the cluster
-__device__ __forceinline__ void mbar_arrive_remote(uint32_t bar, uint32_t cta) {
-    asm volatile(
-        "{\n"
-        ".reg .b32 ra;\n"
-        "mapa.shared::cluster.u32 ra, %0, %1;\n"
-        "mbarrier.arrive.shared::cluster.b64 _, [ra];\n"
-        "}\n" ::"r"(bar), "r"(cta)
-        : "memory");
-}
-__device__ __forceinline__ void tmem_alloc_2cta(uint32_t smem_dst, uint32_t ncols) {
-    asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_dst), "r"(ncols) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc_2cta(uint32_t taddr, uint32_t ncols) {
-    asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-// TMA load issued by either CTA of the pair; the transaction bytes are credited to the LEADER CTA's mbarrier
-// (peer bit of the barrier address cleared, as CUTLASS' SM100_TMA_2SM_LOAD does)
-__device__ __forceinline__ void tma_load_2d_2cta(uint32_t smem_dst, const CUtensorMap* m, uint32_t bar, int c_inner, int c_outer) {
-    asm volatile(
-        "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes"
-        " [%0], [%1, {%3, %4}], [%2];"
-        ::"r"(smem_dst), "l"(reinterpret_cast<uint64_t>(m)), "r"(bar & 0xFEFFFFFFu), "r"(c_inner), "r"(c_outer)
-        : "memory");
-}
-// D[tmem of both CTAs] (+)= A * B with M = 256 split over the CTA pair; issued by ONE thread of the leader CTA
-__device__ __forceinline__ void umma_bf16_2cta(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc, uint32_t accumulate) {
+// D[64 x 64] (+)= A[64 x 16] * B[16 x 64], both operands from shared-memory descriptors (fragment of D as above).
+template <int TA, int TB>
+__device__ __forceinline__ void wgmma_m64n64k16_ss(float (&d)[32], uint64_t a_desc, uint64_t b_desc, uint32_t accumulate) {
     asm volatile(
         "{\n"
         ".reg .pred p;\n"
-        "setp.ne.b32 p, %4, 0;\n"
-        "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n"
-        "}\n" ::"r"(d_tmem), "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate)
-        : "memory");
+        "setp.ne.b32 p, %34, 0;\n"
+        "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, "
+        "%32, %33, p, 1, 1, %35, %36;\n"
+        "}\n"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+          "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+          "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+          "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+        : "l"(a_desc), "l"(b_desc), "r"(accumulate), "n"(TA), "n"(TB));
 }
-// commit: when the MMAs issued so far retire, arrive on the mbarrier at this offset in every CTA of `cta_mask`
-// (bit i = CTA rank i of the cluster; 3 = both CTAs of the first pair)
-__device__ __forceinline__ void umma_commit_2cta(uint32_t bar, uint32_t cta_mask = 3u) {
-    asm volatile("tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(bar),
-                 "h"(static_cast<uint16_t>(cta_mask))
-                 : "memory");
-}
-// TMA store of one box from (swizzled) shared memory; completion is tracked per thread in bulk async-groups
-__device__ __forceinline__ void tma_store_2d(const CUtensorMap* m, uint32_t smem_src, int c_inner, int c_outer) {
-    asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%2, %3}], [%1];"
-                 ::"l"(reinterpret_cast<uint64_t>(m)), "r"(smem_src), "r"(c_inner), "r"(c_outer)
-                 : "memory");
-}
-__device__ __forceinline__ void bulk_commit_group() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
-// the issuing thread's bulk groups have finished READING shared memory (the source may be overwritten)
-__device__ __forceinline__ void bulk_wait_group_read0() { asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory"); }
-__device__ __forceinline__ void bulk_wait_group0() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
-__device__ __forceinline__ void sts_v4(uint32_t saddr, uint32_t a, uint32_t b, uint32_t c, uint32_t d) {
-    asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(saddr), "r"(a), "r"(b), "r"(c), "r"(d) : "memory");
-}
-// TMA load multicast to the CTAs of `cta_mask`: the box lands at the same CTA-relative offset in each of them and the
-// bytes are credited to the barrier at this offset in the LEADER of each destination CTA's pair (peer bit cleared)
-__device__ __forceinline__ void tma_load_2d_2cta_mc(uint32_t smem_dst, const CUtensorMap* m, uint32_t bar, int c_inner, int c_outer,
-                                                    uint32_t cta_mask) {
-    asm volatile(
-        "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster"
-        " [%0], [%1, {%3, %4}], [%2], %5;"
-        ::"r"(smem_dst), "l"(reinterpret_cast<uint64_t>(m)), "r"(bar & 0xFEFFFFFFu), "r"(c_inner), "r"(c_outer),
-          "h"(static_cast<uint16_t>(cta_mask))
-        : "memory");
-}
-
-// 32 lanes x 32 columns of 32-bit: thread i of the warp receives row (lane base + i), 32 columns.
-__device__ __forceinline__ void tmem_ld_32x32b_x32(uint32_t taddr, uint32_t (&v)[32]) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-        : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]),
-          "=r"(v[7]), "=r"(v[8]), "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]),
-          "=r"(v[14]), "=r"(v[15]), "=r"(v[16]), "=r"(v[17]), "=r"(v[18]), "=r"(v[19]), "=r"(v[20]),
-          "=r"(v[21]), "=r"(v[22]), "=r"(v[23]), "=r"(v[24]), "=r"(v[25]), "=r"(v[26]), "=r"(v[27]),
-          "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-        : "r"(taddr)
-        : "memory");
-}
-__device__ __forceinline__ void tmem_ld_32x32b_x8(uint32_t taddr, uint32_t (&v)[8]) {
-    asm volatile("tcgen05.ld.sync.aligned.32x32b.x8.b32 {%0, %1, %2, %3, %4, %5, %6, %7}, [%8];"
-                 : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7])
-                 : "r"(taddr)
-                 : "memory");
-}
-__device__ __forceinline__ void tmem_ld_32x32b_x16(uint32_t taddr, uint32_t (&v)[16]) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-        : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]),
-          "=r"(v[8]), "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15])
-        : "r"(taddr)
-        : "memory");
-}
-// A operand from TMEM (TS form): D[tmem] (+)= A[tmem, K-major: lane = row, 2 bf16 per 32-bit column] * B[smem desc]
-__device__ __forceinline__ void umma_bf16_ts(uint32_t d_tmem, uint32_t a_tmem, uint64_t b_desc, uint32_t idesc, uint32_t accumulate) {
+// same with A from registers: a[0..3] of thread (warp w, lane l) hold the bf16 pairs (16 w + l/4, 2 (l%4)), (+8 rows, same cols),
+// (same row, +8 cols), (+8 rows, +8 cols) — the accumulator layout of a 64 x 16 slice, so a result feeds the next MMA directly.
+template <int TB>
+__device__ __forceinline__ void wgmma_m64n64k16_rs(float (&d)[32], const uint32_t (&a)[4], uint64_t b_desc, uint32_t accumulate) {
     asm volatile(
         "{\n"
         ".reg .pred p;\n"
-        "setp.ne.b32 p, %4, 0;\n"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %2, %3, p;\n"
-        "}\n" ::"r"(d_tmem), "r"(a_tmem), "l"(b_desc), "r"(idesc), "r"(accumulate)
-        : "memory");
+        "setp.ne.b32 p, %37, 0;\n"
+        "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, "
+        "{%32, %33, %34, %35}, %36, p, 1, 1, %38;\n"
+        "}\n"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+          "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+          "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+          "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+        : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(b_desc), "r"(accumulate), "n"(TB));
 }
-// 32 lanes x 8 columns of 32-bit: thread i of the warp writes row (lane base + i), 8 consecutive columns
-__device__ __forceinline__ void tmem_st_32x32b_x8(uint32_t taddr, const uint32_t (&v)[8]) {
-    asm volatile("tcgen05.st.sync.aligned.32x32b.x8.b32 [%0], {%1, %2, %3, %4, %5, %6, %7, %8};" ::"r"(taddr), "r"(v[0]), "r"(v[1]),
-                 "r"(v[2]), "r"(v[3]), "r"(v[4]), "r"(v[5]), "r"(v[6]), "r"(v[7])
-                 : "memory");
-}
-__device__ __forceinline__ void tmem_st_32x32b_x4(uint32_t taddr, uint32_t a, uint32_t b, uint32_t c, uint32_t d) {
-    asm volatile("tcgen05.st.sync.aligned.32x32b.x4.b32 [%0], {%1, %2, %3, %4};" ::"r"(taddr), "r"(a), "r"(b), "r"(c), "r"(d) : "memory");
-}
-__device__ __forceinline__ void tmem_st_wait() {
-    asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory");
-}
-// One lane of a CONVERGED warp (elect.sync). The MMA-issuing role runs its loop with all 32 lanes converged and predicates
-// only the tcgen05 instructions on this: the compiler then keeps descriptors and loop state in uniform registers. Guarding
-// the whole role with `if (lane == 0)` instead makes the code divergent, and every tcgen05.mma gets wrapped in an
-// ELECT / BRA.U.ANY serialisation loop (~100+ cycles of issue latency per MMA — measured in the attention kernels).
+// One lane of a CONVERGED warp (elect.sync): the producer loop runs with all 32 lanes converged and only the issue is
+// predicated, so loop state stays in uniform registers.
 __device__ __forceinline__ bool elect_one() {
     uint32_t pred;
     asm volatile(
@@ -482,17 +349,14 @@ __device__ __forceinline__ bool elect_one() {
         : "=r"(pred));
     return pred != 0;
 }
-// Register re-distribution between warp roles (whole warpgroups of 4 warps): the control warpgroup shrinks its
-// allocation, the element-wise warpgroups grow theirs; ptxas compiles the code that follows against the new limit.
+// Register re-distribution between warp roles (whole warpgroups of 4 warps): the producer warpgroup shrinks its
+// allocation, the MMA warpgroups grow theirs; ptxas compiles the code that follows against the new limit.
 template <int N>
 __device__ __forceinline__ void reg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N)); }
 template <int N>
 __device__ __forceinline__ void reg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(N)); }
 __device__ __forceinline__ void named_bar_sync(int id, int nthreads) {
     asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() {
-    asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -502,16 +366,14 @@ __device__ __forceinline__ uint4 ldg_v4(const void* p) {
     return __ldg(reinterpret_cast<const uint4*>(p));
 }
 __device__ __forceinline__ void stg_v4(void* p, uint4 v) { *reinterpret_cast<uint4*>(p) = v; }
-// 256-bit global access (sm_100): one full 32-byte sector per thread per instruction
+// 32 bytes per thread as two 128-bit accesses (one full 32-byte sector)
 __device__ __forceinline__ void ldg_v8(const void* p, uint32_t (&r)[8]) {
-    asm volatile("ld.global.nc.v8.b32 {%0, %1, %2, %3, %4, %5, %6, %7}, [%8];"
-                 : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7])
-                 : "l"(p));
+    const uint4 a = ldg_v4(p), b = ldg_v4(static_cast<const uint8_t*>(p) + 16);
+    r[0] = a.x; r[1] = a.y; r[2] = a.z; r[3] = a.w; r[4] = b.x; r[5] = b.y; r[6] = b.z; r[7] = b.w;
 }
 __device__ __forceinline__ void stg_v8(void* p, const uint32_t (&r)[8]) {
-    asm volatile("st.global.v8.b32 [%0], {%1, %2, %3, %4, %5, %6, %7, %8};" ::"l"(p), "r"(r[0]), "r"(r[1]),
-                 "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7])
-                 : "memory");
+    stg_v4(p, make_uint4(r[0], r[1], r[2], r[3]));
+    stg_v4(static_cast<uint8_t*>(p) + 16, make_uint4(r[4], r[5], r[6], r[7]));
 }
 __device__ __forceinline__ void red_add_v4_f32(float* p, float a, float b, float c, float d) {
     asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(p), "f"(a), "f"(b), "f"(c),

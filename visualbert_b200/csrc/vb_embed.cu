@@ -113,7 +113,7 @@ embed_fwd_kernel(const EmbedParams p) {
 // Adjoint of the gather / concat: word rows are scattered with vector reductions; the position, token-type and visual
 // position / type gradients — a few rows that EVERY example adds into — are first summed in registers over a chunk of
 // examples at a fixed sequence position (a warp task = (position s, 32 examples)), so each table row receives one vector
-// reduction per task instead of one scalar atomic per element (round 1: 0.28 ms, almost all of it atomic contention).
+// reduction per task instead of one scalar atomic per element (which made atomic contention the bulk of the kernel's time).
 // smem: [n_types][H] text types, [n_types][H] visual types, [H] visual position row 0 (block accumulators, flushed once)
 template <int NC>
 __global__ void __launch_bounds__(kEmbWarps * 32)

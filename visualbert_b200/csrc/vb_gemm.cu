@@ -1,13 +1,13 @@
-// vb_gemm.cu — the dense-contraction core of the VisualBERT encoder hot path on sm_100a.
+// vb_gemm.cu — the dense-contraction core of the VisualBERT encoder hot path on sm_90a.
 //
-// One persistent, warp-specialised kernel computes D[M,N] = epi(sum_k A(m,k) B(n,k)) in bf16 with
-// fp32 accumulation:
-//   warp 0     TMA producer  (cp.async.bulk.tensor, 128B-swizzled 64-wide tiles, 4-stage mbarrier ring)
-//   warp 1     MMA issuer    (one elected thread issues tcgen05.mma 128xBNx16, accumulators in TMEM,
-//                             two accumulator stages so the epilogue of tile i overlaps tile i+1)
-//   warp 2     TMEM allocator
-//   warps 4-11 epilogue      (pipelined tcgen05.ld -> bias / dropout / residual / GELU / GELU' -> 32-byte stores,
-//                             or fp32 red.add for split-K weight gradients)
+// One warp-specialised kernel computes D[M,N] = epi(sum_k A(m,k) B(n,k)) in bf16 with fp32 accumulation,
+// one 128 x BLOCK_N tile per CTA (BLOCK_N = 256, or 128 for narrow / ragged N):
+//   warpgroup 0     TMA producer  (one elected thread: cp.async.bulk.tensor, 128B-swizzled 64-wide k-slabs,
+//                                  4-stage mbarrier ring)
+//   warpgroups 1-2  MMA + epilogue (wgmma.mma_async 64 x 128 x 16 from shared-memory descriptors, fp32 accumulators in
+//                                  registers, 64 rows per warpgroup; then the tile goes through shared memory so that a
+//                                  thread owns 16-column pieces of one row for bias / dropout / residual / GELU / GELU'
+//                                  and 32-byte stores, or fp32 red.add for split-K weight gradients)
 //
 // Replaces every nn.Linear on the path (reference modeling.py:232-234 Q/K/V, 271 attention output,
 // 303 intermediate, 316 output, 1220 visual projection) together with the element-wise work that
@@ -71,9 +71,9 @@ ProfScope::~ProfScope() {
 // ---------------------------------------------------------------------------------------------
 constexpr int BLOCK_M = 128;
 constexpr int BLOCK_K = 64;  // 64 bf16 = 128 bytes = one swizzle atom row
-constexpr int UMMA_K = 16;
+constexpr int WGMMA_K = 16;
 constexpr int kStages = 4;
-constexpr int kEpiWarps = 8;
+constexpr int kEpiWarps = 8;                    // the two MMA warpgroups
 constexpr int kThreads = 128 + kEpiWarps * 32;  // 384
 constexpr int kAtomBytes = 64 * BLOCK_K * 2;    // one 64(MN) x 64(K) bf16 swizzle atom = 8 KB
 
@@ -82,12 +82,15 @@ struct Cfg {
     static constexpr int A_BYTES = BLOCK_M * BLOCK_K * 2;
     static constexpr int B_BYTES = BLOCK_N * BLOCK_K * 2;
     static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
-    static constexpr int BAR_OFF = kStages * STAGE_BYTES;
-    static constexpr int NUM_BARS = 2 * kStages + 4;
-    static constexpr int TMEM_PTR_OFF = BAR_OFF + NUM_BARS * 8;
-    static constexpr int BIAS_OFF = TMEM_PTR_OFF + 16;           // 2 accumulator stages x BLOCK_N fp32
-    static constexpr int SMEM_BYTES = BIAS_OFF + 2 * BLOCK_N * 4 + 1024;  // +1024: manual 1 KB alignment
-    static constexpr int TMEM_COLS = 2 * BLOCK_N;                // power of two: 256 or 512
+    // fp32 accumulator tile for the epilogue, written over the drained operand ring; +4 floats per row keeps the
+    // row-per-lane reads of the epilogue free of bank conflicts
+    static constexpr int ACC_LD = BLOCK_N + 4;
+    static constexpr int RING_BYTES = kStages * STAGE_BYTES > BLOCK_M * ACC_LD * 4 ? kStages * STAGE_BYTES : BLOCK_M * ACC_LD * 4;
+    static constexpr int BAR_OFF = RING_BYTES;
+    static constexpr int NUM_BARS = 2 * kStages;
+    static constexpr int BIAS_OFF = BAR_OFF + NUM_BARS * 8;
+    static constexpr int SMEM_BYTES = BIAS_OFF + BLOCK_N * 4 + 1024;  // +1024: manual 1 KB alignment
+    static_assert(SMEM_BYTES <= 227 * 1024, "shared memory per block");
 };
 
 struct GemmParams {
@@ -103,34 +106,12 @@ struct GemmParams {
     unsigned drop_thresh16;  // n = round(p * 256): 8-bit keep threshold (see dropout_quantise)
     unsigned long long drop_seed;
     unsigned drop_stream;
-    int m_fast;              // tile order of the CTA-pair kernel: m-blocks run faster than n-blocks (see decode_tile)
+    int m_fast;              // tile order: m-blocks run faster than n-blocks (see decode_tile)
     float* delta_out;        // EPI_DELTA: fp32 [rows / delta_seq][N / 64][delta_seq]
     int delta_seq;
 };
-// vb_gemm_args.gp_tiled is honoured by the CTA-pair kernel with the staged-store epilogue on whole tiles only
 bool gemm_gp_tiled_ok(int M, int N);
 bool gemm_delta_ok(int M, int N);
-
-// UMMA shared-memory matrix descriptor (sm_100: version = 1), SWIZZLE_128B.
-//  K-major  operand tile [rows][64]: 8-row groups are 1024 B apart (SBO); LBO unused.
-//  MN-major operand tile [atoms of 64 along MN][64 k-rows][64]: 8 k-rows = 1024 B (SBO),
-//           next 64-wide MN atom = 64 k-rows * 128 B = 8192 B (LBO).
-__device__ __forceinline__ uint64_t make_smem_desc(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
-    uint64_t d = 0;
-    d |= static_cast<uint64_t>((saddr & 0x3FFFFu) >> 4);
-    d |= static_cast<uint64_t>((lbo_bytes >> 4) & 0x3FFFu) << 16;
-    d |= static_cast<uint64_t>((sbo_bytes >> 4) & 0x3FFFu) << 32;
-    d |= 1ull << 46;  // descriptor version (sm_100)
-    d |= 2ull << 61;  // SWIZZLE_128B
-    return d;
-}
-
-// tcgen05 instruction descriptor, kind::f16: D=f32, A=B=bf16, M=128, N=BLOCK_N, majors as given.
-__host__ __device__ constexpr uint32_t make_idesc(int n, bool a_mn, bool b_mn) {
-    return (1u << 4) | (1u << 7) | (1u << 10) | (static_cast<uint32_t>(a_mn) << 15) |
-           (static_cast<uint32_t>(b_mn) << 16) | (static_cast<uint32_t>(n >> 3) << 17) |
-           (static_cast<uint32_t>(BLOCK_M >> 4) << 24);
-}
 
 struct TileCoord {
     int m_blk, n_blk, kb_begin, kb_end;
@@ -138,8 +119,8 @@ struct TileCoord {
 // Tile order: the split index runs fastest, then the dimension with FEWER blocks (m_fast: there are fewer m-blocks), so that the
 // tiles in flight at any time share the slabs of the operand that spans the dimension with MORE blocks — the big one, which
 // must not be fetched from DRAM once per block of the other dimension (FFN-down weight gradient: M = 768, N = 3072, B = gelu(u)
-// is 258 MB, twice the L2: n-fastest order read it 2.4 times, profiles/r02b_layer_kernels_table.md).
-__device__ __forceinline__ TileCoord decode_tile(int t, int n_blocks, int splits, int k_blocks, int m_blocks = 0, bool m_fast = false) {
+// is several times the L2).
+__device__ __forceinline__ TileCoord decode_tile(int t, int n_blocks, int splits, int k_blocks, int m_blocks, bool m_fast) {
     TileCoord c;
     const int split = t % splits;
     const int mn = t / splits;
@@ -156,7 +137,7 @@ __device__ __forceinline__ TileCoord decode_tile(int t, int n_blocks, int splits
 }
 
 // Epilogue for 16 consecutive columns of one row held as fp32 in x[16]. All global traffic is
-// 32 bytes per thread per access (256-bit LDG/STG): a thread owns a row, so 32-byte pieces are the
+// 32 bytes per thread per access (two 128-bit accesses): a thread owns a row, so 32-byte pieces are the
 // unit that keeps every DRAM/L2 sector fully written.
 __device__ __forceinline__ void load16_bf16(const bf16* p, float (&f)[16]) {
     uint32_t r[8];
@@ -177,24 +158,23 @@ __device__ __forceinline__ void store16_bf16(bf16* p, const float (&f)[16]) {
 
 // `sbias` points at the 16 staged bias values of these columns in shared memory (or nullptr).
 // `ex` holds the 16 bf16 of the residual (addend) or of gelu'(u) (aux_in) for these columns, prefetched by the
-// caller one chunk ahead so the row-strided global load never sits on the critical path.
-// EPI selects the epilogue at COMPILE time for the CTA-pair kernel: the generic form (every option a run-time branch, all 8 chunks
-// unrolled) compiled to ~6 000 instructions (95 KB) per kernel — three times the SM's 32 KB L1.5 instruction cache, with
-// `no_instruction` stalls of 0.5-2.4 warps per issue cycle on the epilogue-bound launches. A specialised kernel carries only its path.
+// caller before the accumulators are staged, so the row-strided global load never sits on the critical path.
+// EPI selects the epilogue at COMPILE time: the generic form (every option a run-time branch, all chunks unrolled) is several
+// times larger than one specialised path, and instruction-cache misses then stall the epilogue. A specialised kernel carries
+// only its path.
 // _T: gelu'(u) is kept in the TILE-NATIVE layout (vb_gemm_args.gp_tiled): the only reader of that tensor is the epilogue of the
-// backward GEMM with the same tiling, where the same thread holds the same 16 columns — so it is written and read as whole
-// 1 KB warp blocks (lane l: 32 bytes at block + 32 l) instead of 32-byte pieces of 32 different rows.
+// backward GEMM, where the same thread holds the same 16 columns — so it is written and read as whole 1 KB warp blocks
+// (lane l: 32 bytes at block + 32 l) instead of 32-byte pieces of 32 different rows.
 // EPI_DELTA: plain bf16 store plus the attention backward's D[b, head, s] = sum_d dO[row, head, d] * O[row, head, d] (vb_gemm_args.delta_*):
 // the GEMM that PRODUCES dO (input gradient of attention.output.dense) has, in each epilogue thread, 128 consecutive columns of one row —
-// two whole heads — so the row-wise dot product with O needs no exchange; O is read like a residual operand (whole tile row requested
-// before the accumulator barrier).
+// two whole heads — so the row-wise dot product with O needs no exchange; O is read like a residual operand.
 enum { EPI_GENERIC = 0, EPI_BIAS = 1, EPI_RESID = 2, EPI_DROP_RESID = 3, EPI_GELU_FWD = 4, EPI_DGELU_BWD = 5, EPI_GELU_FWD_T = 6,
        EPI_DGELU_BWD_T = 7, EPI_DELTA = 8 };
 __host__ __device__ constexpr bool epi_is_gelu(int e) { return e == EPI_GELU_FWD || e == EPI_GELU_FWD_T; }
 __host__ __device__ constexpr bool epi_is_dgelu(int e) { return e == EPI_DGELU_BWD || e == EPI_DGELU_BWD_T; }
 
 // TO_REGS: nothing is stored; the 16 bf16 results are returned packed in o0 (what goes to D) and, for the GELU epilogue,
-// o1 (what goes to aux_out) — the caller stages them in shared memory for a TMA store.
+// o1 (what goes to aux_out) — the caller stores them.
 template <bool OUT_F32, int EPI = EPI_GENERIC, bool TO_REGS = false>
 __device__ __forceinline__ void epilogue16(const GemmParams& p, int row, int col, const float* sbias, const uint32_t (&ex)[8],
                                            float (&x)[16], uint32_t* o0 = nullptr, uint32_t* o1 = nullptr) {
@@ -262,11 +242,12 @@ __device__ __forceinline__ void epilogue16(const GemmParams& p, int row, int col
     }
 }
 
-template <bool A_MN, bool B_MN, int BLOCK_N, bool OUT_F32>
+template <bool A_MN, bool B_MN, int BLOCK_N, bool OUT_F32, int EPI = EPI_GENERIC>
 __global__ void __launch_bounds__(kThreads, 1)
-gemm_tcgen05_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
-                    const GemmParams p) {
+gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const GemmParams p) {
     using C = Cfg<BLOCK_N>;
+    static_assert(BLOCK_N % 128 == 0, "64 x 128 wgmma pieces");
+    static_assert(!(EPI == EPI_GELU_FWD_T || EPI == EPI_DGELU_BWD_T) || BLOCK_N == 256, "tile-native gelu' is defined on 256-wide tiles");
     extern __shared__ uint8_t smem_raw[];
     const uint32_t raw = smem_u32(smem_raw);
     const uint32_t base = (raw + 1023u) & ~1023u;  // SWIZZLE_128B tiles need 1 KB alignment
@@ -279,581 +260,192 @@ gemm_tcgen05_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_consta
     auto b_tile = [&](int s) { return base + s * C::STAGE_BYTES + C::A_BYTES; };
     auto full_bar = [&](int s) { return base + C::BAR_OFF + 8 * s; };
     auto empty_bar = [&](int s) { return base + C::BAR_OFF + 8 * (kStages + s); };
-    auto tfull_bar = [&](int s) { return base + C::BAR_OFF + 8 * (2 * kStages + s); };
-    auto tempty_bar = [&](int s) { return base + C::BAR_OFF + 8 * (2 * kStages + 2 + s); };
-    volatile uint32_t* tmem_ptr = reinterpret_cast<volatile uint32_t*>(smem + C::TMEM_PTR_OFF);
 
-    if (warp == 0 && lane == 0) {
+    if (threadIdx.x == 0) {
         tma_prefetch_desc(&tmA);
         tma_prefetch_desc(&tmB);
-    }
-    if (warp == 1 && lane == 0) {
         for (int s = 0; s < kStages; ++s) {
             mbar_init(full_bar(s), 1);
-            mbar_init(empty_bar(s), 1);
-        }
-        for (int s = 0; s < 2; ++s) {
-            mbar_init(tfull_bar(s), 1);
-            mbar_init(tempty_bar(s), kEpiWarps * 32);
+            mbar_init(empty_bar(s), 2);   // one arrival per MMA warpgroup
         }
         fence_barrier_init();
     }
-    if (warp == 2) tmem_alloc(base + C::TMEM_PTR_OFF, C::TMEM_COLS);
-    tcgen05_fence_before();
     __syncthreads();
-    tcgen05_fence_after();
-    const uint32_t tmem_base = *tmem_ptr;
     pdl_trigger();
     pdl_wait();  // everything above is on-chip set-up; operands of the previous kernel are read only from here on
 
     const int m_blocks = (p.M + BLOCK_M - 1) / BLOCK_M;
     const int n_blocks = (p.N + BLOCK_N - 1) / BLOCK_N;
     const int k_blocks = (p.K + BLOCK_K - 1) / BLOCK_K;
-    const int num_tiles = m_blocks * n_blocks * p.splits;
+    const TileCoord tc = decode_tile(blockIdx.x, n_blocks, p.splits, k_blocks, m_blocks, p.m_fast != 0);
 
-    if (warp == 0) {
-        {
+    if (warp < 4) {
+        reg_dec<40>();
+        if (warp == 0) {
             // ---------------- TMA producer (converged warp, one elected lane issues) ----------------
             int stage = 0;
             uint32_t phase = 0;
-            for (int t = blockIdx.x; t < num_tiles; t += gridDim.x) {
-                const TileCoord tc = decode_tile(t, n_blocks, p.splits, k_blocks);
-                for (int kb = tc.kb_begin; kb < tc.kb_end; ++kb) {
-                    mbar_wait(empty_bar(stage), phase ^ 1u);
-                    if (elect_one()) {
+            for (int kb = tc.kb_begin; kb < tc.kb_end; ++kb) {
+                mbar_wait(empty_bar(stage), phase ^ 1u);
+                if (elect_one()) {
                     mbar_arrive_expect_tx(full_bar(stage), C::STAGE_BYTES);
                     if constexpr (!A_MN) {
                         tma_load_2d(a_tile(stage), &tmA, full_bar(stage), kb * BLOCK_K, tc.m_blk * BLOCK_M);
                     } else {
 #pragma unroll
                         for (int i = 0; i < BLOCK_M / 64; ++i)
-                            tma_load_2d(a_tile(stage) + i * kAtomBytes, &tmA, full_bar(stage),
-                                        tc.m_blk * BLOCK_M + i * 64, kb * BLOCK_K);
+                            tma_load_2d(a_tile(stage) + i * kAtomBytes, &tmA, full_bar(stage), tc.m_blk * BLOCK_M + i * 64, kb * BLOCK_K);
                     }
                     if constexpr (!B_MN) {
                         tma_load_2d(b_tile(stage), &tmB, full_bar(stage), kb * BLOCK_K, tc.n_blk * BLOCK_N);
                     } else {
 #pragma unroll
                         for (int i = 0; i < BLOCK_N / 64; ++i)
-                            tma_load_2d(b_tile(stage) + i * kAtomBytes, &tmB, full_bar(stage),
-                                        tc.n_blk * BLOCK_N + i * 64, kb * BLOCK_K);
+                            tma_load_2d(b_tile(stage) + i * kAtomBytes, &tmB, full_bar(stage), tc.n_blk * BLOCK_N + i * 64, kb * BLOCK_K);
                     }
-                    }
-                    __syncwarp();
-                    if (++stage == kStages) { stage = 0; phase ^= 1u; }
                 }
-            }
-        }
-    } else if (warp == 1) {
-        {
-            // ---------------- MMA issuer: the warp runs the loop converged, one elected lane issues (uniform-register
-            // descriptors, back-to-back UTCHMMA; see profiles/r02_attention_tc.md §2) ----------------
-            constexpr uint32_t idesc = make_idesc(BLOCK_N, A_MN, B_MN);
-            // K-major: advance 16 elements (32 B) inside the swizzle row; MN-major: 16 k-rows (2 KB)
-            constexpr uint32_t a_kstep = A_MN ? UMMA_K * 128 : UMMA_K * 2;
-            constexpr uint32_t b_kstep = B_MN ? UMMA_K * 128 : UMMA_K * 2;
-            constexpr uint32_t a_lbo = A_MN ? kAtomBytes : 0;
-            constexpr uint32_t b_lbo = B_MN ? kAtomBytes : 0;
-            int stage = 0;
-            uint32_t phase = 0;
-            int it = 0;
-            for (int t = blockIdx.x; t < num_tiles; t += gridDim.x, ++it) {
-                const TileCoord tc = decode_tile(t, n_blocks, p.splits, k_blocks);
-                const int acc = it & 1;
-                const uint32_t acc_phase = (it >> 1) & 1;
-                mbar_wait(tempty_bar(acc), acc_phase ^ 1u);
-                tcgen05_fence_after();
-                const uint32_t d_tmem = tmem_base + acc * BLOCK_N;
-                for (int kb = tc.kb_begin; kb < tc.kb_end; ++kb) {
-                    mbar_wait(full_bar(stage), phase);
-                    tcgen05_fence_after();
-                    const UmmaDesc ad = make_umma_desc_sw128(a_tile(stage), a_lbo, 1024), bd = make_umma_desc_sw128(b_tile(stage), b_lbo, 1024);
-                    if (elect_one()) {
-#pragma unroll
-                        for (int k = 0; k < BLOCK_K / UMMA_K; ++k)
-                            umma_bf16(d_tmem, ad.at(k * a_kstep), bd.at(k * b_kstep), idesc, (kb > tc.kb_begin || k > 0) ? 1u : 0u);
-                        umma_commit(empty_bar(stage));  // frees the smem slot when these MMAs retire
-                        if (kb == tc.kb_end - 1) umma_commit(tfull_bar(acc));
-                    }
-                    __syncwarp();
-                    if (++stage == kStages) { stage = 0; phase ^= 1u; }
-                }
-            }
-        }
-    } else if (warp >= 4) {
-        // ---------------- epilogue ----------------
-        const int ew = warp - 4;
-        const int q = warp & 3;   // TMEM lane quarter this warp may access
-        const int half = ew >> 2; // which half of the tile's columns
-        const int et = threadIdx.x - 128;  // 0..255 among the epilogue threads
-        float* sbias_all = reinterpret_cast<float*>(smem + C::BIAS_OFF);
-        constexpr int NCH = BLOCK_N / 2 / 16;  // 16-column chunks per warp
-        int it = 0;
-        for (int t = blockIdx.x; t < num_tiles; t += gridDim.x, ++it) {
-            const TileCoord tc = decode_tile(t, n_blocks, p.splits, k_blocks);
-            const int acc = it & 1;
-            const uint32_t acc_phase = (it >> 1) & 1;
-            // Stage this tile's bias slice while its MMAs are still running. The barrier is executed on EVERY
-            // tile (uniformly) when a bias exists: passing it proves all epilogue warps finished the previous
-            // tile, so the slab written two tiles later is no longer being read. With split-K the bias
-            // belongs to the whole sum: only split 0 adds it, the other splits stage zeros.
-            const bool has_bias = p.bias != nullptr;
-            float* sb = sbias_all + acc * BLOCK_N;
-            if (has_bias) {
-                const bool mine = p.splits == 1 || (t % p.splits) == 0;
-                for (int i = et; i < BLOCK_N; i += kEpiWarps * 32) {
-                    const int col = tc.n_blk * BLOCK_N + i;
-                    sb[i] = (mine && col < p.N) ? __ldg(p.bias + col) : 0.f;
-                }
-                named_bar_sync(1, kEpiWarps * 32);
-            }
-            const int row = tc.m_blk * BLOCK_M + q * 32 + lane;
-            const int col0 = tc.n_blk * BLOCK_N + half * (BLOCK_N / 2);
-            // Residual / gelu' operand of this thread's row: one 32-byte load per 16-column chunk. The loads are
-            // row-strided DRAM accesses (~1 us each under load), so kExAhead of them are kept in flight and the
-            // first batch is issued BEFORE waiting for the accumulator.
-            constexpr int kExAhead = 4;
-            uint32_t ex[kExAhead][8];
-            const bf16* exp_ = nullptr;
-            if constexpr (!OUT_F32) {
-                if (p.addend != nullptr) exp_ = p.addend + static_cast<long long>(row) * p.ld_add;
-                else if (p.epilogue == VB_EPI_DGELU) exp_ = p.aux_in + static_cast<long long>(row) * p.ld_aux;
-                if (row >= p.M) exp_ = nullptr;
-            }
-#pragma unroll
-            for (int k = 0; k < kExAhead; ++k)
-                if (exp_ != nullptr && col0 + k * 16 < p.N) ldg_v8(exp_ + col0 + k * 16, ex[k]);
-            mbar_wait(tfull_bar(acc), acc_phase);
-            tcgen05_fence_after();
-            const uint32_t taddr0 = tmem_base + (static_cast<uint32_t>(q * 32) << 16) + acc * BLOCK_N +
-                                    half * (BLOCK_N / 2);
-            // software pipeline: the TMEM load of chunk k+1 is in flight while chunk k is processed
-            uint32_t v[2][16];
-            tmem_ld_32x32b_x16(taddr0, v[0]);
-#pragma unroll
-            for (int k = 0; k < NCH; ++k) {
-                tmem_ld_wait();
-                if (k + 1 < NCH) tmem_ld_32x32b_x16(taddr0 + (k + 1) * 16, v[(k + 1) & 1]);
-                const int col = col0 + k * 16;
-                if (row < p.M && col < p.N) {
-                    float x[16];
-#pragma unroll
-                    for (int i = 0; i < 16; ++i) x[i] = __uint_as_float(v[k & 1][i]);
-                    epilogue16<OUT_F32>(p, row, col, has_bias ? sb + half * (BLOCK_N / 2) + k * 16 : nullptr, ex[k % kExAhead], x);
-                }
-                // buffer k % kExAhead is free again: refill it with the operand of chunk k + kExAhead
-                if (k + kExAhead < NCH && exp_ != nullptr && col0 + (k + kExAhead) * 16 < p.N)
-                    ldg_v8(exp_ + col0 + (k + kExAhead) * 16, ex[k % kExAhead]);
-            }
-            tcgen05_fence_before();
-            mbar_arrive(tempty_bar(acc));
-        }
-    }
-
-    tcgen05_fence_before();
-    __syncthreads();
-    if (warp == 2) {
-        tcgen05_fence_after();
-        tmem_dealloc(tmem_base, C::TMEM_COLS);
-    }
-}
-
-// ---------------------------------------------------------------------------------------------
-// CTA-pair variant (cta_group::2): a cluster of two CTAs on neighbouring SMs computes one 256 x 256 tile.
-// Each CTA stages its own 128 rows of A and HALF of the B tile (128 of the 256 columns); the leader's single
-// tcgen05.mma.cta_group::2 (M = 256) reads both halves from both shared memories, so per-SM shared-memory
-// traffic per FLOP drops by a third and the ring fits 6 stages. Each CTA keeps its 128 x 256 fp32 accumulator
-// rows in its own TMEM and runs its own epilogue.
-//   full[s]   lives in the leader: 2 arrivals (leader: expect_tx of both CTAs' bytes; peer: remote arrive) + tx
-//   empty[s], tmem_full[a]  live in both CTAs, arrived by the leader's multicast tcgen05.commit
-//   tmem_empty[a]           lives in the leader: 2 x 256 epilogue-thread arrivals (peer arrives remotely)
-// ---------------------------------------------------------------------------------------------
-#ifndef VB_GEMM_DEEP_EX
-#define VB_GEMM_DEEP_EX 1   // 0: ring of four operand buffers instead of the whole tile row (A/B timing, scripts/build_variant.sh)
-#endif
-// TMA_ST: the epilogue stages its bf16 output in shared memory (one private 32-row x 64-column swizzled slab per epilogue
-// warp) and writes it with TMA stores. A thread owns a ROW of the tile, so direct global stores are 32 separate 32-byte
-// sectors per warp instruction; measured (scripts/gpu_check_gemm.py perf) every such scattered sector costs ~3 cycles of
-// the SM's load/store path — 12.7 k cycles per tile for the two outputs of the GELU epilogue against 9 k for the tile's
-// main loop. The slabs take the room of one pipeline stage (5 instead of 6).
-template <bool TMA_ST>
-struct Cfg2T {
-    static constexpr int kStages2 = TMA_ST ? 5 : 6;
-    static constexpr int STAGING_BYTES = TMA_ST ? kEpiWarps * 4096 : 0;
-    static constexpr int BLOCK_N = 256;
-    static constexpr int A_BYTES = 128 * BLOCK_K * 2;       // this CTA's 128 rows of A
-    static constexpr int B_BYTES = 128 * BLOCK_K * 2;       // this CTA's half of the 256 B rows
-    static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
-    static constexpr int STAGING_OFF = kStages2 * STAGE_BYTES;  // 1 KB aligned (stages are 32 KB)
-    static constexpr int BAR_OFF = STAGING_OFF + STAGING_BYTES;
-    static constexpr int NUM_BARS = 2 * kStages2 + 4;
-    static constexpr int TMEM_PTR_OFF = BAR_OFF + NUM_BARS * 8;
-    static constexpr int BIAS_OFF = TMEM_PTR_OFF + 16;
-    static constexpr int SMEM_BYTES = BIAS_OFF + 2 * BLOCK_N * 4 + 1024;
-    static constexpr int TMEM_COLS = 512;
-};
-using Cfg2 = Cfg2T<false>;
-
-__host__ __device__ constexpr uint32_t make_idesc_m(int m, int n, bool a_mn, bool b_mn) {
-    return (1u << 4) | (1u << 7) | (1u << 10) | (static_cast<uint32_t>(a_mn) << 15) |
-           (static_cast<uint32_t>(b_mn) << 16) | (static_cast<uint32_t>(n >> 3) << 17) |
-           (static_cast<uint32_t>(m >> 4) << 24);
-}
-
-// CL = 4 ("quad"): two CTA pairs per cluster work on the SAME 256 columns of B and on neighbouring 256-row blocks of A.
-// Each CTA fetches only half of its 128 x 64 part of the B tile and TMA-multicasts it to the CTA holding the same part
-// in the other pair, so the L2 -> SM operand traffic per pair and k-block drops from 64 KB to 48 KB. (These GEMMs run at
-// the L2 bandwidth limit — see DESIGN.md — which is why this matters.) A stage may only be refilled once BOTH pairs have
-// consumed it (the other pair writes into it too): empty[s] counts one commit from each pair.
-template <bool A_MN, bool B_MN, bool OUT_F32, int EPI, int CL = 2, bool TMA_ST = false>
-__global__ void __launch_bounds__(kThreads, 1)
-gemm_tcgen05_2cta_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
-                         const __grid_constant__ CUtensorMap tmD, const __grid_constant__ CUtensorMap tmAux, const GemmParams p) {
-    constexpr bool kTmaSt = TMA_ST;
-    static_assert(!TMA_ST || (!OUT_F32 && EPI != EPI_GENERIC), "staged stores: bf16 outputs of the specialised epilogues");
-    using C = Cfg2T<kTmaSt>;
-    constexpr int kStages2 = C::kStages2;
-    constexpr int BLOCK_N = 256;
-    extern __shared__ uint8_t smem_raw[];
-    const uint32_t raw = smem_u32(smem_raw);
-    const uint32_t base = (raw + 1023u) & ~1023u;
-    uint8_t* smem = smem_raw + (base - raw);
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    constexpr bool kQuad = CL == 4;
-    static_assert(CL == 2 || CL == 4, "cluster of one or two CTA pairs");
-    static_assert(!kQuad || !OUT_F32, "the quad variant has no split-K path");
-    const uint32_t crank = cluster_ctarank();
-    const uint32_t rank = crank & 1u;          // rank inside the CTA pair
-    const uint32_t pair = crank >> 1;          // 0, or 0/1 in a quad
-    const uint32_t leader_rank = crank & ~1u;  // cluster rank of this pair's leader
-    const bool leader = rank == 0;
-
-    auto a_tile = [&](int s) { return base + s * C::STAGE_BYTES; };
-    auto b_tile = [&](int s) { return base + s * C::STAGE_BYTES + C::A_BYTES; };
-    auto full_bar = [&](int s) { return base + C::BAR_OFF + 8 * s; };
-    auto empty_bar = [&](int s) { return base + C::BAR_OFF + 8 * (kStages2 + s); };
-    auto tfull_bar = [&](int s) { return base + C::BAR_OFF + 8 * (2 * kStages2 + s); };
-    auto tempty_bar = [&](int s) { return base + C::BAR_OFF + 8 * (2 * kStages2 + 2 + s); };
-    volatile uint32_t* tmem_ptr = reinterpret_cast<volatile uint32_t*>(smem + C::TMEM_PTR_OFF);
-
-    if (warp == 0 && lane == 0) {
-        tma_prefetch_desc(&tmA);
-        tma_prefetch_desc(&tmB);
-    }
-    if (warp == 1 && lane == 0) {
-        for (int s = 0; s < kStages2; ++s) {
-            mbar_init(full_bar(s), 2);
-            mbar_init(empty_bar(s), kQuad ? 2 : 1);
-        }
-        for (int s = 0; s < 2; ++s) {
-            mbar_init(tfull_bar(s), 1);
-            mbar_init(tempty_bar(s), 2 * kEpiWarps * 32);
-        }
-        fence_barrier_init();
-    }
-    cluster_sync_all();  // barriers of both CTAs initialised before anyone signals across the pair
-    if (warp == 2) tmem_alloc_2cta(base + C::TMEM_PTR_OFF, C::TMEM_COLS);
-    tcgen05_fence_before();
-    cluster_sync_all();
-    tcgen05_fence_after();
-    const uint32_t tmem_base = *tmem_ptr;
-    pdl_trigger();
-    pdl_wait();  // everything above is on-chip set-up; operands of the previous kernel are read only from here on
-
-    const int m_blocks = (p.M + 255) / 256;
-    const int n_blocks = (p.N + BLOCK_N - 1) / BLOCK_N;
-    const int k_blocks = (p.K + BLOCK_K - 1) / BLOCK_K;
-    // quad: a "tile" of the loops below is a pair of m-blocks (2j, 2j + 1) x one n-block; pair 1 of an odd tail works on
-    // an all-out-of-bounds block (TMA zero fill, epilogue rows masked) so the four CTAs stay in step
-    const int num_tiles = kQuad ? ((m_blocks + 1) / 2) * n_blocks : m_blocks * n_blocks * p.splits;
-    const int cluster_id = blockIdx.x / CL, num_clusters = gridDim.x / CL;
-    auto tile_of = [&](int t) {
-        TileCoord c = decode_tile(t, n_blocks, kQuad ? 1 : p.splits, k_blocks, m_blocks, !kQuad && p.m_fast != 0);
-        if constexpr (kQuad) c.m_blk = c.m_blk * 2 + static_cast<int>(pair);
-        return c;
-    };
-    const uint32_t empty_mask = kQuad ? 0xFu : 3u, pair_mask = 3u << (2 * pair);
-
-    // Epilogues that read a second operand (residual / gelu') hold the whole tile row of it in registers (see below): the
-    // four control warps hand registers to the eight epilogue warps (128 * 72 + 256 * 216 = 384 * 168).
-    constexpr bool kDeepEx = VB_GEMM_DEEP_EX && !OUT_F32 && (EPI == EPI_RESID || EPI == EPI_DROP_RESID || EPI == EPI_DELTA || epi_is_dgelu(EPI));
-    if (warp == 0) {
-        if constexpr (kDeepEx) reg_dec<72>();
-        {
-            // ---------------- TMA producer (both CTAs; converged warp, one elected lane issues) ----------------
-            int stage = 0;
-            uint32_t phase = 0;
-            for (int t = cluster_id; t < num_tiles; t += num_clusters) {
-                const TileCoord tc = tile_of(t);
-                const int m0 = tc.m_blk * 256 + static_cast<int>(rank) * 128;
-                const int n0 = tc.n_blk * BLOCK_N + static_cast<int>(rank) * 128;
-                for (int kb = tc.kb_begin; kb < tc.kb_end; ++kb) {
-                    mbar_wait(empty_bar(stage), phase ^ 1u);
-                    if (elect_one()) {
-                    if (leader) mbar_arrive_expect_tx(full_bar(stage), 2 * C::STAGE_BYTES);
-                    else mbar_arrive_remote(full_bar(stage), leader_rank);
-                    if constexpr (!A_MN) {
-                        tma_load_2d_2cta(a_tile(stage), &tmA, full_bar(stage), kb * BLOCK_K, m0);
-                    } else {
-#pragma unroll
-                        for (int i = 0; i < 2; ++i)
-                            tma_load_2d_2cta(a_tile(stage) + i * kAtomBytes, &tmA, full_bar(stage), m0 + i * 64, kb * BLOCK_K);
-                    }
-                    if constexpr (kQuad) {
-                        // this CTA's half (64 of the 128 B columns it holds: one 8 KB swizzle-atom block in either major),
-                        // multicast to the CTA with the same pair rank in the other pair
-                        const uint32_t mc = rank ? 0xAu : 0x5u;
-                        const uint32_t dst = b_tile(stage) + pair * kAtomBytes;
-                        if constexpr (!B_MN) tma_load_2d_2cta_mc(dst, &tmB, full_bar(stage), kb * BLOCK_K, n0 + static_cast<int>(pair) * 64, mc);
-                        else                 tma_load_2d_2cta_mc(dst, &tmB, full_bar(stage), n0 + static_cast<int>(pair) * 64, kb * BLOCK_K, mc);
-                    } else if constexpr (!B_MN) {
-                        tma_load_2d_2cta(b_tile(stage), &tmB, full_bar(stage), kb * BLOCK_K, n0);
-                    } else {
-#pragma unroll
-                        for (int i = 0; i < 2; ++i)
-                            tma_load_2d_2cta(b_tile(stage) + i * kAtomBytes, &tmB, full_bar(stage), n0 + i * 64, kb * BLOCK_K);
-                    }
-                    }
-                    __syncwarp();
-                    if (++stage == kStages2) { stage = 0; phase ^= 1u; }
-                }
-            }
-        }
-    } else if (warp == 1) {
-        if constexpr (kDeepEx) reg_dec<72>();
-        if (leader) {
-            // ---------------- MMA issuer (leader CTA only): converged warp, one elected lane issues ----------------
-            constexpr uint32_t idesc = make_idesc_m(256, BLOCK_N, A_MN, B_MN);
-            constexpr uint32_t a_kstep = A_MN ? UMMA_K * 128 : UMMA_K * 2;
-            constexpr uint32_t b_kstep = B_MN ? UMMA_K * 128 : UMMA_K * 2;
-            constexpr uint32_t a_lbo = A_MN ? kAtomBytes : 0;
-            constexpr uint32_t b_lbo = B_MN ? kAtomBytes : 0;
-            int stage = 0;
-            uint32_t phase = 0;
-            int it = 0;
-            for (int t = cluster_id; t < num_tiles; t += num_clusters, ++it) {
-                const TileCoord tc = tile_of(t);
-                const int acc = it & 1;
-                const uint32_t acc_phase = (it >> 1) & 1;
-                mbar_wait(tempty_bar(acc), acc_phase ^ 1u);
-                tcgen05_fence_after();
-                const uint32_t d_tmem = tmem_base + acc * BLOCK_N;
-                for (int kb = tc.kb_begin; kb < tc.kb_end; ++kb) {
-                    mbar_wait(full_bar(stage), phase);
-                    tcgen05_fence_after();
-                    const UmmaDesc ad = make_umma_desc_sw128(a_tile(stage), a_lbo, 1024), bd = make_umma_desc_sw128(b_tile(stage), b_lbo, 1024);
-                    if (elect_one()) {
-#pragma unroll
-                        for (int k = 0; k < BLOCK_K / UMMA_K; ++k)
-                            umma_bf16_2cta(d_tmem, ad.at(k * a_kstep), bd.at(k * b_kstep), idesc, (kb > tc.kb_begin || k > 0) ? 1u : 0u);
-                        umma_commit_2cta(empty_bar(stage), empty_mask);
-                        if (kb == tc.kb_end - 1) umma_commit_2cta(tfull_bar(acc), pair_mask);
-                    }
-                    __syncwarp();
-                    if (++stage == kStages2) { stage = 0; phase ^= 1u; }
-                }
-            }
-            // the peer's epilogue arrives remotely on our tmem_empty barriers: wait for the last two tiles'
-            // arrivals before this CTA may exit (its shared memory must stay valid until then)
-            for (int j = (it >= 2 ? it - 2 : 0); j < it; ++j) mbar_wait(tempty_bar(j & 1), (j >> 1) & 1);
-        }
-    } else if (warp >= 4) {
-        if constexpr (kDeepEx) reg_inc<216>();
-        // ---------------- epilogue (both CTAs, 128 rows each) ----------------
-        const int ew = warp - 4;
-        const int q = warp & 3;
-        const int half = ew >> 2;
-        const int et = threadIdx.x - 128;
-        float* sbias_all = reinterpret_cast<float*>(smem + C::BIAS_OFF);
-        constexpr int NCH = BLOCK_N / 2 / 16;
-        int it = 0;
-        for (int t = cluster_id; t < num_tiles; t += num_clusters, ++it) {
-            const TileCoord tc = tile_of(t);
-            const int acc = it & 1;
-            const uint32_t acc_phase = (it >> 1) & 1;
-            const bool has_bias = p.bias != nullptr;
-            float* sb = sbias_all + acc * BLOCK_N;
-            if (has_bias) {
-                const bool mine = p.splits == 1 || (t % p.splits) == 0;
-                for (int i = et; i < BLOCK_N; i += kEpiWarps * 32) {
-                    const int col = tc.n_blk * BLOCK_N + i;
-                    sb[i] = (mine && col < p.N) ? __ldg(p.bias + col) : 0.f;
-                }
-                named_bar_sync(1, kEpiWarps * 32);
-            }
-            const int row0w = tc.m_blk * 256 + static_cast<int>(rank) * 128 + q * 32;  // first of this warp's 32 rows
-            const int row = row0w + lane;
-            const int col0 = tc.n_blk * BLOCK_N + half * (BLOCK_N / 2);
-            // staged TMA store (kTmaSt): this warp's private slab, 32 rows x 128 bytes, 128-byte swizzle
-            const uint32_t slab = base + C::STAGING_OFF + ew * 4096;
-            auto stage16 = [&](int kk, const uint32_t (&o)[8]) {  // 16 columns = 16-byte units 2kk, 2kk + 1 of this thread's row
-                const uint32_t rowa = slab + lane * 128, sw = static_cast<uint32_t>(lane & 7);
-                sts_v4(rowa + ((2u * kk) ^ sw) * 16, o[0], o[1], o[2], o[3]);
-                sts_v4(rowa + ((2u * kk + 1u) ^ sw) * 16, o[4], o[5], o[6], o[7]);
-            };
-            auto slab_free = [&]() {  // the previous store of this warp has read the slab
-                if (lane == 0) bulk_wait_group_read0();
                 __syncwarp();
-            };
-            auto flush = [&](const CUtensorMap* tm, int c0) {  // rows / columns beyond M / N are clipped by the TMA unit
-                fence_proxy_async_smem();
-                __syncwarp();
-                if (lane == 0) { tma_store_2d(tm, slab, c0, row0w); bulk_commit_group(); }
-            };
-            constexpr int kExAhead = 4;
-            const bf16* exp_ = nullptr;
-            if constexpr (!OUT_F32) {
-                constexpr bool kWantAdd = EPI == EPI_RESID || EPI == EPI_DROP_RESID || EPI == EPI_DELTA;   // EPI_DELTA: addend = O
-                if (kWantAdd || (EPI == EPI_GENERIC && p.addend != nullptr)) exp_ = p.addend + static_cast<long long>(row) * p.ld_add;
-                else if (EPI == EPI_DGELU_BWD || (EPI == EPI_GENERIC && p.epilogue == VB_EPI_DGELU)) exp_ = p.aux_in + static_cast<long long>(row) * p.ld_aux;
-                if (row >= p.M) exp_ = nullptr;
+                if (++stage == kStages) { stage = 0; phase ^= 1u; }
             }
-            // chunk k of the operand: exb + k * ex_step. Row-major: 16 columns further in this thread's row. Tile-native gelu'(u)
-            // (M, N multiples of 256): the next 1 KB warp block of this warp's 8 KB region, lane l at + 32 l bytes.
-            constexpr long long ex_step = EPI == EPI_DGELU_BWD_T ? 512 : 16;
-            const long long gp_tile_off = ((((static_cast<long long>(tc.m_blk) * n_blocks + tc.n_blk) * 2 + rank) * kEpiWarps + ew) * NCH) * 512 + lane * 16;
-            const bf16* exb = exp_ != nullptr ? exp_ + col0 : nullptr;
-            if constexpr (EPI == EPI_DGELU_BWD_T) { exp_ = p.aux_in; exb = p.aux_in + gp_tile_off; }
-            const uint32_t taddr0 = tmem_base + (static_cast<uint32_t>(q * 32) << 16) + acc * BLOCK_N + half * (BLOCK_N / 2);
-            uint32_t v[2][16];
-            if constexpr (kDeepEx) {
-                // The whole tile row of the operand (8 chunks = 256 bytes per thread) is requested BEFORE waiting for the
-                // accumulator, i.e. while this tile's main loop is still running: nothing of the DRAM latency is left in the
-                // epilogue. Two banks of four buffers; the group loop stays rolled (code size) and picks its bank with
-                // selects.
-                static_assert(NCH == 2 * kExAhead, "two banks");
-                uint32_t exA[kExAhead][8], exB[kExAhead][8];
+        }
+        return;
+    }
+    reg_inc<232>();
+
+    // ---------------- MMA warpgroups: rows 64 wg .. 64 wg + 63 of the tile, all BLOCK_N columns ----------------
+    const int wg = (warp >> 2) - 1;
+    const int et = threadIdx.x - 128;  // 0..255 among the MMA / epilogue threads
+    float* sbias = reinterpret_cast<float*>(smem + C::BIAS_OFF);
+    const bool has_bias = p.bias != nullptr;
+    if (has_bias) {   // with split-K the bias belongs to the whole sum: only split 0 adds it, the other splits stage zeros
+        const bool mine = p.splits == 1 || (blockIdx.x % p.splits) == 0;
+        for (int i = et; i < BLOCK_N; i += kEpiWarps * 32) {
+            const int col = tc.n_blk * BLOCK_N + i;
+            sbias[i] = (mine && col < p.N) ? __ldg(p.bias + col) : 0.f;
+        }
+    }
+    constexpr int NH = BLOCK_N / 128;
+    // K-major: advance 16 elements (32 B) inside the swizzle row; MN-major: 16 k-rows (2 KB)
+    constexpr uint32_t a_kstep = A_MN ? WGMMA_K * 128 : WGMMA_K * 2;
+    constexpr uint32_t b_kstep = B_MN ? WGMMA_K * 128 : WGMMA_K * 2;
+    float acc[NH][64];
+    {
+        int stage = 0, prev = 0;
+        uint32_t phase = 0;
+        for (int kb = tc.kb_begin; kb < tc.kb_end; ++kb) {
+            mbar_wait(full_bar(stage), phase);
+            // this warpgroup's 64 rows of A: 64 K-major rows or one 64-wide MN-major atom = 8 KB further in both layouts;
+            // the second 128 columns of B likewise start 16 KB further
+            const uint32_t a0 = a_tile(stage) + wg * 8192, b0 = b_tile(stage);
+            wgmma_fence();
 #pragma unroll
-                for (int k = 0; k < kExAhead; ++k)
-                    if (exp_ != nullptr && col0 + k * 16 < p.N) ldg_v8(exb + k * ex_step, exA[k]);
+            for (int k = 0; k < BLOCK_K / WGMMA_K; ++k) {
+                const uint64_t ad = wgmma_desc_sw128(a0 + k * a_kstep, kAtomBytes, 1024);
 #pragma unroll
-                for (int k = 0; k < kExAhead; ++k)
-                    if (exp_ != nullptr && col0 + (k + kExAhead) * 16 < p.N) ldg_v8(exb + (k + kExAhead) * ex_step, exB[k]);
-                mbar_wait(tfull_bar(acc), acc_phase);
-                tcgen05_fence_after();
-                tmem_ld_32x32b_x16(taddr0, v[0]);
-                [[maybe_unused]] float hsum = 0.f;
-#pragma unroll 1
-                for (int k0 = 0; k0 < NCH; k0 += kExAhead) {
+                for (int h = 0; h < NH; ++h)
+                    wgmma_m64n128k16<A_MN ? 1 : 0, B_MN ? 1 : 0>(acc[h], ad, wgmma_desc_sw128(b0 + h * 16384 + k * b_kstep, kAtomBytes, 1024),
+                                                                 (kb > tc.kb_begin || k > 0) ? 1u : 0u);
+            }
+            wgmma_commit();
+            // the MMAs of the previous k-block have retired: its slot may be refilled
+            wgmma_wait<1>();
+            if (kb > tc.kb_begin && (threadIdx.x & 127) == 0) mbar_arrive(empty_bar(prev));
+            prev = stage;
+            if (++stage == kStages) { stage = 0; phase ^= 1u; }
+        }
+        wgmma_wait<0>();
+    }
+
+    // ---------------- epilogue ----------------
+    // Thread -> element map: epilogue warp ew owns rows 32 (ew % 4) .. + 31 (one per lane) and the column half ew / 4 of the tile,
+    // in 16-column chunks. Operands read by the epilogue (residual / gelu') are requested before the accumulators are staged.
+    const int ew = warp - 4;
+    const int q = ew & 3, half = ew >> 2;
+    const int lrow = q * 32 + lane;
+    const int row = tc.m_blk * BLOCK_M + lrow;
+    const int col0 = tc.n_blk * BLOCK_N + half * (BLOCK_N / 2);
+    constexpr int NCH = BLOCK_N / 2 / 16;
+    // tile-native gelu'(u) (M, N multiples of 256; vbert_b200.h): 1 KB warp blocks, lane l at + 32 l bytes
+    const long long gp_tile_off =
+        ((((static_cast<long long>(tc.m_blk >> 1) * n_blocks + tc.n_blk) * 2 + (tc.m_blk & 1)) * kEpiWarps + ew) * NCH) * 512 + lane * 16;
+    const bf16* exb = nullptr;
+    long long ex_step = 16;
+    if constexpr (!OUT_F32) {
+        constexpr bool kWantAdd = EPI == EPI_RESID || EPI == EPI_DROP_RESID || EPI == EPI_DELTA;   // EPI_DELTA: addend = O
+        if (row < p.M) {
+            if (kWantAdd || (EPI == EPI_GENERIC && p.addend != nullptr)) exb = p.addend + static_cast<long long>(row) * p.ld_add + col0;
+            else if (EPI == EPI_DGELU_BWD || (EPI == EPI_GENERIC && p.epilogue == VB_EPI_DGELU))
+                exb = p.aux_in + static_cast<long long>(row) * p.ld_aux + col0;
+            else if (EPI == EPI_DGELU_BWD_T) { exb = p.aux_in + gp_tile_off; ex_step = 512; }
+        }
+    }
+    constexpr bool kEx = !OUT_F32 && EPI != EPI_BIAS && !epi_is_gelu(EPI);
+    uint32_t ex[kEx ? NCH : 1][8];
+    if constexpr (kEx) {
 #pragma unroll
-                    for (int kk = 0; kk < kExAhead; ++kk) {
-                        const int k = k0 + kk;
-                        tmem_ld_wait();
-                        if (k + 1 < NCH) tmem_ld_32x32b_x16(taddr0 + (k + 1) * 16, v[(kk + 1) & 1]);
-                        const int col = col0 + k * 16;
-                        if (kTmaSt || (row < p.M && col < p.N)) {
-                            float x[16];
-                            uint32_t e[8];
+        for (int k = 0; k < NCH; ++k)
+            if (exb != nullptr && col0 + k * 16 < p.N) ldg_v8(exb + k * ex_step, ex[k]);
+    }
+
+    // both warpgroups' MMAs have retired (and with them every read of the ring): stage the accumulators over the ring
+    named_bar_sync(1, kEpiWarps * 32);
+    float* sacc = reinterpret_cast<float*>(smem);
+    {
+        const int r0 = wg * 64 + ((warp & 3) << 4) + (lane >> 2);
 #pragma unroll
-                            for (int i = 0; i < 16; ++i) x[i] = __uint_as_float(v[kk & 1][i]);
+        for (int h = 0; h < NH; ++h)
 #pragma unroll
-                            for (int i = 0; i < 8; ++i) e[i] = k0 ? exB[kk][i] : exA[kk][i];
-                            if constexpr (kTmaSt) {
-                                uint32_t o0[8];
-                                epilogue16<OUT_F32, EPI, true>(p, row, col, has_bias ? sb + half * (BLOCK_N / 2) + k * 16 : nullptr, e, x, o0);
-                                if constexpr (EPI == EPI_DELTA) {   // dot product of the ROUNDED dO (what the attention kernel will read) with O
+            for (int j = 0; j < 16; ++j)
 #pragma unroll
-                                    for (int i = 0; i < 8; ++i) {
-                                        const float2 a = unpack_bf16x2(o0[i]), b = unpack_bf16x2(e[i]);
-                                        hsum = fmaf(a.x, b.x, fmaf(a.y, b.y, hsum));
-                                    }
-                                }
-                                if (kk == 0) slab_free();
-                                stage16(kk, o0);
-                            } else {
-                                epilogue16<OUT_F32, EPI>(p, row, col, has_bias ? sb + half * (BLOCK_N / 2) + k * 16 : nullptr, e, x);
-                            }
-                        }
-                    }
-                    if constexpr (kTmaSt) flush(&tmD, col0 + k0 * 16);
-                    if constexpr (EPI == EPI_DELTA) {   // the group's four chunks are exactly one head (col0 is a multiple of 128)
-                        const int head = (col0 + k0 * 16) >> 6;
-                        if (row < p.M && col0 + k0 * 16 < p.N) {
-                            const int bi = row / p.delta_seq, si = row - bi * p.delta_seq;
-                            p.delta_out[(static_cast<long long>(bi) * (p.N >> 6) + head) * p.delta_seq + si] = hsum;
-                        }
-                        hsum = 0.f;
-                    }
+                for (int i = 0; i < 2; ++i)
+                    *reinterpret_cast<float2*>(sacc + (r0 + 8 * i) * C::ACC_LD + h * 128 + j * 8 + 2 * (lane & 3)) =
+                        make_float2(acc[h][4 * j + 2 * i], acc[h][4 * j + 2 * i + 1]);
+    }
+    named_bar_sync(1, kEpiWarps * 32);
+
+    const float* srow = sacc + lrow * C::ACC_LD + half * (BLOCK_N / 2);
+    [[maybe_unused]] float hsum = 0.f;
+#pragma unroll
+    for (int k = 0; k < NCH; ++k) {
+        const int col = col0 + k * 16;
+        if (row < p.M && col < p.N) {
+            float x[16];
+#pragma unroll
+            for (int i = 0; i < 4; ++i) {
+                const float4 v = *reinterpret_cast<const float4*>(srow + k * 16 + 4 * i);
+                x[4 * i] = v.x; x[4 * i + 1] = v.y; x[4 * i + 2] = v.z; x[4 * i + 3] = v.w;
+            }
+            const float* sb = has_bias ? sbias + half * (BLOCK_N / 2) + k * 16 : nullptr;
+            const uint32_t (&e)[8] = ex[kEx ? k : 0];
+            if constexpr (EPI == EPI_GELU_FWD_T) {
+                // gelu'(u): one coalesced 1 KB warp store into the tile-native buffer; gelu(u): row-major
+                uint32_t o0[8], o1[8];
+                epilogue16<OUT_F32, EPI, true>(p, row, col, sb, e, x, o0, o1);
+                stg_v8(reinterpret_cast<bf16*>(p.D) + gp_tile_off + k * 512, o0);
+                stg_v8(p.aux_out + static_cast<long long>(row) * p.ld_aux + col, o1);
+            } else if constexpr (EPI == EPI_DELTA) {
+                uint32_t o0[8];
+                epilogue16<OUT_F32, EPI, true>(p, row, col, sb, e, x, o0);
+                stg_v8(reinterpret_cast<bf16*>(p.D) + static_cast<long long>(row) * p.ldd + col, o0);
+#pragma unroll
+                for (int i = 0; i < 8; ++i) {   // dot product of the ROUNDED dO (what the attention kernel will read) with O
+                    const float2 a = unpack_bf16x2(o0[i]), b = unpack_bf16x2(e[i]);
+                    hsum = fmaf(a.x, b.x, fmaf(a.y, b.y, hsum));
                 }
             } else {
-                // Residual / gelu' operand of this thread's row (generic kernel): one 32-byte load per 16-column chunk,
-                // kExAhead of them in flight, the first batch issued BEFORE waiting for the accumulator.
-                uint32_t ex[kExAhead][8];
-#pragma unroll
-                for (int k = 0; k < kExAhead; ++k)
-                    if (exp_ != nullptr && col0 + k * 16 < p.N) ldg_v8(exb + k * ex_step, ex[k]);
-                mbar_wait(tfull_bar(acc), acc_phase);
-                tcgen05_fence_after();
-                tmem_ld_32x32b_x16(taddr0, v[0]);
-                // chunks in groups: inside a group every buffer index is static; the group loop is NOT unrolled (code size)
-                // (epilogues without a prefetched operand only need the 2-deep TMEM double buffer: groups of 2 halve their code again)
-                constexpr int kGroup = (!kTmaSt && (epi_is_gelu(EPI) || EPI == EPI_BIAS)) ? 2 : kExAhead;  // staged stores: one slab = 4 chunks
-                static_assert(NCH % kGroup == 0, "chunk groups");
-                uint32_t gk[kTmaSt && EPI == EPI_GELU_FWD ? kGroup : 1][8];  // gelu(u) of the slab, stored after gelu'(u)
-#pragma unroll 1
-                for (int k0 = 0; k0 < NCH; k0 += kGroup) {
-#pragma unroll
-                    for (int kk = 0; kk < kGroup; ++kk) {
-                        const int k = k0 + kk;
-                        tmem_ld_wait();
-                        if (k + 1 < NCH) tmem_ld_32x32b_x16(taddr0 + (k + 1) * 16, v[(kk + 1) & 1]);
-                        const int col = col0 + k * 16;
-                        if (kTmaSt || (row < p.M && col < p.N)) {
-                            float x[16];
-#pragma unroll
-                            for (int i = 0; i < 16; ++i) x[i] = __uint_as_float(v[kk & 1][i]);
-                            if constexpr (EPI == EPI_GELU_FWD_T) {
-                                // gelu'(u): one coalesced 1 KB warp store into the tile-native buffer; gelu(u): staged for the TMA store
-                                static_assert(kTmaSt, "the tile-native GELU epilogue stages gelu(u)");
-                                uint32_t o0[8], o1[8];
-                                epilogue16<OUT_F32, EPI, true>(p, row, col, has_bias ? sb + half * (BLOCK_N / 2) + k * 16 : nullptr, ex[kk], x, o0, o1);
-                                stg_v8(reinterpret_cast<bf16*>(p.D) + gp_tile_off + k * 512, o0);
-                                if (kk == 0) slab_free();
-                                stage16(kk, o1);
-                            } else if constexpr (kTmaSt) {
-                                uint32_t o0[8];
-                                epilogue16<OUT_F32, EPI, true>(p, row, col, has_bias ? sb + half * (BLOCK_N / 2) + k * 16 : nullptr, ex[kk], x, o0,
-                                                               gk[EPI == EPI_GELU_FWD ? kk : 0]);
-                                if (kk == 0) slab_free();
-                                stage16(kk, o0);
-                            } else {
-                                epilogue16<OUT_F32, EPI>(p, row, col, has_bias ? sb + half * (BLOCK_N / 2) + k * 16 : nullptr, ex[kk], x);
-                            }
-                        }
-                        // buffer kk is free again: refill it with the operand of chunk k + kExAhead
-                        if (k + kExAhead < NCH && exp_ != nullptr && col0 + (k + kExAhead) * 16 < p.N)
-                            ldg_v8(exb + (k + kExAhead) * ex_step, ex[kk]);
-                    }
-                    if constexpr (EPI == EPI_GELU_FWD_T) {
-                        flush(&tmAux, col0 + k0 * 16);
-                    } else if constexpr (kTmaSt) {
-                        flush(&tmD, col0 + k0 * 16);
-                        if constexpr (EPI == EPI_GELU_FWD) {
-                            slab_free();
-#pragma unroll
-                            for (int kk = 0; kk < kGroup; ++kk) stage16(kk, gk[kk]);
-                            flush(&tmAux, col0 + k0 * 16);
-                        }
-                    }
-                }
+                epilogue16<OUT_F32, EPI>(p, row, col, sb, e, x);
             }
-            tcgen05_fence_before();
-            if (leader) mbar_arrive(tempty_bar(acc));
-            else mbar_arrive_remote(tempty_bar(acc), leader_rank);
         }
-        if constexpr (kTmaSt) {
-            if (lane == 0) bulk_wait_group0();   // the staged stores have left shared memory and are complete before the CTA exits
-            __syncwarp();
+        if constexpr (EPI == EPI_DELTA) {
+            if ((k & 3) == 3) {   // four chunks are exactly one head (col0 is a multiple of 64)
+                const int c4 = col - 48;
+                if (row < p.M && c4 < p.N) {
+                    const int bi = row / p.delta_seq, si = row - bi * p.delta_seq;
+                    p.delta_out[(static_cast<long long>(bi) * (p.N >> 6) + (c4 >> 6)) * p.delta_seq + si] = hsum;
+                }
+                hsum = 0.f;
+            }
         }
-    } else {
-        if constexpr (kDeepEx) reg_dec<72>();   // warps 2 and 3 release their share as well (the pool is per CTA)
-    }
-
-    tcgen05_fence_before();
-    cluster_sync_all();
-    if (warp == 2) {
-        tcgen05_fence_after();
-        tmem_dealloc_2cta(tmem_base, C::TMEM_COLS);
     }
 }
 
@@ -931,15 +523,6 @@ int make_tmap_bf16(CUtensorMap* m, const void* ptr, uint64_t inner, uint64_t out
     return encode_tmap_cached(m, ptr, 2, dims, strides, box);
 }
 
-// 3-D bf16 tensor map over x[B][S][ld]: box = 64 columns x box_rows rows x 1 batch, 128-byte swizzle, OOB rows -> 0
-int make_tmap_3d(CUtensorMap* m, const void* ptr, int S, int B, int ld, int box_rows) {
-    VB_REQUIRE((reinterpret_cast<uintptr_t>(ptr) & 15) == 0 && (ld * 2) % 16 == 0, "TMA operand (3-D) not 16-byte aligned");
-    cuuint64_t dims[3] = {static_cast<cuuint64_t>(ld), static_cast<cuuint64_t>(S), static_cast<cuuint64_t>(B)};
-    cuuint64_t strides[2] = {static_cast<cuuint64_t>(ld) * 2, static_cast<cuuint64_t>(S) * ld * 2};
-    cuuint32_t box[3] = {64, static_cast<cuuint32_t>(box_rows), 1};
-    return encode_tmap_cached(m, ptr, 3, dims, strides, box);
-}
-
 int current_device() {
     int dev = 0;
     cudaGetDevice(&dev);
@@ -952,94 +535,26 @@ int num_sms() {
     if (n[dev] == 0) {
         int v = 0;
         cudaDeviceGetAttribute(&v, cudaDevAttrMultiProcessorCount, dev);
-        n[dev] = v > 0 ? v : 148;
+        n[dev] = v > 0 ? v : 132;
     }
     return n[dev];
 }
 
-template <bool A_MN, bool B_MN, int BLOCK_N, bool OUT_F32>
+template <bool A_MN, bool B_MN, int BLOCK_N, bool OUT_F32, int EPI = EPI_GENERIC>
 static int launch(const CUtensorMap& ta, const CUtensorMap& tb, const GemmParams& p, cudaStream_t st) {
     using C = Cfg<BLOCK_N>;
-    auto kern = gemm_tcgen05_kernel<A_MN, B_MN, BLOCK_N, OUT_F32>;
+    auto kern = gemm_wgmma_kernel<A_MN, B_MN, BLOCK_N, OUT_F32, EPI>;
     static int configured[kMaxDevices] = {0};
     VB_CHECK_CUDA(ensure_dyn_smem(kern, C::SMEM_BYTES, configured));
-    const int m_blocks = (p.M + BLOCK_M - 1) / BLOCK_M;
-    const int n_blocks = (p.N + BLOCK_N - 1) / BLOCK_N;
-    const int tiles = m_blocks * n_blocks * p.splits;
-    const int grid = tiles < num_sms() ? tiles : num_sms();
+    const long long tiles = static_cast<long long>((p.M + BLOCK_M - 1) / BLOCK_M) * ((p.N + BLOCK_N - 1) / BLOCK_N) * p.splits;
+    VB_REQUIRE(tiles < (1LL << 31), "vb_gemm: too many tiles");
     {
         ProfScope ps(st, OUT_F32 ? PROF_GEMM_WGRAD : (B_MN ? PROF_GEMM_DGRAD : PROF_GEMM_FWD), 2.0 * p.M * p.N * p.K, 1);
-        VB_CHECK_CUDA(launch_pdl(kern, dim3(grid), dim3(kThreads), C::SMEM_BYTES, st, ta, tb, p));
+        VB_CHECK_CUDA(launch_pdl(kern, dim3(static_cast<unsigned>(tiles)), dim3(kThreads), C::SMEM_BYTES, st, ta, tb, p));
     }
     VB_CHECK_CUDA(cudaGetLastError());
     return 0;
 }
-
-// td / tx: tensor maps of D and aux_out for the staged TMA stores (unused by kernels that store from registers)
-template <bool A_MN, bool B_MN, bool OUT_F32, int EPI = EPI_GENERIC, bool TMA_ST = false>
-static int launch2(const CUtensorMap& ta, const CUtensorMap& tb, const CUtensorMap& td, const CUtensorMap& tx, const GemmParams& p,
-                   cudaStream_t st) {
-    auto kern = gemm_tcgen05_2cta_kernel<A_MN, B_MN, OUT_F32, EPI, 2, TMA_ST>;
-    using C = Cfg2T<TMA_ST>;
-    static int configured[kMaxDevices] = {0};
-    VB_CHECK_CUDA(ensure_dyn_smem(kern, C::SMEM_BYTES, configured));
-    const int tiles = ((p.M + 255) / 256) * ((p.N + 255) / 256) * p.splits;
-    int clusters = num_sms() / 2;
-    if (clusters > tiles) clusters = tiles;
-    {
-        ProfScope ps(st, OUT_F32 ? PROF_GEMM_WGRAD : (B_MN ? PROF_GEMM_DGRAD : PROF_GEMM_FWD), 2.0 * p.M * p.N * p.K, 1);
-        VB_CHECK_CUDA(launch_pdl_cluster(kern, dim3(2 * clusters), dim3(kThreads), C::SMEM_BYTES, st, 2, ta, tb, td, tx, p));
-    }
-    VB_CHECK_CUDA(cudaGetLastError());
-    return 0;
-}
-
-// Quad variant (two CTA pairs per cluster sharing the B tile by TMA multicast). Returns -1 when clusters of four cannot be
-// placed on this device (the caller then uses the pair kernel).
-template <bool B_MN, int EPI, bool TMA_ST = false>
-static int launch4(const CUtensorMap& ta, const CUtensorMap& tb, const CUtensorMap& td, const CUtensorMap& tx, const GemmParams& p,
-                   cudaStream_t st) {
-    auto kern = gemm_tcgen05_2cta_kernel<false, B_MN, false, EPI, 4, TMA_ST>;
-    using Cfg2 = Cfg2T<TMA_ST>;
-    static int configured[kMaxDevices] = {0};
-    static int resident[kMaxDevices] = {0};  // clusters of four that fit on the device at once (0 = not asked yet)
-    VB_CHECK_CUDA(ensure_dyn_smem(kern, Cfg2::SMEM_BYTES, configured));
-    const int dev = current_device();
-    if (resident[dev] == 0) {
-        cudaLaunchConfig_t cfg = {};
-        cfg.gridDim = dim3(4 * (num_sms() / 4));
-        cfg.blockDim = dim3(kThreads);
-        cfg.dynamicSmemBytes = Cfg2::SMEM_BYTES;
-        cudaLaunchAttribute attr[1];
-        attr[0].id = cudaLaunchAttributeClusterDimension;
-        attr[0].val.clusterDim.x = 4; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
-        cfg.attrs = attr;
-        cfg.numAttrs = 1;
-        int n = 0;
-        if (cudaOccupancyMaxActiveClusters(&n, kern, &cfg) != cudaSuccess) { cudaGetLastError(); n = 0; }
-        resident[dev] = n > 0 ? n : -1;
-        if (getenv("VB_GEMM_DEBUG")) fprintf(stderr, "[vb_gemm] device %d: %d clusters of four CTAs fit (%d SMs)\n", dev, n, num_sms());
-    }
-    if (resident[dev] < 0) return -1;
-    const int tiles = (((p.M + 255) / 256 + 1) / 2) * ((p.N + 255) / 256);
-    int clusters = resident[dev] < num_sms() / 4 ? resident[dev] : num_sms() / 4;
-    if (clusters > tiles) clusters = tiles;
-    {
-        ProfScope ps(st, B_MN ? PROF_GEMM_DGRAD : PROF_GEMM_FWD, 2.0 * p.M * p.N * p.K, 1);
-        VB_CHECK_CUDA(launch_pdl_cluster(kern, dim3(4 * clusters), dim3(kThreads), Cfg2::SMEM_BYTES, st, 4, ta, tb, td, tx, p));
-    }
-    VB_CHECK_CUDA(cudaGetLastError());
-    return 0;
-}
-// VB_GEMM_QUAD=1 opts in to the quad kernels. Off by default: measured on B200 (r02, scripts/gpu_check_gemm.py perf) only
-// 33 clusters of four are co-resident (132 of 148 SMs) and the saved L2 traffic does not make up for the idle SMs — the
-// layer's GEMMs are 5-9 % slower than on the pair kernel (DESIGN.md "negative results").
-static int quad_mode() {   // 0: never, 1: every specialised epilogue, 2: only the tile-native GELU / DGELU launches
-    static int v = -1;
-    if (v < 0) { const char* e = getenv("VB_GEMM_QUAD"); v = e != nullptr ? atoi(e) : 0; }
-    return v;
-}
-static bool use_quad() { return quad_mode() == 1; }
 
 bool pdl_enabled() {
     static const bool on = [] {
@@ -1049,20 +564,14 @@ bool pdl_enabled() {
     return on;
 }
 
-// VB_GEMM_2CTA=0 disables the CTA-pair kernels (testing / tuning)
-static bool use_2cta() {
-    static int v = -1;
-    if (v < 0) { const char* e = getenv("VB_GEMM_2CTA"); v = (e != nullptr && atoi(e) == 0) ? 0 : 1; }
-    return v == 1;
-}
 bool gemm_delta_ok(int M, int N) {
     static const int off = [] { const char* e = getenv("VB_GEMM_DELTA"); return (e != nullptr && atoi(e) == 0) ? 1 : 0; }();
     const int n_pad256 = (N + 255) / 256 * 256;
-    return !off && use_2cta() && M >= 256 && N >= 256 && N % 64 == 0 && (n_pad256 - N) * 8 <= N;
+    return !off && M >= 256 && N >= 256 && N % 64 == 0 && (n_pad256 - N) * 8 <= N;
 }
 bool gemm_gp_tiled_ok(int M, int N) {
     static const int off = [] { const char* e = getenv("VB_GEMM_GP_TILED"); return (e != nullptr && atoi(e) == 0) ? 1 : 0; }();
-    return !off && use_2cta() && M >= 256 && M % 256 == 0 && N % 256 == 0;
+    return !off && M >= 256 && M % 256 == 0 && N % 256 == 0;
 }
 
 int gemm(const vb_gemm_args& a, cudaStream_t st) {
@@ -1087,6 +596,9 @@ int gemm(const vb_gemm_args& a, cudaStream_t st) {
                "vb_gemm: delta_out needs a plain bf16 input-gradient GEMM (b_mn_major, no bias / addend / dropout) and vb_gemm_delta_ok(M, N)");
     VB_REQUIRE(!a.gp_tiled || (gemm_gp_tiled_ok(a.M, a.N) && !a.d_fp32 && !a.a_mn_major && (a.epilogue == VB_EPI_GELU || a.epilogue == VB_EPI_DGELU)),
                "vb_gemm: gp_tiled needs a GELU / DGELU epilogue and vb_gemm_gp_tiled_ok(M, N)");
+    VB_REQUIRE(!a.gp_tiled || a.epilogue != VB_EPI_DGELU || a.b_mn_major,
+               "vb_gemm: gp_tiled with the DGELU epilogue needs an MN-major B (the input-gradient GEMM)");
+    VB_REQUIRE(!a.gp_tiled || a.epilogue != VB_EPI_GELU || !a.b_mn_major, "vb_gemm: gp_tiled with the GELU epilogue needs a K-major B");
 
     GemmParams p;
     memset(&p, 0, sizeof(p));
@@ -1108,7 +620,7 @@ int gemm(const vb_gemm_args& a, cudaStream_t st) {
     }
     {
         static const int order_off = [] { const char* e = getenv("VB_GEMM_TILE_ORDER"); return (e != nullptr && atoi(e) == 0) ? 1 : 0; }();
-        p.m_fast = (!order_off && (a.M + 255) / 256 < (a.N + 255) / 256) ? 1 : 0;
+        p.m_fast = (!order_off && (a.M + BLOCK_M - 1) / BLOCK_M < (a.N + 255) / 256) ? 1 : 0;
     }
     if (a.dropout_p > 0.0f) {
         const DropQ q = dropout_quantise(a.dropout_p);
@@ -1121,117 +633,48 @@ int gemm(const vb_gemm_args& a, cudaStream_t st) {
     // BLOCK_N: 256 unless N is small or padding N up to a multiple of 256 wastes more than 1/8 of the columns
     const int n_pad256 = (a.N + 255) / 256 * 256;
     const bool bn256 = (a.N >= 256) && ((n_pad256 - a.N) * 8 <= a.N);
-    const int BN = bn256 ? 256 : 128;
+    VB_REQUIRE(!a.delta_out || bn256, "vb_gemm: delta_out needs 256-wide tiles");
 
     CUtensorMap ta, tb;
     int rc;
-    // CTA-pair kernel: 256 x 256 tiles, each CTA loads 128-row boxes of A and of its half of B
-    if (use_2cta() && bn256 && a.M >= 256) {
-        if (!a.a_mn_major) rc = make_tmap_bf16(&ta, a.A, a.K, a.M, a.lda, 128);
-        else               rc = make_tmap_bf16(&ta, a.A, a.M, a.K, a.lda, BLOCK_K);
-        if (rc) return rc;
-        if (!a.b_mn_major) rc = make_tmap_bf16(&tb, a.B, a.K, a.N, a.ldb, 128);
-        else               rc = make_tmap_bf16(&tb, a.B, a.N, a.K, a.ldb, BLOCK_K);
-        if (rc) return rc;
-        if (!a.d_fp32) {
-            // specialised epilogues for the shapes of the layer (forward and input-gradient GEMMs); anything else: generic
-            const bool drop = a.dropout_p > 0.0f, add = a.addend != nullptr;
-            int epi = EPI_GENERIC;
-            if (a.epilogue == VB_EPI_GELU && !drop && !add) epi = a.gp_tiled ? EPI_GELU_FWD_T : EPI_GELU_FWD;
-            else if (a.epilogue == VB_EPI_DGELU && !drop && !add) epi = a.gp_tiled ? EPI_DGELU_BWD_T : EPI_DGELU_BWD;
-            else if (a.epilogue == VB_EPI_NONE) epi = add ? (drop ? EPI_DROP_RESID : EPI_RESID) : (drop ? EPI_GENERIC : EPI_BIAS);
-            if (a.delta_out) epi = EPI_DELTA;
-            VB_REQUIRE(!a.gp_tiled || epi == EPI_GELU_FWD_T || epi == EPI_DGELU_BWD_T,
-                       "vb_gemm: gp_tiled needs a plain GELU / DGELU epilogue (no dropout, no addend)");
-            // Staged TMA stores where the epilogue, not the main loop, bounds the tile (measured r02, same box, us per
-            // launch with / without: FFN-up + GELU 200 / 214, attention-output 59 / 66, but K = 3072 or bias-only epilogues
-            // 3-4 us SLOWER — the slabs cost a pipeline stage). VB_GEMM_TMA_STORE=0 / 1 forces never / wherever possible.
-            static const int tma_mode = [] { const char* e = getenv("VB_GEMM_TMA_STORE"); return e ? atoi(e) : 2; }();
-            bool tma_st = false;
-            if (tma_mode == 1 || epi == EPI_GELU_FWD_T || epi == EPI_DELTA) tma_st = epi != EPI_GENERIC;
-            else if (tma_mode != 0)
-                tma_st = epi_is_gelu(epi) || epi_is_dgelu(epi) || ((epi == EPI_RESID || epi == EPI_DROP_RESID) && a.K <= 1536);
-            // output tensor maps for the staged TMA stores: 64-column x 32-row boxes (one epilogue warp's slab)
-            CUtensorMap td = ta, tx = ta;
-            if (tma_st) {
-                rc = make_tmap_bf16(&td, a.D, a.N, a.M, a.ldd, 32);
-                if (rc) return rc;
-                if (epi_is_gelu(epi)) {
-                    rc = make_tmap_bf16(&tx, a.aux_out, a.N, a.M, a.ld_aux, 32);
-                    if (rc) return rc;
-                }
-            }
-            // quad clusters for the tall activation GEMMs of the layer (at least two 256-row blocks to pair up)
-            if (quad_mode() == 2 && a.M > 256) {
-                int q = -1;
-                if (epi == EPI_GELU_FWD_T) {
-                    CUtensorMap tq;
-                    rc = make_tmap_bf16(&tq, a.B, a.K, a.N, a.ldb, 64);
-                    if (rc) return rc;
-                    q = launch4<false, EPI_GELU_FWD_T, true>(ta, tq, td, tx, p, st);
-                } else if (epi == EPI_DGELU_BWD_T && a.b_mn_major) {
-                    q = launch4<true, EPI_DGELU_BWD_T, true>(ta, tb, td, tx, p, st);
-                }
-                if (q >= 0) return q;
-            }
-            if (use_quad() && epi != EPI_GENERIC && epi != EPI_GELU_FWD_T && epi != EPI_DGELU_BWD_T && !a.a_mn_major && a.M > 256) {
-                CUtensorMap tq;  // K-major B is fetched in 64-row boxes (half of a CTA's part), MN-major B already is
-                int q = 1;
-                if (!a.b_mn_major) {
-                    rc = make_tmap_bf16(&tq, a.B, a.K, a.N, a.ldb, 64);
-                    if (rc) return rc;
-                    switch (epi) {
-                        case EPI_BIAS: q = launch4<false, EPI_BIAS>(ta, tq, td, tx, p, st); break;
-                        case EPI_RESID: q = launch4<false, EPI_RESID>(ta, tq, td, tx, p, st); break;
-                        case EPI_DROP_RESID: q = launch4<false, EPI_DROP_RESID>(ta, tq, td, tx, p, st); break;
-                        case EPI_GELU_FWD: q = launch4<false, EPI_GELU_FWD>(ta, tq, td, tx, p, st); break;
-                        default: q = -1; break;
-                    }
-                } else {
-                    switch (epi) {
-                        case EPI_BIAS: q = launch4<true, EPI_BIAS>(ta, tb, td, tx, p, st); break;
-                        case EPI_RESID: q = launch4<true, EPI_RESID>(ta, tb, td, tx, p, st); break;
-                        case EPI_DGELU_BWD: q = launch4<true, EPI_DGELU_BWD>(ta, tb, td, tx, p, st); break;
-                        default: q = -1; break;
-                    }
-                }
-                if (q >= 0) return q;  // launched (0) or failed (> 0); -1: no room for clusters of four, fall through
-            }
-            if (!a.a_mn_major && !a.b_mn_major) {
-                switch (epi) {
-                    case EPI_BIAS: return (tma_st ? launch2<false, false, false, EPI_BIAS, true>(ta, tb, td, tx, p, st) : launch2<false, false, false, EPI_BIAS, false>(ta, tb, td, tx, p, st));
-                    case EPI_RESID: return (tma_st ? launch2<false, false, false, EPI_RESID, true>(ta, tb, td, tx, p, st) : launch2<false, false, false, EPI_RESID, false>(ta, tb, td, tx, p, st));
-                    case EPI_DROP_RESID: return (tma_st ? launch2<false, false, false, EPI_DROP_RESID, true>(ta, tb, td, tx, p, st) : launch2<false, false, false, EPI_DROP_RESID, false>(ta, tb, td, tx, p, st));
-                    case EPI_GELU_FWD: return (tma_st ? launch2<false, false, false, EPI_GELU_FWD, true>(ta, tb, td, tx, p, st) : launch2<false, false, false, EPI_GELU_FWD, false>(ta, tb, td, tx, p, st));
-                    case EPI_GELU_FWD_T: return launch2<false, false, false, EPI_GELU_FWD_T, true>(ta, tb, td, tx, p, st);
-                    default: return launch2<false, false, false>(ta, tb, ta, ta, p, st);
-                }
-            }
-            if (!a.a_mn_major && a.b_mn_major) {
-                switch (epi) {
-                    case EPI_BIAS: return (tma_st ? launch2<false, true, false, EPI_BIAS, true>(ta, tb, td, tx, p, st) : launch2<false, true, false, EPI_BIAS, false>(ta, tb, td, tx, p, st));
-                    case EPI_RESID: return (tma_st ? launch2<false, true, false, EPI_RESID, true>(ta, tb, td, tx, p, st) : launch2<false, true, false, EPI_RESID, false>(ta, tb, td, tx, p, st));
-                    case EPI_DGELU_BWD: return (tma_st ? launch2<false, true, false, EPI_DGELU_BWD, true>(ta, tb, td, tx, p, st) : launch2<false, true, false, EPI_DGELU_BWD, false>(ta, tb, td, tx, p, st));
-                    case EPI_DELTA: return launch2<false, true, false, EPI_DELTA, true>(ta, tb, td, tx, p, st);
-                    case EPI_DGELU_BWD_T: return (tma_st ? launch2<false, true, false, EPI_DGELU_BWD_T, true>(ta, tb, td, tx, p, st) : launch2<false, true, false, EPI_DGELU_BWD_T, false>(ta, tb, td, tx, p, st));
-                    default: return launch2<false, true, false>(ta, tb, ta, ta, p, st);
-                }
-            }
-            if (a.a_mn_major && a.b_mn_major) return launch2<true, true, false>(ta, tb, ta, ta, p, st);
-            return launch2<true, false, false>(ta, tb, ta, ta, p, st);
-        } else {
-            if (!a.a_mn_major && !a.b_mn_major) return launch2<false, false, true>(ta, tb, ta, ta, p, st);
-            if (!a.a_mn_major && a.b_mn_major) return launch2<false, true, true>(ta, tb, ta, ta, p, st);
-            if (a.a_mn_major && a.b_mn_major) return launch2<true, true, true>(ta, tb, ta, ta, p, st);
-            return launch2<true, false, true>(ta, tb, ta, ta, p, st);
-        }
-    }
     if (!a.a_mn_major) rc = make_tmap_bf16(&ta, a.A, a.K, a.M, a.lda, BLOCK_M);
     else               rc = make_tmap_bf16(&ta, a.A, a.M, a.K, a.lda, BLOCK_K);
     if (rc) return rc;
-    if (!a.b_mn_major) rc = make_tmap_bf16(&tb, a.B, a.K, a.N, a.ldb, BN);
+    if (!a.b_mn_major) rc = make_tmap_bf16(&tb, a.B, a.K, a.N, a.ldb, bn256 ? 256 : 128);
     else               rc = make_tmap_bf16(&tb, a.B, a.N, a.K, a.ldb, BLOCK_K);
     if (rc) return rc;
+
+    if (bn256 && !a.d_fp32) {
+        // specialised epilogues for the shapes of the layer (forward and input-gradient GEMMs); anything else: generic
+        const bool drop = a.dropout_p > 0.0f, add = a.addend != nullptr;
+        int epi = EPI_GENERIC;
+        if (a.epilogue == VB_EPI_GELU && !drop && !add) epi = a.gp_tiled ? EPI_GELU_FWD_T : EPI_GELU_FWD;
+        else if (a.epilogue == VB_EPI_DGELU && !drop && !add) epi = a.gp_tiled ? EPI_DGELU_BWD_T : EPI_DGELU_BWD;
+        else if (a.epilogue == VB_EPI_NONE) epi = add ? (drop ? EPI_DROP_RESID : EPI_RESID) : (drop ? EPI_GENERIC : EPI_BIAS);
+        if (a.delta_out) epi = EPI_DELTA;
+        VB_REQUIRE(!a.gp_tiled || epi == EPI_GELU_FWD_T || epi == EPI_DGELU_BWD_T,
+                   "vb_gemm: gp_tiled needs a plain GELU / DGELU epilogue (no dropout, no addend)");
+        if (!a.a_mn_major && !a.b_mn_major) {
+            switch (epi) {
+                case EPI_BIAS: return launch<false, false, 256, false, EPI_BIAS>(ta, tb, p, st);
+                case EPI_RESID: return launch<false, false, 256, false, EPI_RESID>(ta, tb, p, st);
+                case EPI_DROP_RESID: return launch<false, false, 256, false, EPI_DROP_RESID>(ta, tb, p, st);
+                case EPI_GELU_FWD: return launch<false, false, 256, false, EPI_GELU_FWD>(ta, tb, p, st);
+                case EPI_GELU_FWD_T: return launch<false, false, 256, false, EPI_GELU_FWD_T>(ta, tb, p, st);
+                default: return launch<false, false, 256, false>(ta, tb, p, st);
+            }
+        }
+        if (!a.a_mn_major && a.b_mn_major) {
+            switch (epi) {
+                case EPI_BIAS: return launch<false, true, 256, false, EPI_BIAS>(ta, tb, p, st);
+                case EPI_RESID: return launch<false, true, 256, false, EPI_RESID>(ta, tb, p, st);
+                case EPI_DGELU_BWD: return launch<false, true, 256, false, EPI_DGELU_BWD>(ta, tb, p, st);
+                case EPI_DELTA: return launch<false, true, 256, false, EPI_DELTA>(ta, tb, p, st);
+                case EPI_DGELU_BWD_T: return launch<false, true, 256, false, EPI_DGELU_BWD_T>(ta, tb, p, st);
+                default: return launch<false, true, 256, false>(ta, tb, p, st);
+            }
+        }
+    }
 
 #define VB_DISPATCH(AM, BM, F32)                                         \
     (bn256 ? launch<AM, BM, 256, F32>(ta, tb, p, st) : launch<AM, BM, 128, F32>(ta, tb, p, st))

@@ -14,7 +14,6 @@ namespace vb {
 
 constexpr int kLnWarps = 8;
 
-// (two rows per warp, both requested up front, measured SLOWER in-step: 0.965 vs 0.905 ms per step, r02)
 template <int NC>
 __global__ void __launch_bounds__(kLnWarps * 32)
 ln_fwd_kernel(const bf16* __restrict__ x, long long ldx, const float* __restrict__ gamma,
@@ -150,7 +149,7 @@ ln_bwd_kernel(const bf16* __restrict__ dy, const bf16* __restrict__ x, const flo
         const float nmr = -mu * rs;
         const float rs_cur = rs;
         // the row is unpacked ONCE: xh = xhat and dv = dy stay in fp32 registers for both passes (the kernel is
-        // instruction-issue bound, not register/occupancy bound: profiles/r01final_layer_kernels.md)
+        // instruction-issue bound, not register/occupancy bound)
         float xh[NC][8], dv[NC][8];
         float s1 = 0.f, s2 = 0.f;
 #pragma unroll

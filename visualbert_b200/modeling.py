@@ -4,7 +4,7 @@ Drop-in boundary (SURVEY.md §8b): `TrainVisualBERTObjective` / `BertVisualModel
 `from_pretrained`, forward signature, output dict and `state_dict` keys of
 uclanlp/visualbert `visualbert/pytorch_pretrained_bert/modeling.py` (cited as M.py:line below), so the
 repo's AllenNLP wrappers (`visualbert/models/model.py:213-288`) can import these classes instead.
-What differs is underneath: embeddings + the BertLayer stack execute as hand-written sm_100a kernels
+What differs is underneath: embeddings + the BertLayer stack execute as hand-written sm_90a kernels
 (bf16 activations, fp32 master weights and gradients); task heads, pooler and losses stay PyTorch.
 
 Modules here are parameter containers with the reference's names; `forward` hands the parameters to
@@ -730,7 +730,7 @@ class TrainVisualBERTObjective(PreTrainedBertModel):
         head = self.cls.predictions
         if rows.numel() == 0 or not hidden.is_cuda:
             return F.cross_entropy(head(hidden).float(), labels.index_select(0, rows))
-        # decoder + loss on the library's kernels: tcgen05 GEMMs (fwd / dgrad / wgrad into the tied word-embedding
+        # decoder + loss on the library's kernels: wgmma GEMMs (fwd / dgrad / wgrad into the tied word-embedding
         # gradient) and the fused cross-entropy; the small transform (dense + gelu + LayerNorm on ~12 % of the rows)
         # stays PyTorch
         scores = ops.mlm_decoder(head.transform(hidden), head.decoder.weight, head.bias, self._decoder_cache(), self.training)

@@ -1,7 +1,7 @@
 """torch.autograd bindings of the libvbert_b200 C ABI (include/vbert_b200.h).
 
 PyTorch supplies device memory, the current stream and the autograd graph; every FLOP of the
-encoder path runs in the sm_100a kernels. There is no fallback: on a machine without the library or
+encoder path runs in the sm_90a kernels. There is no fallback: on a machine without the library or
 without a CUDA device these ops raise.
 
 Activations are bf16; parameters are the model's fp32 master weights, cast to bf16 "compute weights"
@@ -27,7 +27,7 @@ def _ptr(t):
 def _require_cuda(t, what):
     if not t.is_cuda:
         raise _lib.VBertLibraryError(
-            f"{what}: tensor is on {t.device}; visualbert_b200 runs only on CUDA (sm_100a) — no CPU fallback")
+            f"{what}: tensor is on {t.device}; visualbert_b200 runs only on CUDA (sm_90a) — no CPU fallback")
 
 
 # --------------------------------------------------------------------------------------------
@@ -541,7 +541,7 @@ def bert_embeddings(meta, input_ids, token_type_ids, visual_type, feats, word, p
 
 
 # --------------------------------------------------------------------------------------------
-# masked-LM head on the library's kernels (SURVEY.md §8f rank 1): decoder GEMMs on tcgen05, fused cross-entropy
+# masked-LM head on the library's kernels (SURVEY.md §8f rank 1): decoder GEMMs on wgmma, fused cross-entropy
 # --------------------------------------------------------------------------------------------
 def _gemm(dev, **kw):
     a = _lib.GemmArgs()
@@ -590,7 +590,7 @@ class DecoderWeights:
 
 class _MlmDecoderFn(torch.autograd.Function):
     """logits[n, Vp] = t[n, H] @ E[V, H]^T + bias (BertLMPredictionHead decoder, reference M.py:403-421) — forward,
-    input-gradient and weight-gradient GEMMs all on gemm_tcgen05_kernel; the weight gradient accumulates straight
+    input-gradient and weight-gradient GEMMs all on gemm_wgmma_kernel; the weight gradient accumulates straight
     into the (tied) word-embedding gradient when that buffer exists."""
 
     @staticmethod

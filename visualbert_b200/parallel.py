@@ -4,7 +4,7 @@ per step over a flat fp32 gradient buffer — replacing the reference's single-p
 
 `FlatGradSync` makes every `p.grad` a view into one contiguous buffer, so the collective needs no
 packing copy; `allreduce()` issues a single `torch.distributed.all_reduce` (NCCL over NVLink on the
-B200 box, gloo in the CPU tests) and divides by the world size, i.e. the mean of per-rank mean losses —
+GPU machine, gloo in the CPU tests) and divides by the world size, i.e. the mean of per-rank mean losses —
 the same semantics as the reference's `loss.mean()` over DataParallel replicas (model_wrapper.py:75).
 """
 import torch

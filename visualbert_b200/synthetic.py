@@ -11,7 +11,7 @@ import torch
 CONFIGS = {
     "cfg1": dict(layers=2, hidden=768, heads=12, inter=3072, B=4, V=36, T=20, Dv=2048, head="pretraining"),
     "cfg2": dict(layers=12, hidden=768, heads=12, inter=3072, B=256, V=36, T=128, Dv=2048, head="pretraining"),
-    # configs[2..4] are quoted as GLOBAL batches over 8 data-parallel B200s: `dp` = ranks the batch B is spread over
+    # configs[2..4] are quoted as GLOBAL batches over 8 data-parallel GPUs: `dp` = ranks the batch B is spread over
     "cfg3": dict(layers=12, hidden=768, heads=12, inter=3072, B=512, dp=8, V=36, T=128, Dv=2048, head="vqa"),
     "cfg4": dict(layers=12, hidden=768, heads=12, inter=3072, B=256, dp=8, V=72, T=40, Dv=2048, head="nlvr"),
     "cfg5": dict(layers=24, hidden=1024, heads=16, inter=4096, B=1024, dp=8, V=100, T=256, Dv=2048, head="pretraining"),
