@@ -1,0 +1,347 @@
+"""Every attention kernel against a plain fp64 restatement of the same op, through the C ABI (ctypes).
+
+The library has four attention paths; which one runs depends on the sequence length and on environment switches that
+are read once per process:
+
+    wgmma            S <= 192 (default)                 attn_fwd_wgmma_kernel / attn_bwd_wgmma_kernel
+    head, P/dS smem  S <= 176 with VB_ATTN_HEAD=1       attn_fwd_head_kernel  / attn_bwd_head_ps_kernel
+    head, recompute  193 <= S <= 256 (default), or      attn_fwd_head_kernel  / attn_bwd_head_kernel
+                     VB_ATTN_HEAD=1 with S > 176 or VB_ATTN_BWD_PS=0
+    staged           S > 256 (default), VB_ATTN_STAGED=1  attn_fwd_kernel / attn_bwd_dq_kernel + attn_bwd_dkv_kernel
+
+The parametrized tests below run the shapes of the route selected by the current environment; test_attention_switches
+reruns this file in a subprocess for each switch set. Each case checks ctx, lse, dQ, dK and dV separately against the
+reference, that every output element is written (outputs are pre-filled with NaN), that nothing is read or written
+outside the tensors (they are views inside buffers whose guard bands hold NaN for inputs and a sentinel for outputs),
+and that two identical calls are bit-identical. With dropout, the reference applies the bits the forward stored in the
+keep buffer, so a match also shows that the forward applied exactly the stored bits."""
+import ctypes
+import os
+import re
+import subprocess
+import sys
+
+import pytest
+import torch
+
+pytestmark = pytest.mark.gpu
+
+CTX_TOL = 1.0e-2   # bf16 output rounding (2^-8 relative), relative to max |ref|
+GRAD_TOL = 2.0e-2  # per gradient, relative to max(max |ref|, problem scale), see _check_grads
+LSE_TOL = 2.0e-2   # absolute, natural-log domain
+GUARD_ROWS = 64    # guard rows around every [rows, cols] tensor: whole rows keep the views 16-byte aligned
+GUARD_FLAT = 256   # guard elements around the [B, A, S] fp32 tensors (1 KB)
+GUARD_KEEP = 1024  # guard bytes around the keep buffer
+SENTINEL = -12345.0
+KEEP_SENTINEL = 0xA5
+P_FIRST = 0.1      # dropout of the reference comparisons (quantised to 26/256)
+
+ROUTES = {
+    "default": {},
+    "head": {"VB_ATTN_HEAD": "1"},
+    "head_recompute": {"VB_ATTN_HEAD": "1", "VB_ATTN_BWD_PS": "0"},
+    "staged": {"VB_ATTN_STAGED": "1"},
+}
+KERNELS = {
+    "wgmma": {"attn_fwd_wgmma_kernel", "attn_delta_kernel", "attn_bwd_wgmma_kernel"},
+    "head_ps": {"attn_fwd_head_kernel", "attn_delta_kernel", "attn_bwd_head_ps_kernel"},
+    "head_recompute": {"attn_fwd_head_kernel", "attn_delta_kernel", "attn_bwd_head_kernel"},
+    "staged": {"attn_fwd_kernel", "attn_bwd_dq_kernel", "attn_bwd_dkv_kernel"},
+}
+
+
+def _route():
+    """The switch set of this process, as the library reads it (vb_attention.cu, vb_attention_head.cu)."""
+    def on(k):
+        try:
+            return int(os.environ.get(k, "0")) != 0
+        except ValueError:
+            return False
+    if on("VB_ATTN_STAGED"):
+        return "staged"
+    if on("VB_ATTN_HEAD"):
+        return "head_recompute" if os.environ.get("VB_ATTN_BWD_PS", "").startswith("0") else "head"
+    return "default"
+
+
+def _path(route, S):
+    """The implementation the library picks for sequence length S (16-byte aligned operands)."""
+    if route == "staged" or S > 256:
+        return "staged"
+    if route == "default" and S <= 192:
+        return "wgmma"
+    if route == "head" and S <= 176:  # P and dS of a whole head fit in shared memory up to S = 176
+        return "head_ps"
+    return "head_recompute"
+
+
+# sequence lengths per route: tile edges (1, 63/64/65, 127/128/129, 191/192), the cut-overs 176/177, 192/193 and
+# 256/257, and 513 (staged: stages of 4, 4 and 1 key blocks)
+SEQS = {
+    "default": [1, 2, 17, 63, 64, 65, 100, 127, 128, 129, 164, 191, 192, 193, 200, 255, 256, 257, 320, 356, 513],
+    "head": [1, 17, 64, 65, 128, 129, 176, 177],
+    "head_recompute": [17, 65, 177, 192],
+    "staged": [1, 65, 192],
+}
+# dropout comparisons: a partial and a full last tile per path
+DROP_SEQS = {
+    "default": [65, 128, 192, 200, 256, 257, 320, 356, 513],
+    "head": [65, 128, 176, 177, 192],
+    "head_recompute": [65, 192],
+    "staged": [65, 192],
+}
+# persistent whole-head kernels: B*A = 288 heads, more than twice the SM count, so every CTA walks several heads
+WALK = {"default": [200], "head": [164], "head_recompute": [164], "staged": []}
+# one shape per path for the routing test
+ROUTING_SEQS = {"default": [100, 200, 356], "head": [128, 177], "head_recompute": [65], "staged": [65]}
+
+ROUTE = _route()
+CASES = ([(B, S, A, 0.0) for S in SEQS[ROUTE] for B in (1, 3) for A in (1, 2, 12)]
+         + [(3, S, 12, P_FIRST) for S in DROP_SEQS[ROUTE]]
+         + [(24, S, 12, p) for S in WALK[ROUTE] for p in (0.0, P_FIRST)])
+
+
+def _setup():
+    from visualbert_b200 import _lib
+    return _lib, _lib.lib(), torch.device("cuda:0"), ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
+
+
+def _ptr(t):
+    return ctypes.c_void_p(t.data_ptr()) if t is not None else None
+
+
+class _Guarded:
+    """A tensor of `shape` placed in the middle of a flat buffer with `guard` elements of `fill` on each side."""
+
+    def __init__(self, shape, dtype, guard, fill, dev):
+        n = 1
+        for s in shape:
+            n *= s
+        self.n, self.guard, self.fill = n, guard, fill
+        self.buf = torch.full((n + 2 * guard,), fill, dtype=dtype, device=dev)
+        self.t = self.buf[guard:guard + n].view(shape)
+
+    def guards_intact(self):
+        g = torch.cat([self.buf[:self.guard], self.buf[self.guard + self.n:]])
+        if g.dtype.is_floating_point and self.fill != self.fill:
+            return bool(torch.isnan(g).all())
+        return torch.equal(g, torch.full_like(g, self.fill))
+
+
+def _keep_bits(keep, B, S, A, half=0):
+    """[B*A, S, S] 0/1 keep decisions from the keep buffer: half 0 = rows are queries, half 1 = its transpose."""
+    nkb = (S + 63) // 64
+    words = keep.view(torch.int64).view(2, B * A, nkb * 64, nkb)[half]
+    bits = (words.unsqueeze(-1) >> torch.arange(64, device=keep.device)) & 1
+    return bits.reshape(B * A, nkb * 64, nkb * 64)[:, :S, :S]
+
+
+def _reference(qkv, bias, dctx, keep, B, S, A, p):
+    """softmax(QK^T / 8 + bias) [* keep * 256 / (256 - round(256 p))] V in fp64, gradients by autograd."""
+    H = A * 64
+    x = qkv.double().requires_grad_(True)
+    q, k, v = x.view(B, S, 3, A, 64).permute(2, 0, 3, 1, 4)
+    sc = q @ k.transpose(-1, -2) / 8.0 + bias.double()[:, None, None, :]
+    lse = torch.logsumexp(sc, -1)
+    pr = torch.softmax(sc, -1)
+    if p > 0:
+        n = int(p * 256 + 0.5)
+        pr = pr * _keep_bits(keep, B, S, A).view(B, A, S, S).double() * (256.0 / (256 - n))
+    o = (pr @ v).permute(0, 2, 1, 3).reshape(B * S, H)
+    (g,) = torch.autograd.grad(o, x, dctx.double())
+    return o.detach(), lse.detach(), g
+
+
+def _err(out, ref, scale=0.0):
+    out, ref = out.double(), ref.double()
+    return ((out - ref).abs().max() / max(ref.abs().max().item(), scale, 1e-30)).item()
+
+
+def _inputs(B, S, A, dev, seed, fully_masked=False):
+    """qkv and dO unit normal; ragged key lengths; with `fully_masked`, example 1 has no valid key (additive -10000, not
+    -inf: it attends uniformly over raw scores, M.py:1293)."""
+    g = torch.Generator(device=dev)
+    g.manual_seed(seed)
+    H = A * 64
+    qkv = torch.randn(B * S, 3 * H, device=dev, generator=g).bfloat16()
+    dctx = torch.randn(B * S, H, device=dev, generator=g).bfloat16()
+    lens = torch.randint(max(1, S // 2), S + 1, (B,), device=dev, generator=g)
+    bias = ((torch.arange(S, device=dev)[None, :] >= lens[:, None]).float() * -10000.0)
+    if fully_masked:
+        bias[1] = -10000.0
+    return qkv, bias.contiguous(), dctx
+
+
+def _run(L, _lib, st, qkv, bias, dctx, B, S, A, p, dev, seed=99, stream=5, guarded=True):
+    """One forward + backward through the C ABI. Inputs are copied into NaN-guarded buffers and outputs are NaN-filled
+    views inside sentinel-guarded buffers. Returns {name: _Guarded}."""
+    H = A * 64
+    nan = float("nan")
+    gr, gf = (GUARD_ROWS, GUARD_FLAT) if guarded else (0, 0)
+    T = {
+        "qkv": _Guarded((B * S, 3 * H), torch.bfloat16, gr * 3 * H, nan, dev),
+        "bias": _Guarded((B, S), torch.float32, gf, nan, dev),
+        "dctx": _Guarded((B * S, H), torch.bfloat16, gr * H, nan, dev),
+        "ctx": _Guarded((B * S, H), torch.bfloat16, gr * H, SENTINEL, dev),
+        "lse": _Guarded((B, A, S), torch.float32, gf, SENTINEL, dev),
+        "dqkv": _Guarded((B * S, 3 * H), torch.bfloat16, gr * 3 * H, SENTINEL, dev),
+        "drow": _Guarded((B, A, S), torch.float32, gf, SENTINEL, dev),
+    }
+    T["qkv"].t.copy_(qkv); T["bias"].t.copy_(bias); T["dctx"].t.copy_(dctx)
+    for k in ("ctx", "lse", "dqkv"):
+        T[k].t.fill_(nan)
+    keep = None
+    if p > 0:
+        T["keep"] = _Guarded((int(L.vb_attention_keep_bytes(B, S, A)),), torch.uint8, GUARD_KEEP if guarded else 0,
+                             KEEP_SENTINEL, dev)
+        T["keep"].t.zero_()
+        keep = T["keep"].t
+    args = (ctypes.c_float(p), ctypes.c_uint64(seed), stream, st)
+    P = _ptr
+    _lib.check(L.vb_attention_fwd(P(T["qkv"].t), P(T["bias"].t), P(T["ctx"].t), P(T["lse"].t), P(keep), B, S, A, H, *args),
+               "attn_fwd")
+    _lib.check(L.vb_attention_bwd(P(T["qkv"].t), P(T["bias"].t), P(T["ctx"].t), P(T["lse"].t), P(keep), P(T["dctx"].t),
+                                  P(T["dqkv"].t), P(T["drow"].t), B, S, A, H, *args), "attn_bwd")
+    return T
+
+
+def _check_grads(dqkv, g, H, where):
+    """dQ, dK and dV each against the reference. dV = P^T dO involves no cancellation; dQ and dK go through the softmax
+    Jacobian P (dP - D), whose two terms cancel exactly at S = 1 (dQ = dK = 0) and nearly at S = 2. Their bound is
+    therefore taken against max(max |ref|, max |ref dV| / 4): for S >= 17 max |dQ| and max |dK| are above 0.6 max |dV|
+    for unit-normal inputs, so the floor only acts where the reference itself (nearly) vanishes."""
+    dv_scale = g[:, 2 * H:].abs().max().item()
+    for i, name in enumerate("QKV"):
+        scale = dv_scale / 4 if name != "V" else 0.0
+        e = _err(dqkv[:, i * H:(i + 1) * H], g[:, i * H:(i + 1) * H], scale)
+        assert e < GRAD_TOL, f"{where}: d{name} error {e:.3g}"
+
+
+def _check_case(B, S, A, p, seed, fully_masked):
+    """One forward + backward against the reference, with all checks described in the module docstring."""
+    _lib, L, dev, st = _setup()
+    H = A * 64
+    where = f"{ROUTE}/{_path(ROUTE, S)} B={B} S={S} A={A} p={p}"
+    qkv, bias, dctx = _inputs(B, S, A, dev, seed, fully_masked)
+    T = _run(L, _lib, st, qkv, bias, dctx, B, S, A, p, dev)
+    T2 = _run(L, _lib, st, qkv, bias, dctx, B, S, A, p, dev, guarded=False)
+    torch.cuda.synchronize()
+    ctx, lse, dqkv = T["ctx"].t, T["lse"].t, T["dqkv"].t
+
+    # every element written, nothing outside the tensors read (NaN guards) or written (sentinels)
+    for k in ("ctx", "lse", "dqkv"):
+        assert torch.isfinite(T[k].t).all(), f"{where}: {k} has unwritten (NaN) elements"
+    for k, gt in T.items():
+        assert gt.guards_intact(), f"{where}: guard band of {k} changed"
+    # deterministic: no atomics, so a second call gives the same bits
+    for k in ("ctx", "lse", "dqkv") + (("keep",) if p > 0 else ()):
+        assert torch.equal(T[k].t, T2[k].t), f"{where}: {k} differs between two identical calls"
+
+    keep = T["keep"].t if p > 0 else None
+    o, lse_ref, g = _reference(qkv, bias, dctx, keep, B, S, A, p)
+    e = _err(ctx, o)
+    assert e < CTX_TOL, f"{where}: ctx error {e:.3g}"
+    e = (lse.double() - lse_ref).abs().max().item()
+    assert e < LSE_TOL, f"{where}: lse error {e:.3g}"
+    _check_grads(dqkv, g, H, where)
+
+    if p > 0:
+        n = int(p * 256 + 0.5)
+        q = n / 256
+        bits = _keep_bits(keep, B, S, A)
+        if _path(ROUTE, S) != "staged":  # the mask kernel also writes the transpose (rows = keys); the staged path does not
+            assert torch.equal(bits, _keep_bits(keep, B, S, A, half=1).transpose(1, 2)), f"{where}: transposed keep bits differ"
+        assert abs(bits.float().mean().item() - (1 - q)) < 5e-3, f"{where}: keep rate {bits.float().mean().item():.4f}"
+        for kb in range((S + 63) // 64):  # per 64-key block: 6 standard deviations of a binomial rate
+            blk = bits[:, :, kb * 64:(kb + 1) * 64].float()
+            tol = 6 * (q * (1 - q) / blk.numel()) ** 0.5
+            assert abs(blk.mean().item() - (1 - q)) < tol, f"{where}: keep rate {blk.mean().item():.4f} in key block {kb}"
+        o0, _, _ = _reference(qkv, bias, dctx, None, B, S, A, 0.0)
+        assert _err(ctx, o0) > 0.05, f"{where}: dropout did not change the output"
+        # E[dropout(P)] = P: averaged over many rows the output stays close to the no-dropout one
+        assert abs(ctx.double().mean().item() - o0.mean().item()) < 5e-3, f"{where}: mean output moved"
+        # for a fixed mask the output is linear in V: <dO, O> = <dV, V>
+        lhs = (dctx.double() * ctx.double()).sum().item()
+        rhs = (dqkv[:, 2 * H:].double() * qkv[:, 2 * H:].double()).sum().item()
+        assert abs(lhs - rhs) < 2e-2 * max(abs(lhs), 1.0) + 2.0, f"{where}: <dO, O> = {lhs} but <dV, V> = {rhs}"
+
+
+
+@pytest.mark.parametrize("B,S,A,p", CASES)
+def test_attention_matches_reference(B, S, A, p):
+    _check_case(B, S, A, p, seed=1000 * S + 10 * B + A, fully_masked=B == 3)
+
+
+def test_attention_fully_masked_example_stays_finite():
+    """An example whose mask is all zero gets the additive -10000 on every key (not -inf), so it attends uniformly over
+    its raw scores (M.py:1293): its outputs and gradients stay finite and match the reference."""
+    _check_case(2, 70, 1, 0.0, seed=6, fully_masked=True)
+
+
+def test_attention_dropout_consistent_between_fwd_and_bwd():
+    """p = 0.2 (quantised to 51/256): the backward applies the bits the forward stored, so dQ, dK and dV match the
+    reference built from those bits; the output is linear in V for a fixed mask (<dO, O> = <dV, V>) and its mean is
+    preserved."""
+    _check_case(2, 100, 2, 0.2, seed=7, fully_masked=False)
+
+@pytest.mark.parametrize("S", SEQS[ROUTE])
+def test_attention_dropout_words_are_distinct(S):
+    """At p = 0.5 a keep decision is the top bit of an 8-bit hash value, so each stored 64-bit word of a valid row
+    (query < S, every key block, all 64 bits) is 64 independent random bits: two of them are equal with probability
+    2^-64. A repeated word means a reused hash counter, i.e. masks that are not independent across rows or heads."""
+    _lib, L, dev, st = _setup()
+    B, A = 2, 2
+    H = A * 64
+    qkv, bias, _ = _inputs(B, S, A, dev, seed=S)
+    keep = torch.zeros(int(L.vb_attention_keep_bytes(B, S, A)), device=dev, dtype=torch.uint8)
+    ctx = torch.empty(B * S, H, device=dev, dtype=torch.bfloat16)
+    lse = torch.empty(B, A, S, device=dev)
+    P = _ptr
+    _lib.check(L.vb_attention_fwd(P(qkv), P(bias), P(ctx), P(lse), P(keep), B, S, A, H, ctypes.c_float(0.5), ctypes.c_uint64(7),
+                                  3, st), "attn_fwd")
+    torch.cuda.synchronize()
+    nkb = (S + 63) // 64
+    words = keep.view(torch.int64).view(2, B * A, nkb * 64, nkb)[0, :, :S, :].reshape(-1)
+    dup = words.numel() - torch.unique(words).numel()
+    assert dup == 0, f"{ROUTE}/{_path(ROUTE, S)} S={S}: {dup} repeated keep words of {words.numel()}"
+    bits = _keep_bits(keep, B, S, A).float()
+    for kb in range(nkb):
+        blk = bits[:, :, kb * 64:(kb + 1) * 64]
+        assert abs(blk.mean().item() - 0.5) < 6 * (0.25 / blk.numel()) ** 0.5, f"S={S}: keep rate {blk.mean().item():.4f} in block {kb}"
+
+
+@pytest.mark.parametrize("S", ROUTING_SEQS[ROUTE])
+def test_attention_routing(S):
+    """The kernels one forward + backward launches are those of the expected path: a change to the dispatch must not send
+    every case silently to one implementation."""
+    from torch.profiler import ProfilerActivity, profile
+    _lib, L, dev, st = _setup()
+    B, A, p = 2, 2, P_FIRST
+    qkv, bias, dctx = _inputs(B, S, A, dev, seed=S)
+    _run(L, _lib, st, qkv, bias, dctx, B, S, A, p, dev)   # first call: one-time setup outside the profile
+    torch.cuda.synchronize()
+    with profile(activities=[ProfilerActivity.CUDA]) as prof:
+        _run(L, _lib, st, qkv, bias, dctx, B, S, A, p, dev)
+        torch.cuda.synchronize()
+    names = [e.name for e in prof.events() if e.device_type == torch.autograd.DeviceType.CUDA]
+    if not names:
+        pytest.skip("torch.profiler recorded no device kernels")
+    ran = {m.group(1) for n in names for m in [re.search(r"\b(attn_\w+_kernel)\b", n)] if m}
+    path = _path(ROUTE, S)
+    want = KERNELS[path] | ({"attn_keep_mask_kernel"} if path != "staged" else set())
+    assert ran == want, f"{ROUTE} S={S}: expected {sorted(want)}, ran {sorted(ran)}"
+
+
+@pytest.mark.parametrize("route", [r for r in ROUTES if r != "default"])
+def test_attention_switches(route):
+    """The whole-head mma.sync kernels (with their P/dS-in-shared-memory backward and with the recompute backward) and the
+    staged kernels, forced through the library's environment switches, must pass the same checks: the switches are read
+    once per process, so this file reruns in a subprocess per switch set."""
+    if ROUTE != "default":
+        pytest.skip("already running under a switch set")
+    env = {k: v for k, v in os.environ.items() if k not in ("VB_ATTN_HEAD", "VB_ATTN_BWD_PS", "VB_ATTN_STAGED")}
+    env.update(ROUTES[route])
+    r = subprocess.run([sys.executable, "-m", "pytest", os.path.abspath(__file__), "-m", "gpu", "-q", "-p", "no:cacheprovider",
+                        "-k", "not test_attention_switches"], env=env, capture_output=True, text=True, timeout=900)
+    assert r.returncode == 0, r.stdout[-3000:] + r.stderr[-2000:]
+    assert " passed" in r.stdout and " skipped" not in r.stdout.splitlines()[-1], r.stdout[-2000:]

@@ -189,116 +189,6 @@ def test_layernorm_fwd_bwd(rows, H):
     assert _rel(dbias, dx.float().sum(0)) < 2e-3
 
 
-def _attn_ref(qkv, bias, B, S, A, H):
-    q, k, v = qkv.float().view(B, S, 3, A, 64).permute(2, 0, 3, 1, 4)
-    sc = q @ k.transpose(-1, -2) / 8.0 + bias[:, None, None, :]
-    p = torch.softmax(sc, -1)
-    return (p @ v).permute(0, 2, 1, 3).reshape(B * S, H), torch.logsumexp(sc, -1)
-
-
-@pytest.mark.parametrize("B,S,A", [(3, 56, 2), (2, 164, 12), (2, 200, 3), (1, 64, 1), (2, 356, 2)])
-def test_attention_fwd_bwd(B, S, A):
-    _lib, L, dev, st = _setup()
-    torch.manual_seed(5)
-    H = A * 64
-    qkv = torch.randn(B * S, 3 * H, device=dev).bfloat16()
-    lens = torch.randint(S // 2, S + 1, (B,), device=dev)
-    mask = (torch.arange(S, device=dev)[None, :] < lens[:, None]).float()
-    bias = ((1 - mask) * -10000.0).contiguous()
-    ctx = torch.empty(B * S, H, device=dev, dtype=torch.bfloat16); lse = torch.empty(B, A, S, device=dev)
-    P = lambda t: ctypes.c_void_p(t.data_ptr())
-    _lib.check(L.vb_attention_fwd(P(qkv), P(bias), P(ctx), P(lse), None, B, S, A, H, ctypes.c_float(0.0), ctypes.c_uint64(0), 0, st), "attn_fwd")
-    qr = qkv.float().requires_grad_(True)
-    ref, lse_ref = _attn_ref(qr, bias, B, S, A, H)
-    torch.cuda.synchronize()
-    assert _rel(ctx, ref) < BF16_TOL
-    assert (lse - lse_ref).abs().max().item() < 2e-2
-    dctx = torch.randn(B * S, H, device=dev).bfloat16()
-    ref.backward(dctx.float())
-    dqkv = torch.empty_like(qkv); drow = torch.empty(B, A, S, device=dev)
-    _lib.check(L.vb_attention_bwd(P(qkv), P(bias), P(ctx), P(lse), None, P(dctx), P(dqkv), P(drow), B, S, A, H,
-                                  ctypes.c_float(0.0), ctypes.c_uint64(0), 0, st), "attn_bwd")
-    torch.cuda.synchronize()
-    g = qr.grad
-    for i, name in enumerate("qkv"):
-        r = _rel(dqkv[:, i * H:(i + 1) * H], g[:, i * H:(i + 1) * H])
-        assert r < 2e-2, f"d{name}: {r}"
-
-
-def test_attention_fully_masked_example_stays_finite():
-    """additive -10000 (not -inf): an example whose mask is all zero attends uniformly over raw scores (M.py:1293)."""
-    _lib, L, dev, st = _setup()
-    B, S, A = 2, 70, 1
-    H = 64
-    torch.manual_seed(6)
-    qkv = torch.randn(B * S, 3 * H, device=dev).bfloat16()
-    bias = torch.zeros(B, S, device=dev); bias[1] = -10000.0
-    ctx = torch.empty(B * S, H, device=dev, dtype=torch.bfloat16); lse = torch.empty(B, A, S, device=dev)
-    P = lambda t: ctypes.c_void_p(t.data_ptr())
-    _lib.check(L.vb_attention_fwd(P(qkv), P(bias), P(ctx), P(lse), None, B, S, A, H, ctypes.c_float(0.0), ctypes.c_uint64(0), 0, st), "attn_fwd")
-    ref, _ = _attn_ref(qkv, bias, B, S, A, H)
-    torch.cuda.synchronize()
-    assert _rel(ctx, ref) < BF16_TOL
-
-
-def test_attention_dropout_consistent_between_fwd_and_bwd():
-    """With dropout the forward is linear in V for a fixed mask: finite-difference-free check of dV via <dO, O>."""
-    _lib, L, dev, st = _setup()
-    B, S, A = 2, 100, 2
-    H = A * 64
-    torch.manual_seed(7)
-    qkv = torch.randn(B * S, 3 * H, device=dev).bfloat16()
-    bias = torch.zeros(B, S, device=dev)
-    P = lambda t: ctypes.c_void_p(t.data_ptr())
-    ctx = torch.empty(B * S, H, device=dev, dtype=torch.bfloat16); lse = torch.empty(B, A, S, device=dev)
-    args = (ctypes.c_float(0.2), ctypes.c_uint64(99), 5, st)
-    L.vb_attention_keep_bytes.restype = ctypes.c_int64
-    keep = torch.zeros(int(L.vb_attention_keep_bytes(B, S, A)), device=dev, dtype=torch.uint8)
-    keep2 = torch.zeros_like(keep)
-    _lib.check(L.vb_attention_fwd(P(qkv), P(bias), P(ctx), P(lse), P(keep), B, S, A, H, *args), "attn_fwd")
-    ctx2 = torch.empty_like(ctx)
-    _lib.check(L.vb_attention_fwd(P(qkv), P(bias), P(ctx2), P(lse), P(keep2), B, S, A, H, *args), "attn_fwd")
-    ref, _ = _attn_ref(qkv, bias, B, S, A, H)
-    dctx = torch.randn(B * S, H, device=dev).bfloat16()
-    dqkv = torch.empty_like(qkv); drow = torch.empty(B, A, S, device=dev)
-    _lib.check(L.vb_attention_bwd(P(qkv), P(bias), P(ctx), P(lse), P(keep), P(dctx), P(dqkv), P(drow), B, S, A, H, *args), "attn_bwd")
-    torch.cuda.synchronize()
-    assert torch.equal(ctx, ctx2) and torch.equal(keep, keep2)
-    # stored keep-mask: valid (query < S, key < S) bits are ~80 % ones for p = 0.2 (quantised to 51/256)
-    nkb = (S + 63) // 64
-    both = keep.view(torch.int64).view(2, B * A, nkb * 64, nkb)   # [0]: rows = queries, [1]: the transpose (rows = keys)
-    unpack = lambda w: ((w.unsqueeze(-1) >> torch.arange(64, device=dev)) & 1).reshape(B * A, nkb * 64, nkb * 64)
-    bits, bits_t = unpack(both[0]), unpack(both[1])
-    import os
-    if os.environ.get("VB_ATTN_STAGED") != "1":  # the staged kernels (seq > 256) draw their own bits, query-major only
-        assert torch.equal(bits[:, :S, :S], bits_t[:, :S, :S].transpose(1, 2))
-    bits = bits[:, :S, :S]
-    assert abs(bits.float().mean().item() - (1 - 51 / 256)) < 5e-3
-    assert _rel(ctx, ref) > 0.05  # dropout really changed the output
-    # O is linear in V: sum(dO * O) == sum(dV * V)
-    lhs = (dctx.float() * ctx.float()).sum().item()
-    rhs = (dqkv[:, 2 * H:].float() * qkv[:, 2 * H:].float()).sum().item()
-    assert abs(lhs - rhs) < 2e-2 * max(abs(lhs), 1.0) + 2.0
-    # mean over many rows: E[dropout(P)] = P, so the average output stays close to the no-dropout one
-    assert abs(ctx.float().mean().item() - ref.mean().item()) < 5e-3
-
-
-@pytest.mark.parametrize("impl", ["head", "staged", "head_recompute"])
-def test_attention_alternative_implementations(impl):
-    """The whole-head mma.sync kernels (the fallback of the default wgmma kernels; `head_recompute`: their backward variant
-    that recomputes P instead of keeping it in shared memory) and the generic staged kernels must pass the same checks.
-    They are forced per process through the library's environment switches, so each runs in a subprocess."""
-    import os, subprocess, sys
-    env = dict(os.environ)
-    env.update({"head": {"VB_ATTN_HEAD": "1"}, "staged": {"VB_ATTN_STAGED": "1"},
-                "head_recompute": {"VB_ATTN_HEAD": "1", "VB_ATTN_BWD_PS": "0"}}[impl])
-    root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-    r = subprocess.run([sys.executable, "-m", "pytest", os.path.join(root, "tests", "test_kernels_gpu.py"), "-m", "gpu", "-q",
-                        "-k", "attention_fwd_bwd or attention_dropout or attention_fully"], env=env, capture_output=True, text=True,
-                       timeout=600)
-    assert r.returncode == 0, r.stdout[-2000:] + r.stderr[-2000:]
-
-
 @pytest.mark.parametrize("n,V", [(300, 30522), (77, 1000), (5, 512)])
 def test_mlm_decoder_and_fused_cross_entropy(n, V):
     """ops.mlm_decoder + ops.cross_entropy_rows against F.linear + F.cross_entropy (fp32) incl. gradients."""

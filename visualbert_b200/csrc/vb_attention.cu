@@ -129,8 +129,8 @@ attn_fwd_kernel(const AttnParams p, const int nsub) {
                 }
                 if (p.drop_scale != 0.f) {
                     const int qa = qrow0 + mt * 16 + g, qc = qa + 8;
-                    const uint32_t ka_bits = attn_keep16(p.drop_seed, bh, qa, kb, t, S, p.drop_thresh16);
-                    const uint32_t kc_bits = attn_keep16(p.drop_seed, bh, qc, kb, t, S, p.drop_thresh16);
+                    const uint32_t ka_bits = attn_keep16(p.drop_seed, bh, qa, kb, t, nkb, p.drop_thresh16);
+                    const uint32_t kc_bits = attn_keep16(p.drop_seed, bh, qc, kb, t, nkb, p.drop_thresh16);
 #pragma unroll
                     for (int nt = 0; nt < 8; ++nt) {
                         s[mt][nt][0] = ((ka_bits >> (2 * nt)) & 1u) ? s[mt][nt][0] * p.drop_scale : 0.f;
@@ -521,6 +521,9 @@ int attn_fwd(const void* qkv, const float* mask_bias, void* ctx, float* lse, voi
     dim3 grid((S + kBlk - 1) / kBlk, A, B);
     if (wgmma_path(p)) return attn_fwd_wgmma(p, st, mask_ready);
     if (head_path(S)) return attn_fwd_head(p, static_cast<int>(grid.x), st, mask_ready);
+    const long long nkb = grid.x;
+    VB_REQUIRE(p.drop_scale == 0.f || static_cast<long long>(B) * A * (nkb * kBlk) * nkb * 16 < (1LL << 32),
+               "attention dropout: mask counter space exceeded (B*A*S too large)");
     const int nsub = static_cast<int>(grid.x) < kMaxSub ? static_cast<int>(grid.x) : kMaxSub;
     const int smem = (1 + 2 * nsub) * kTileBytes;
     static int configured[kMaxDevices] = {0};

@@ -218,10 +218,14 @@ __device__ __forceinline__ void zero_acc(float (&c)[8][4]) {
 // kernels read the bits back instead of re-hashing — the kernels are instruction-issue bound and the per-element
 // hashing was ~45 % of their instruction count. The drop probability is quantised to round(p*256)/256
 // (0.1 -> 26/256) and survivors are scaled by 256/(256 - that), so E[dropout(P)] = P exactly.
-// keep8x2: for one query row, the 16 elements a thread owns in a 64-key block (keys nt*8 + 2t + {0,1}).
-__device__ __forceinline__ uint32_t attn_keep16(unsigned seed, unsigned bh, int q, int kb, int t, int S, unsigned thresh8) {
-    const unsigned base = (((bh * static_cast<unsigned>(S) + static_cast<unsigned>(q)) << 6) + (static_cast<unsigned>(kb) << 4) +
-                           (static_cast<unsigned>(t) << 2));
+// attn_keep16 (staged kernels): for one query row, the 16 elements a thread owns in a 64-key block (keys nt*8 + 2t + {0,1}).
+// Hash counters: 16 w + 4 t + j (j < 4), where w = (bh * nkb*64 + q) * nkb + kb is the index of the 64-bit keep word of
+// (query row q, key block kb) in the mask buffer. Every (bh, q, kb, t, j) with q < nkb*64 therefore gets its own counter, as
+// long as B*A * nkb*64 * nkb * 16 < 2^32 (checked on the host), and no two keep words of a call share a random bit.
+__device__ __forceinline__ uint32_t attn_keep16(unsigned seed, unsigned bh, int q, int kb, int t, int nkb, unsigned thresh8) {
+    const unsigned np64 = static_cast<unsigned>(nkb) * kBlk;
+    const unsigned w = (bh * np64 + static_cast<unsigned>(q)) * static_cast<unsigned>(nkb) + static_cast<unsigned>(kb);
+    const unsigned base = (w << 4) + (static_cast<unsigned>(t) << 2);
     uint32_t bits = 0;
 #pragma unroll
     for (int j = 0; j < 4; ++j) {  // hash j covers n-tiles 2j and 2j+1
