@@ -23,7 +23,7 @@
 extern "C" {
 #endif
 
-#define VB_ABI_VERSION 2
+#define VB_ABI_VERSION 3
 
 /* ---- library ---------------------------------------------------------------------------- */
 int vb_abi_version(void);
@@ -115,6 +115,21 @@ int vb_attention_fwd(const void* qkv, const float* mask_bias, void* ctx, float* 
 int vb_attention_bwd(const void* qkv, const float* mask_bias, const void* ctx, const float* lse, const void* keep_mask,
                      const void* dctx, void* dqkv, float* drow, int32_t batch, int32_t seq, int32_t heads,
                      int32_t hidden, float dropout_p, uint64_t dropout_seed, uint32_t dropout_stream, void* stream);
+/* Variable-length ("unpadded") attention: `batch` sequences packed without padding. qkv bf16 [total, 3*hidden], sequence b
+ * owns rows [cu_seqlens[b], cu_seqlens[b+1]); cu_seqlens is int32 [batch + 1] in DEVICE memory; max_seq >= every length.
+ * ctx bf16 [total, hidden], dqkv bf16 [total, 3*hidden], lse and drow fp32 [heads, total]; keep_mask as for the dense call
+ * with seq = max_seq (vb_attention_keep_bytes(batch, max_seq, heads)). There is no mask: every row of a sequence is a valid
+ * key. Only rows inside [cu[b], cu[b] + len_b) are written. The route (wgmma / whole-head / staged) and its environment
+ * switches are chosen from max_seq as the dense call chooses them from seq.
+ * Caller contract (not checked, that would need a host synchronisation): cu_seqlens is non-decreasing from 0 to at most total
+ * and no length exceeds max_seq. The kernels clamp every length to [0, max_seq] and every row range to [0, total), so a bad
+ * table gives wrong values but no access outside the tensors. */
+int vb_attention_fwd_varlen(const void* qkv, const int32_t* cu_seqlens, void* ctx, float* lse, void* keep_mask, int32_t batch,
+                            int32_t max_seq, int32_t total, int32_t heads, int32_t hidden, float dropout_p, uint64_t dropout_seed,
+                            uint32_t dropout_stream, void* stream);
+int vb_attention_bwd_varlen(const void* qkv, const int32_t* cu_seqlens, const void* ctx, const float* lse, const void* keep_mask,
+                            const void* dctx, void* dqkv, float* drow, int32_t batch, int32_t max_seq, int32_t total, int32_t heads,
+                            int32_t hidden, float dropout_p, uint64_t dropout_seed, uint32_t dropout_stream, void* stream);
 
 /* ---- helpers ----------------------------------------------------------------------------- */
 /* (1 - cat(input_mask, image_mask)) * -10000 -> fp32 [batch, text+regions]  (M.py:1417, 1286-1294);
@@ -224,6 +239,18 @@ int vb_encoder_fwd(const vb_layer_desc* descs, int32_t n_layers, const void* x_i
 /* dy: gradient w.r.t. the LAST layer's output; dx: gradient w.r.t. x_in; grads: HOST array [n_layers]. */
 int vb_encoder_bwd(const vb_layer_desc* descs, int32_t n_layers, const void* x_in, void* arena, const void* dy, void* dx,
                    const vb_layer_grads* grads, const vb_layer_scratch* scratch, void* stream);
+/* Variable-length ("unpadded") encoder: the same calls over `total` packed rows (see vb_attention_fwd_varlen for cu_seqlens and
+ * its caller contract). descs[l].batch is the number of sequences and descs[l].seq the longest length (max_seq); mask_bias is
+ * ignored and may be NULL. x_in, dy, dx and every row-sized arena / scratch buffer have `total` rows; lse and scratch.drow are
+ * fp32 [heads, total]; the keep bits are laid out for (batch, max_seq). The layout returns -1 on a bad shape. total must be
+ * > 0 for the forward and backward. */
+int64_t vb_encoder_arena_layout_varlen(int32_t batch, int32_t max_seq, int32_t total, int32_t hidden, int32_t heads, int32_t inter,
+                                       int32_t attn_dropout_on, int64_t* offsets /* [VB_ENCODER_ARENA_BUFFERS] */);
+int vb_encoder_fwd_varlen(const vb_layer_desc* descs, int32_t n_layers, const int32_t* cu_seqlens, int32_t total, const void* x_in,
+                          void* arena, void* stream);
+int vb_encoder_bwd_varlen(const vb_layer_desc* descs, int32_t n_layers, const int32_t* cu_seqlens, int32_t total, const void* x_in,
+                          void* arena, const void* dy, void* dx, const vb_layer_grads* grads, const vb_layer_scratch* scratch,
+                          void* stream);
 
 /* ---- BertEmbeddingsWithVisualEmbedding (M.py:1169-1257) ----------------------------------- */
 typedef struct {

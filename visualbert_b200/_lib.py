@@ -10,7 +10,7 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 # VB_LIB_PATH: load another build of the same library (A/B timing of kernel variants on one GPU, scripts/build_variant.sh)
 LIB_PATH = os.environ.get("VB_LIB_PATH") or os.path.join(_HERE, "lib", "libvbert_b200.so")
 
-ABI_VERSION = 2   # == VB_ABI_VERSION of include/vbert_b200.h (tests/test_abi.py keeps the two in step)
+ABI_VERSION = 3   # == VB_ABI_VERSION of include/vbert_b200.h (tests/test_abi.py keeps the two in step)
 VB_EPI_NONE, VB_EPI_GELU, VB_EPI_DGELU = 0, 1, 2
 
 c_void_p, c_int, c_i64, c_f32, c_u64, c_u32 = (
@@ -78,6 +78,8 @@ EXPORTS = [
     "vb_attention_keep_bytes", "vb_attention_fwd", "vb_attention_bwd", "vb_mask_bias", "vb_cast_f32_to_bf16", "vb_cast_bf16_to_f32",
     "vb_colsum_bf16", "vb_cross_entropy_fwd", "vb_cross_entropy_bwd", "vb_layer_fwd", "vb_layer_bwd", "vb_embed_fwd", "vb_embed_bwd",
     "vb_bert_adam_step", "vb_cast_multi", "vb_encoder_arena_layout", "vb_encoder_fwd", "vb_encoder_bwd",
+    "vb_attention_fwd_varlen", "vb_attention_bwd_varlen", "vb_encoder_arena_layout_varlen", "vb_encoder_fwd_varlen",
+    "vb_encoder_bwd_varlen",
 ]
 VB_ENCODER_ARENA_BUFFERS = 14
 ARENA_NAMES = ("qkv", "ctx", "lse", "pre1", "mean1", "rstd1", "x1", "u", "g", "pre2", "mean2", "rstd2", "keep_mask", "y")
@@ -104,6 +106,13 @@ def lib():
         h.vb_abi_version.restype = ctypes.c_int
         h.vb_attention_keep_bytes.restype = ctypes.c_int64
         h.vb_encoder_arena_layout.restype = ctypes.c_int64
+        h.vb_encoder_arena_layout_varlen.restype = ctypes.c_int64
+        _P, _I, _F, _U64, _U32 = c_void_p, c_int, c_f32, c_u64, c_u32
+        h.vb_attention_fwd_varlen.argtypes = [_P, _P, _P, _P, _P, _I, _I, _I, _I, _I, _F, _U64, _U32, _P]
+        h.vb_attention_bwd_varlen.argtypes = [_P, _P, _P, _P, _P, _P, _P, _P, _I, _I, _I, _I, _I, _F, _U64, _U32, _P]
+        h.vb_encoder_arena_layout_varlen.argtypes = [_I, _I, _I, _I, _I, _I, _I, _P]
+        h.vb_encoder_fwd_varlen.argtypes = [_P, _I, _P, _I, _P, _P, _P]
+        h.vb_encoder_bwd_varlen.argtypes = [_P, _I, _P, _I, _P, _P, _P, _P, _P, _P, _P]
         _lib = h
     return _lib
 

@@ -53,19 +53,32 @@ static vb_gemm_args wgrad_args(const void* dY, const void* X, float* dW, int M, 
     return a;
 }
 
-static int check_layer(const vb_layer_desc* d) {
+// The rows a layer call works on. Dense: batch * seq rows, sequence b at rows b * seq. Variable-length ("unpadded"): `total`
+// packed rows, sequence b at rows [cu_seqlens[b], cu_seqlens[b + 1]) (device memory), at most seq (the longest) rows each;
+// the attention runs through the varlen kernels, everything else is row-local and only sees M = total.
+struct LayerRows {
+    const int* cu_seqlens;  // nullptr: dense
+    int total;
+};
+static const LayerRows kDenseRows = {nullptr, 0};
+
+static int check_layer(const vb_layer_desc* d, const LayerRows& r) {
     VB_REQUIRE(d != nullptr, "layer: null descriptor");
     VB_REQUIRE(d->batch > 0 && d->seq > 0, "layer: empty batch");
     VB_REQUIRE(d->hidden == d->heads * 64, "layer: hidden (%d) must equal heads (%d) * 64", d->hidden, d->heads);
     VB_REQUIRE(d->hidden % 16 == 0 && d->inter % 16 == 0, "layer: hidden/intermediate must be multiples of 16");
-    VB_REQUIRE(d->w_qkv && d->w_attn_out && d->w_inter && d->w_out && d->mask_bias, "layer: null weight pointer");
+    VB_REQUIRE(d->w_qkv && d->w_attn_out && d->w_inter && d->w_out, "layer: null weight pointer");
+    VB_REQUIRE(r.cu_seqlens != nullptr || d->mask_bias != nullptr, "layer: null mask_bias");
+    VB_REQUIRE(r.cu_seqlens == nullptr || r.total > 0, "layer: varlen call without rows (total = %d)", r.total);
     return 0;
 }
 
-int layer_fwd(const vb_layer_desc* d, const void* x_in, void* x_out, const vb_layer_acts* s, cudaStream_t st) {
-    VB_TRY(check_layer(d));
+int layer_fwd(const vb_layer_desc* d, const void* x_in, void* x_out, const vb_layer_acts* s, cudaStream_t st,
+              const LayerRows& rows = kDenseRows) {
+    VB_TRY(check_layer(d, rows));
     VB_REQUIRE(x_in && x_out && s, "layer_fwd: null pointer");
-    const int M = d->batch * d->seq, H = d->hidden, I = d->inter;
+    const bool vl = rows.cu_seqlens != nullptr;
+    const int M = vl ? rows.total : d->batch * d->seq, H = d->hidden, I = d->inter;
     vb_gemm_args a = fwd_args(x_in, d->w_qkv, s->qkv, M, 3 * H, H);
     a.bias = d->b_qkv;
     // the attention-dropout bits depend on (seed, layer) only: they are drawn on a side stream UNDER the QKV GEMM (attn_mask_async)
@@ -83,8 +96,12 @@ int layer_fwd(const vb_layer_desc* d, const void* x_in, void* x_out, const vb_la
                                      drop_stream(d->layer_index, kSiteAttnProbs), before_qkv[dev], st);
         if (mask_ready < 0) return 2;
     }
-    VB_TRY(attn_fwd(s->qkv, d->mask_bias, s->ctx, s->lse, s->keep_mask, d->batch, d->seq, d->heads, H, d->attn_dropout, d->seed,
-                    drop_stream(d->layer_index, kSiteAttnProbs), st, mask_ready == 1));
+    if (vl)
+        VB_TRY(attn_fwd_varlen(s->qkv, rows.cu_seqlens, s->ctx, s->lse, s->keep_mask, d->batch, d->seq, rows.total, d->heads, H,
+                               d->attn_dropout, d->seed, drop_stream(d->layer_index, kSiteAttnProbs), st, mask_ready == 1));
+    else
+        VB_TRY(attn_fwd(s->qkv, d->mask_bias, s->ctx, s->lse, s->keep_mask, d->batch, d->seq, d->heads, H, d->attn_dropout, d->seed,
+                        drop_stream(d->layer_index, kSiteAttnProbs), st, mask_ready == 1));
     a = fwd_args(s->ctx, d->w_attn_out, s->pre1, M, H, H);
     a.bias = d->b_attn_out; a.addend = x_in; a.ld_add = H;
     a.dropout_p = d->hidden_dropout; a.dropout_seed = d->seed; a.dropout_stream = drop_stream(d->layer_index, kSiteAttnOut);
@@ -103,10 +120,11 @@ int layer_fwd(const vb_layer_desc* d, const void* x_in, void* x_out, const vb_la
 }
 
 int layer_bwd(const vb_layer_desc* d, const void* x_in, const vb_layer_acts* s, const void* dy, void* dx,
-              const vb_layer_grads* g, const vb_layer_scratch* w, cudaStream_t st) {
-    VB_TRY(check_layer(d));
+              const vb_layer_grads* g, const vb_layer_scratch* w, cudaStream_t st, const LayerRows& rows = kDenseRows) {
+    VB_TRY(check_layer(d, rows));
     VB_REQUIRE(x_in && s && dy && dx && g && w, "layer_bwd: null pointer");
-    const int M = d->batch * d->seq, H = d->hidden, I = d->inter;
+    const bool vl = rows.cu_seqlens != nullptr;
+    const int M = vl ? rows.total : d->batch * d->seq, H = d->hidden, I = d->inter;
     const bool hd = d->hidden_dropout > 0.f;
     VB_REQUIRE(!hd || w->d_pre_drop, "layer_bwd: d_pre_drop scratch required when hidden_dropout > 0");
     void* dpm = hd ? w->d_pre_drop : w->d_pre;  // gradient entering the Linear in front of each LayerNorm
@@ -135,11 +153,17 @@ int layer_bwd(const vb_layer_desc* d, const void* x_in, const vb_layer_acts* s, 
     // D = rowsum(dO * O) of the attention backward falls out of this GEMM's epilogue (a thread holds two whole heads of a row)
     const bool fused_delta = gemm_delta_ok(M, H) && w->drow != nullptr &&
                              attn_bwd_takes_delta(s->qkv, w->d_ctx, w->d_big, d->batch, d->seq, d->heads, H);
-    if (fused_delta) { a.delta_ctx = s->ctx; a.delta_out = w->drow; a.delta_seq = d->seq; }
+    // (varlen: drow is [heads, total], i.e. delta_out[0][h][row] with delta_seq = total)
+    if (fused_delta) { a.delta_ctx = s->ctx; a.delta_out = w->drow; a.delta_seq = vl ? rows.total : d->seq; }
     VB_TRY(gemm(a, st));
     // ---- BertSelfAttention ----
-    VB_TRY(attn_bwd(s->qkv, d->mask_bias, s->ctx, s->lse, s->keep_mask, w->d_ctx, w->d_big, w->drow, d->batch, d->seq, d->heads, H,
-                    d->attn_dropout, d->seed, drop_stream(d->layer_index, kSiteAttnProbs), st, fused_delta));
+    if (vl)
+        VB_TRY(attn_bwd_varlen(s->qkv, rows.cu_seqlens, s->ctx, s->lse, s->keep_mask, w->d_ctx, w->d_big, w->drow, d->batch, d->seq,
+                               rows.total, d->heads, H, d->attn_dropout, d->seed, drop_stream(d->layer_index, kSiteAttnProbs), st,
+                               fused_delta));
+    else
+        VB_TRY(attn_bwd(s->qkv, d->mask_bias, s->ctx, s->lse, s->keep_mask, w->d_ctx, w->d_big, w->drow, d->batch, d->seq, d->heads, H,
+                        d->attn_dropout, d->seed, drop_stream(d->layer_index, kSiteAttnProbs), st, fused_delta));
     VB_TRY(colsum(w->d_big, 3 * H, g->db_qkv, M, 3 * H, st));
     VB_TRY(gemm(wgrad_args(w->d_big, x_in, g->dw_qkv, M, 3 * H, H), st));
     a = dgrad_args(w->d_big, d->w_qkv, dx, M, 3 * H, H);
@@ -151,10 +175,12 @@ int layer_bwd(const vb_layer_desc* d, const void* x_in, const vb_layer_acts* s, 
 // ---- whole-encoder entry points: one arena, one call (see include/vbert_b200.h) ----
 static long long align256(long long x) { return (x + 255) / 256 * 256; }
 
-long long encoder_arena_layout(int B, int S, int H, int A, int I, int attn_drop, long long* off) {
-    const long long M = static_cast<long long>(B) * S;
+// M rows per layer (B * S dense, total varlen); lse holds A * M floats either way ([B, A, S] or [A, total]); the keep bits are
+// laid out for (B, S) with S the longest sequence
+long long encoder_arena_layout(int B, int S, int H, int A, int I, int attn_drop, long long* off, long long packed_rows = -1) {
+    const long long M = packed_rows >= 0 ? packed_rows : static_cast<long long>(B) * S;
     const long long sizes[VB_ENCODER_ARENA_BUFFERS] = {
-        M * 3 * H * 2, M * H * 2, static_cast<long long>(B) * A * S * 4, M * H * 2, M * 4, M * 4, M * H * 2, M * I * 2, M * I * 2,
+        M * 3 * H * 2, M * H * 2, static_cast<long long>(A) * M * 4, M * H * 2, M * 4, M * 4, M * H * 2, M * I * 2, M * I * 2,
         M * H * 2, M * 4, M * 4, attn_drop ? attn_keep_bytes(B, S, A) : 0, M * H * 2};
     long long o = 0;
     for (int i = 0; i < VB_ENCODER_ARENA_BUFFERS; ++i) {
@@ -164,9 +190,10 @@ long long encoder_arena_layout(int B, int S, int H, int A, int I, int attn_drop,
     return o;
 }
 
-static void arena_acts(const vb_layer_desc* d, void* arena, int l, vb_layer_acts* a, void** y) {
+static void arena_acts(const vb_layer_desc* d, void* arena, int l, vb_layer_acts* a, void** y, const LayerRows& rows) {
     long long off[VB_ENCODER_ARENA_BUFFERS];
-    const long long stride = encoder_arena_layout(d->batch, d->seq, d->hidden, d->heads, d->inter, d->attn_dropout > 0.f, off);
+    const long long stride = encoder_arena_layout(d->batch, d->seq, d->hidden, d->heads, d->inter, d->attn_dropout > 0.f, off,
+                                                  rows.cu_seqlens != nullptr ? rows.total : -1);
     char* base = static_cast<char*>(arena) + l * stride;
     a->qkv = base + off[0]; a->ctx = base + off[1]; a->lse = reinterpret_cast<float*>(base + off[2]);
     a->pre1 = base + off[3]; a->mean1 = reinterpret_cast<float*>(base + off[4]); a->rstd1 = reinterpret_cast<float*>(base + off[5]);
@@ -176,7 +203,7 @@ static void arena_acts(const vb_layer_desc* d, void* arena, int l, vb_layer_acts
     *y = base + off[13];
 }
 
-int encoder_fwd(const vb_layer_desc* descs, int n, const void* x_in, void* arena, cudaStream_t st) {
+int encoder_fwd(const vb_layer_desc* descs, int n, const void* x_in, void* arena, cudaStream_t st, const LayerRows& rows = kDenseRows) {
     VB_REQUIRE(descs && n > 0 && x_in && arena, "encoder_fwd: null pointer / no layers");
     const void* x = x_in;
     for (int l = 0; l < n; ++l) {
@@ -185,30 +212,30 @@ int encoder_fwd(const vb_layer_desc* descs, int n, const void* x_in, void* arena
                    (descs[l].attn_dropout > 0.f) == (descs[0].attn_dropout > 0.f), "encoder_fwd: layers differ in shape");
         vb_layer_acts a;
         void* y;
-        arena_acts(&descs[l], arena, l, &a, &y);
-        VB_TRY(layer_fwd(&descs[l], x, y, &a, st));
+        arena_acts(&descs[l], arena, l, &a, &y, rows);
+        VB_TRY(layer_fwd(&descs[l], x, y, &a, st, rows));
         x = y;
     }
     return 0;
 }
 
 int encoder_bwd(const vb_layer_desc* descs, int n, const void* x_in, void* arena, const void* dy, void* dx,
-                const vb_layer_grads* grads, const vb_layer_scratch* w, cudaStream_t st) {
+                const vb_layer_grads* grads, const vb_layer_scratch* w, cudaStream_t st, const LayerRows& rows = kDenseRows) {
     VB_REQUIRE(descs && n > 0 && x_in && arena && dy && dx && grads && w, "encoder_bwd: null pointer / no layers");
     const void* g_in = dy;
     for (int l = n - 1; l >= 0; --l) {
         vb_layer_acts a;
         void* y;
-        arena_acts(&descs[l], arena, l, &a, &y);
+        arena_acts(&descs[l], arena, l, &a, &y, rows);
         const void* xl = x_in;
         if (l > 0) {
             vb_layer_acts ap;
             void* yp;
-            arena_acts(&descs[l - 1], arena, l - 1, &ap, &yp);
+            arena_acts(&descs[l - 1], arena, l - 1, &ap, &yp, rows);
             xl = yp;
         }
         // the gradient buffer ping-pongs inside `dx` (vb_layer_bwd allows dx to alias dy)
-        VB_TRY(layer_bwd(&descs[l], xl, &a, g_in, dx, &grads[l], w, st));
+        VB_TRY(layer_bwd(&descs[l], xl, &a, g_in, dx, &grads[l], w, st, rows));
         g_in = dx;
     }
     return 0;
@@ -307,6 +334,32 @@ int vb_encoder_fwd(const vb_layer_desc* descs, int32_t n_layers, const void* x_i
 int vb_encoder_bwd(const vb_layer_desc* descs, int32_t n_layers, const void* x_in, void* arena, const void* dy, void* dx,
                    const vb_layer_grads* grads, const vb_layer_scratch* scratch, void* stream) {
     return vb::encoder_bwd(descs, n_layers, x_in, arena, dy, dx, grads, scratch, static_cast<cudaStream_t>(stream));
+}
+int64_t vb_encoder_arena_layout_varlen(int32_t batch, int32_t max_seq, int32_t total, int32_t hidden, int32_t heads, int32_t inter,
+                                       int32_t attn_dropout_on, int64_t* offsets) {
+    if (batch <= 0 || max_seq <= 0 || total < 0) {
+        vb::set_error("vb_encoder_arena_layout_varlen: bad shape (batch %d, max_seq %d, total %d)", batch, max_seq, total);
+        return -1;
+    }
+    long long off[VB_ENCODER_ARENA_BUFFERS];
+    const long long stride = vb::encoder_arena_layout(batch, max_seq, hidden, heads, inter, attn_dropout_on, off, total);
+    if (offsets) for (int i = 0; i < VB_ENCODER_ARENA_BUFFERS; ++i) offsets[i] = off[i];
+    return stride;
+}
+int vb_encoder_fwd_varlen(const vb_layer_desc* descs, int32_t n_layers, const int32_t* cu_seqlens, int32_t total, const void* x_in,
+                          void* arena, void* stream) {
+    if (cu_seqlens == nullptr) { vb::set_error("vb_encoder_fwd_varlen: cu_seqlens is NULL"); return 2; }
+    if (total <= 0) { vb::set_error("vb_encoder_fwd_varlen: total (%d) must be > 0", total); return 2; }
+    const vb::LayerRows rows = {cu_seqlens, total};
+    return vb::encoder_fwd(descs, n_layers, x_in, arena, static_cast<cudaStream_t>(stream), rows);
+}
+int vb_encoder_bwd_varlen(const vb_layer_desc* descs, int32_t n_layers, const int32_t* cu_seqlens, int32_t total, const void* x_in,
+                          void* arena, const void* dy, void* dx, const vb_layer_grads* grads, const vb_layer_scratch* scratch,
+                          void* stream) {
+    if (cu_seqlens == nullptr) { vb::set_error("vb_encoder_bwd_varlen: cu_seqlens is NULL"); return 2; }
+    if (total <= 0) { vb::set_error("vb_encoder_bwd_varlen: total (%d) must be > 0", total); return 2; }
+    const vb::LayerRows rows = {cu_seqlens, total};
+    return vb::encoder_bwd(descs, n_layers, x_in, arena, dy, dx, grads, scratch, static_cast<cudaStream_t>(stream), rows);
 }
 int vb_embed_fwd(const vb_embed_desc* d, void* y, const vb_embed_acts* acts, void* stream) {
     return vb::embed_fwd_api(d, y, acts, static_cast<cudaStream_t>(stream));

@@ -29,7 +29,7 @@ namespace vb {
 
 // MT = m16 tiles per warp: 1 -> 4 warps x 16 rows, 2 -> 2 warps x 32 rows (FA2-style: each ldmatrix'd K/V
 // fragment feeds twice as many MMAs and the warp carries twice as many independent accumulators).
-template <int MT, int MINB>
+template <int MT, int MINB, bool VL = false>
 __global__ void __launch_bounds__(128 / MT, MINB)
 attn_fwd_kernel(const AttnParams p, const int nsub) {
     constexpr int NT = 128 / MT;
@@ -38,13 +38,16 @@ attn_fwd_kernel(const AttnParams p, const int nsub) {
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     const int g = lane >> 2, t = lane & 3;
     const int qb = blockIdx.x, h = blockIdx.y, b = blockIdx.z;
-    const int S = p.S;
+    const SeqSpan sp = seq_span<VL>(p, b, h);
+    const int S = sp.len;  // rows of this sequence
+    if (VL && qb * kBlk >= S) return;  // query blocks past the end of a shorter sequence
     const long long ld = 3LL * p.H;
-    const bf16* qbase = p.qkv + static_cast<long long>(b) * S * ld + h * kHd;
+    const bf16* qbase = p.qkv + sp.row0 * ld + h * kHd;
     const bf16* kbase = qbase + p.H;
     const bf16* vbase = qbase + 2 * p.H;
     const uint32_t sQ = smem_u32(dsmem), sK0 = sQ + kTileBytes, sV0 = sK0 + nsub * kTileBytes;
-    const int nkb = (S + kBlk - 1) / kBlk;
+    const int nkb = (p.S + kBlk - 1) / kBlk;      // keep-mask layout: key blocks of the longest sequence
+    const int nkv = VL ? (S + kBlk - 1) / kBlk : nkb;  // key blocks of this one
 
     const float sc2 = p.scale * kLog2e;
     float m[MT][2], l[MT][2];
@@ -60,8 +63,8 @@ attn_fwd_kernel(const AttnParams p, const int nsub) {
     const int qrow0 = qb * kBlk + warp * 16 * MT;
     const bool active = qrow0 < S;  // warps whose query rows are all padding only help with the loads
 
-    for (int kb0 = 0; kb0 < nkb; kb0 += nsub) {
-        const int nb = min(nsub, nkb - kb0);
+    for (int kb0 = 0; kb0 < nkv; kb0 += nsub) {
+        const int nb = min(nsub, nkv - kb0);
         if (kb0 > 0) __syncthreads();  // previous stage fully consumed
         if (kb0 == 0) load_tile<NT>(sQ, qbase, ld, qb * kBlk, S, tid);
         for (int j = 0; j < nb; ++j) {
@@ -71,7 +74,7 @@ attn_fwd_kernel(const AttnParams p, const int nsub) {
         }
         for (int i = tid; i < nb * kBlk; i += NT) {
             const int key = kb0 * kBlk + i;
-            sbias[i] = key < S ? p.mask_bias[static_cast<long long>(b) * S + key] * kLog2e : -INFINITY;
+            sbias[i] = key_bias2<VL>(p, b, key, S);
         }
         for (int j = 0; j < nb; ++j) {
             cp_async_wait_dyn(nb - 1 - j);
@@ -155,9 +158,9 @@ attn_fwd_kernel(const AttnParams p, const int nsub) {
     for (int mt = 0; mt < MT; ++mt) {
         const int r0 = qrow0 + mt * 16;
         const float inv0 = 1.f / l[mt][0], inv1 = 1.f / l[mt][1];
-        store_acc(p.ctx + static_cast<long long>(b) * S * p.H + h * kHd, p.H, r0, S, o[mt], lane, inv0, inv1);
+        store_acc(p.ctx + sp.row0 * p.H + h * kHd, p.H, r0, S, o[mt], lane, inv0, inv1);
         if (t == 0 && p.lse != nullptr) {
-            float* lse = p.lse + (static_cast<long long>(b) * p.A + h) * S;
+            float* lse = p.lse + sp.stat0;
             if (r0 + g < S) lse[r0 + g] = (m[mt][0] + log2f(l[mt][0])) * 0.6931471805599453f;
             if (r0 + g + 8 < S) lse[r0 + g + 8] = (m[mt][1] + log2f(l[mt][1])) * 0.6931471805599453f;
         }
@@ -168,7 +171,7 @@ attn_fwd_kernel(const AttnParams p, const int nsub) {
 // backward A: per query block — D = rowsum(dO * O), dQ = scale * sum_k dS K
 // Shared memory: Q | dO | O | K tiles [nsub] | V tiles [nsub]
 // ------------------------------------------------------------------------------------------------
-template <int MINB>
+template <int MINB, bool VL = false>
 __global__ void __launch_bounds__(128, MINB)
 attn_bwd_dq_kernel(const AttnParams p, const int nsub) {
     extern __shared__ __align__(128) uint8_t dsmem[];
@@ -177,19 +180,22 @@ attn_bwd_dq_kernel(const AttnParams p, const int nsub) {
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     const int g = lane >> 2, t = lane & 3;
     const int qb = blockIdx.x, h = blockIdx.y, b = blockIdx.z;
-    const int S = p.S;
+    const SeqSpan sp = seq_span<VL>(p, b, h);
+    const int S = sp.len;
+    if (VL && qb * kBlk >= S) return;
     const long long ld = 3LL * p.H;
-    const bf16* qbase = p.qkv + static_cast<long long>(b) * S * ld + h * kHd;
+    const bf16* qbase = p.qkv + sp.row0 * ld + h * kHd;
     const bf16* kbase = qbase + p.H;
     const bf16* vbase = qbase + 2 * p.H;
-    const bf16* obase = p.ctx + static_cast<long long>(b) * S * p.H + h * kHd;
-    const bf16* dobase = p.dctx + static_cast<long long>(b) * S * p.H + h * kHd;
+    const bf16* obase = p.ctx + sp.row0 * p.H + h * kHd;
+    const bf16* dobase = p.dctx + sp.row0 * p.H + h * kHd;
     const uint32_t sQ = smem_u32(dsmem), sdO = sQ + kTileBytes, sO = sQ + 2 * kTileBytes;
     const uint32_t sK0 = sQ + 3 * kTileBytes, sV0 = sK0 + nsub * kTileBytes;
-    const int nkb = (S + kBlk - 1) / kBlk;
+    const int nkb = (p.S + kBlk - 1) / kBlk;
+    const int nkv = VL ? (S + kBlk - 1) / kBlk : nkb;
     const int qrow0 = qb * kBlk + warp * 16;
     const bool active = qrow0 < S;
-    const float* lsep = p.lse + (static_cast<long long>(b) * p.A + h) * S;
+    const float* lsep = p.lse + sp.stat0;
     const float lse0 = (qrow0 + g < S) ? lsep[qrow0 + g] * kLog2e : 0.f;
     const float lse1 = (qrow0 + g + 8 < S) ? lsep[qrow0 + g + 8] * kLog2e : 0.f;
     const float sc2 = p.scale * kLog2e;
@@ -199,8 +205,8 @@ attn_bwd_dq_kernel(const AttnParams p, const int nsub) {
     float dq[8][4];
     zero_acc(dq);
 
-    for (int kb0 = 0; kb0 < nkb; kb0 += nsub) {
-        const int nb = min(nsub, nkb - kb0);
+    for (int kb0 = 0; kb0 < nkv; kb0 += nsub) {
+        const int nb = min(nsub, nkv - kb0);
         if (kb0 > 0) __syncthreads();
         if (kb0 == 0) {
             load_tile(sQ, qbase, ld, qb * kBlk, S, tid);
@@ -214,7 +220,7 @@ attn_bwd_dq_kernel(const AttnParams p, const int nsub) {
         }
         for (int i = tid; i < nb * kBlk; i += 128) {
             const int key = kb0 * kBlk + i;
-            sbias[i] = key < S ? p.mask_bias[static_cast<long long>(b) * S + key] * kLog2e : -INFINITY;
+            sbias[i] = key_bias2<VL>(p, b, key, S);
         }
         for (int j = 0; j < nb; ++j) {
             cp_async_wait_dyn(nb - 1 - j);
@@ -239,7 +245,7 @@ attn_bwd_dq_kernel(const AttnParams p, const int nsub) {
                 if (half == 0) {
                     sD[r] = acc;
                     const int q = qb * kBlk + r;
-                    if (q < S) p.drow[(static_cast<long long>(b) * p.A + h) * S + q] = acc;
+                    if (q < S) p.drow[sp.stat0 + q] = acc;
                 }
                 __syncthreads();
                 if (active) {
@@ -291,7 +297,7 @@ attn_bwd_dq_kernel(const AttnParams p, const int nsub) {
         }
     }
     if (!active) return;
-    store_acc(p.dqkv + static_cast<long long>(b) * S * ld + h * kHd, ld, qrow0, S, dq, lane, p.scale, p.scale);
+    store_acc(p.dqkv + sp.row0 * ld + h * kHd, ld, qrow0, S, dq, lane, p.scale, p.scale);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -299,7 +305,7 @@ attn_bwd_dq_kernel(const AttnParams p, const int nsub) {
 // Shared memory: K | V | Q tiles [nsub] | dO tiles [nsub]; K/V fragments are re-read from shared memory
 // per query block instead of being pinned in 32 registers.
 // ------------------------------------------------------------------------------------------------
-template <int MINB>
+template <int MINB, bool VL = false>
 __global__ void __launch_bounds__(128, MINB)
 attn_bwd_dkv_kernel(const AttnParams p, const int nsub) {
     extern __shared__ __align__(128) uint8_t dsmem[];
@@ -308,29 +314,32 @@ attn_bwd_dkv_kernel(const AttnParams p, const int nsub) {
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     const int g = lane >> 2, t = lane & 3;
     const int kbk = blockIdx.x, h = blockIdx.y, b = blockIdx.z;
-    const int S = p.S;
+    const SeqSpan sp = seq_span<VL>(p, b, h);
+    const int S = sp.len;
+    if (VL && kbk * kBlk >= S) return;  // key blocks past the end of a shorter sequence
     const long long ld = 3LL * p.H;
-    const bf16* qbase = p.qkv + static_cast<long long>(b) * S * ld + h * kHd;
+    const bf16* qbase = p.qkv + sp.row0 * ld + h * kHd;
     const bf16* kbase = qbase + p.H;
     const bf16* vbase = qbase + 2 * p.H;
-    const bf16* dobase = p.dctx + static_cast<long long>(b) * S * p.H + h * kHd;
+    const bf16* dobase = p.dctx + sp.row0 * p.H + h * kHd;
     const uint32_t sK = smem_u32(dsmem), sV = sK + kTileBytes, sQ0 = sK + 2 * kTileBytes, sdO0 = sQ0 + nsub * kTileBytes;
-    const int nqb = (S + kBlk - 1) / kBlk;
-    const float* lsep = p.lse + (static_cast<long long>(b) * p.A + h) * S;
-    const float* drp = p.drow + (static_cast<long long>(b) * p.A + h) * S;
+    const int nqb = (p.S + kBlk - 1) / kBlk;            // keep-mask layout
+    const int nqv = VL ? (S + kBlk - 1) / kBlk : nqb;  // query blocks of this sequence
+    const float* lsep = p.lse + sp.stat0;
+    const float* drp = p.drow + sp.stat0;
     const int krow0 = kbk * kBlk + warp * 16;
     const bool active = krow0 < S;
     const int ka = krow0 + g, kc = krow0 + g + 8;
-    const float bias0 = ka < S ? p.mask_bias[static_cast<long long>(b) * S + ka] * kLog2e : -INFINITY;
-    const float bias1 = kc < S ? p.mask_bias[static_cast<long long>(b) * S + kc] * kLog2e : -INFINITY;
+    const float bias0 = key_bias2<VL>(p, b, ka, S);
+    const float bias1 = key_bias2<VL>(p, b, kc, S);
     const float sc2 = p.scale * kLog2e;
     const unsigned bh = static_cast<unsigned>(b * p.A + h);
     float dk[8][4], dv[8][4];
     zero_acc(dk);
     zero_acc(dv);
 
-    for (int qb0 = 0; qb0 < nqb; qb0 += nsub) {
-        const int nb = min(nsub, nqb - qb0);
+    for (int qb0 = 0; qb0 < nqv; qb0 += nsub) {
+        const int nb = min(nsub, nqv - qb0);
         if (qb0 > 0) __syncthreads();
         if (qb0 == 0) {
             load_tile(sK, kbase, ld, kbk * kBlk, S, tid);
@@ -419,7 +428,7 @@ attn_bwd_dkv_kernel(const AttnParams p, const int nsub) {
         }
     }
     if (!active) return;
-    bf16* dbase = p.dqkv + static_cast<long long>(b) * S * ld + h * kHd;
+    bf16* dbase = p.dqkv + sp.row0 * ld + h * kHd;
     store_acc(dbase + p.H, ld, krow0, S, dk, lane, p.scale, p.scale);
     store_acc(dbase + 2 * p.H, ld, krow0, S, dv, lane, 1.f, 1.f);
 }
@@ -462,6 +471,8 @@ static int fill_params(AttnParams& p, const void* qkv, const float* mask_bias, v
     p.dqkv = static_cast<bf16*>(dqkv);
     p.drow = drow;
     p.B = B; p.S = S; p.A = A; p.H = H;
+    p.cu_seqlens = nullptr;
+    p.total = 0;
     p.scale = 0.125f;
     // 8-bit quantised keep threshold (see attn_hash); the scale uses the quantised probability
     const unsigned th8 = static_cast<unsigned>(dropout_p * 256.f + 0.5f);
@@ -513,11 +524,19 @@ int attn_mask_async(void* keep, int B, int S, int A, int H, float dropout_p, uns
     return 1;
 }
 
-int attn_fwd(const void* qkv, const float* mask_bias, void* ctx, float* lse, void* keep, int B, int S, int A, int H,
-             float dropout_p, unsigned long long seed, unsigned stream_id, cudaStream_t st, bool mask_ready) {
-    AttnParams p;
-    int rc = fill_params(p, qkv, mask_bias, ctx, lse, nullptr, nullptr, nullptr, keep, B, S, A, H, dropout_p, seed, stream_id);
-    if (rc) return rc;
+// variable-length calls: the sequence table and the packed row count (what can be checked without reading device memory)
+static int set_varlen(AttnParams& p, const int* cu_seqlens, int total, const void* qkv, const void* out) {
+    VB_REQUIRE(cu_seqlens != nullptr, "attention varlen: cu_seqlens is NULL");
+    VB_REQUIRE(total >= 0, "attention varlen: total (%d) must be >= 0", total);
+    VB_REQUIRE(qkv != nullptr && out != nullptr, "attention varlen: null pointer");
+    VB_REQUIRE(static_cast<long long>(p.A) * total < (1LL << 31), "attention varlen: heads * total too large");
+    p.cu_seqlens = cu_seqlens;
+    p.total = total;
+    return 0;
+}
+
+static int attn_fwd_launch(const AttnParams& p, cudaStream_t st, bool mask_ready) {
+    const int B = p.B, S = p.S, A = p.A;
     dim3 grid((S + kBlk - 1) / kBlk, A, B);
     if (wgmma_path(p)) return attn_fwd_wgmma(p, st, mask_ready);
     if (head_path(S)) return attn_fwd_head(p, static_cast<int>(grid.x), st, mask_ready);
@@ -526,14 +545,38 @@ int attn_fwd(const void* qkv, const float* mask_bias, void* ctx, float* lse, voi
                "attention dropout: mask counter space exceeded (B*A*S too large)");
     const int nsub = static_cast<int>(grid.x) < kMaxSub ? static_cast<int>(grid.x) : kMaxSub;
     const int smem = (1 + 2 * nsub) * kTileBytes;
-    static int configured[kMaxDevices] = {0};
-    VB_CHECK_CUDA(ensure_dyn_smem(attn_fwd_kernel<1, 3>, (1 + 2 * kMaxSub) * kTileBytes, configured));
+    static int configured[kMaxDevices] = {0}, configured_vl[kMaxDevices] = {0};
     {
         ProfScope ps(st, PROF_ATTN_FWD, 4.0 * B * A * S * S * kHd, 1);
-        attn_fwd_kernel<1, 3><<<grid, 128, smem, st>>>(p, nsub);
+        if (p.cu_seqlens == nullptr) {
+            VB_CHECK_CUDA(ensure_dyn_smem(attn_fwd_kernel<1, 3>, (1 + 2 * kMaxSub) * kTileBytes, configured));
+            attn_fwd_kernel<1, 3><<<grid, 128, smem, st>>>(p, nsub);
+        } else {
+            VB_CHECK_CUDA(ensure_dyn_smem(attn_fwd_kernel<1, 3, true>, (1 + 2 * kMaxSub) * kTileBytes, configured_vl));
+            attn_fwd_kernel<1, 3, true><<<grid, 128, smem, st>>>(p, nsub);
+        }
     }
     VB_CHECK_CUDA(cudaGetLastError());
     return 0;
+}
+
+int attn_fwd(const void* qkv, const float* mask_bias, void* ctx, float* lse, void* keep, int B, int S, int A, int H,
+             float dropout_p, unsigned long long seed, unsigned stream_id, cudaStream_t st, bool mask_ready) {
+    AttnParams p;
+    int rc = fill_params(p, qkv, mask_bias, ctx, lse, nullptr, nullptr, nullptr, keep, B, S, A, H, dropout_p, seed, stream_id);
+    if (rc) return rc;
+    return attn_fwd_launch(p, st, mask_ready);
+}
+
+int attn_fwd_varlen(const void* qkv, const int* cu_seqlens, void* ctx, float* lse, void* keep, int B, int max_seq, int total,
+                    int A, int H, float dropout_p, unsigned long long seed, unsigned stream_id, cudaStream_t st, bool mask_ready) {
+    AttnParams p;
+    int rc = fill_params(p, qkv, nullptr, ctx, lse, nullptr, nullptr, nullptr, keep, B, max_seq, A, H, dropout_p, seed, stream_id);
+    if (rc) return rc;
+    VB_REQUIRE(lse != nullptr, "attention varlen: lse is NULL");
+    if ((rc = set_varlen(p, cu_seqlens, total, qkv, ctx))) return rc;
+    if (total == 0) return 0;  // no rows: nothing to compute or store
+    return attn_fwd_launch(p, st, mask_ready);
 }
 
 static int g_bwd_minb = 3;
@@ -542,13 +585,8 @@ bool attn_bwd_takes_delta(const void* qkv, const void* dctx, void* dqkv, int B, 
     return B > 0 && S > 0 && A > 0 && H == A * kHd && head_path(S);
 }
 
-int attn_bwd(const void* qkv, const float* mask_bias, const void* ctx, const float* lse, const void* keep,
-             const void* dctx, void* dqkv, float* drow, int B, int S, int A, int H, float dropout_p,
-             unsigned long long seed, unsigned stream_id, cudaStream_t st, bool delta_ready) {
-    AttnParams p;
-    int rc = fill_params(p, qkv, mask_bias, const_cast<void*>(ctx), const_cast<float*>(lse), dctx, dqkv, drow,
-                         const_cast<void*>(keep), B, S, A, H, dropout_p, seed, stream_id);
-    if (rc) return rc;
+static int attn_bwd_launch(const AttnParams& p, cudaStream_t st, bool delta_ready) {
+    const int B = p.B, S = p.S, A = p.A;
     static int c0[kMaxDevices] = {0}, c1[kMaxDevices] = {0}, c2[kMaxDevices] = {0}, c3[kMaxDevices] = {0};
     VB_CHECK_CUDA(ensure_dyn_smem(attn_bwd_dq_kernel<2>, (3 + 2 * kMaxSub) * kTileBytes, c0));
     VB_CHECK_CUDA(ensure_dyn_smem(attn_bwd_dq_kernel<3>, (3 + 2 * kMaxSub) * kTileBytes, c1));
@@ -564,18 +602,49 @@ int attn_bwd(const void* qkv, const float* mask_bias, const void* ctx, const flo
     if (wgmma_path(p)) return attn_bwd_wgmma(p, st, delta_ready);
     if (head_path(S)) return attn_bwd_head(p, static_cast<int>(grid.x), st, delta_ready);
     const int nsub = static_cast<int>(grid.x) < kMaxSub ? static_cast<int>(grid.x) : kMaxSub;
+    const bool vl = p.cu_seqlens != nullptr;
+    if (vl) {
+        static int v0[kMaxDevices] = {0}, v1[kMaxDevices] = {0};
+        VB_CHECK_CUDA(ensure_dyn_smem(attn_bwd_dq_kernel<3, true>, (3 + 2 * kMaxSub) * kTileBytes, v0));
+        VB_CHECK_CUDA(ensure_dyn_smem(attn_bwd_dkv_kernel<3, true>, (2 + 2 * kMaxSub) * kTileBytes, v1));
+    }
     {   // algorithmic work of the backward = 2x forward (recompute not credited), split evenly over the two kernels
         ProfScope ps(st, PROF_ATTN_DQ, 4.0 * B * A * S * S * kHd, 1);
-        if (g_bwd_minb == 2) attn_bwd_dq_kernel<2><<<grid, 128, (3 + 2 * nsub) * kTileBytes, st>>>(p, nsub);
+        if (vl) attn_bwd_dq_kernel<3, true><<<grid, 128, (3 + 2 * nsub) * kTileBytes, st>>>(p, nsub);
+        else if (g_bwd_minb == 2) attn_bwd_dq_kernel<2><<<grid, 128, (3 + 2 * nsub) * kTileBytes, st>>>(p, nsub);
         else attn_bwd_dq_kernel<3><<<grid, 128, (3 + 2 * nsub) * kTileBytes, st>>>(p, nsub);
     }
     {
         ProfScope ps(st, PROF_ATTN_DKV, 4.0 * B * A * S * S * kHd, 1);
-        if (g_bwd_minb == 2) attn_bwd_dkv_kernel<2><<<grid, 128, (2 + 2 * nsub) * kTileBytes, st>>>(p, nsub);
+        if (vl) attn_bwd_dkv_kernel<3, true><<<grid, 128, (2 + 2 * nsub) * kTileBytes, st>>>(p, nsub);
+        else if (g_bwd_minb == 2) attn_bwd_dkv_kernel<2><<<grid, 128, (2 + 2 * nsub) * kTileBytes, st>>>(p, nsub);
         else attn_bwd_dkv_kernel<3><<<grid, 128, (2 + 2 * nsub) * kTileBytes, st>>>(p, nsub);
     }
     VB_CHECK_CUDA(cudaGetLastError());
     return 0;
+}
+
+int attn_bwd(const void* qkv, const float* mask_bias, const void* ctx, const float* lse, const void* keep,
+             const void* dctx, void* dqkv, float* drow, int B, int S, int A, int H, float dropout_p,
+             unsigned long long seed, unsigned stream_id, cudaStream_t st, bool delta_ready) {
+    AttnParams p;
+    int rc = fill_params(p, qkv, mask_bias, const_cast<void*>(ctx), const_cast<float*>(lse), dctx, dqkv, drow,
+                         const_cast<void*>(keep), B, S, A, H, dropout_p, seed, stream_id);
+    if (rc) return rc;
+    return attn_bwd_launch(p, st, delta_ready);
+}
+
+int attn_bwd_varlen(const void* qkv, const int* cu_seqlens, const void* ctx, const float* lse, const void* keep,
+                    const void* dctx, void* dqkv, float* drow, int B, int max_seq, int total, int A, int H, float dropout_p,
+                    unsigned long long seed, unsigned stream_id, cudaStream_t st, bool delta_ready) {
+    AttnParams p;
+    int rc = fill_params(p, qkv, nullptr, const_cast<void*>(ctx), const_cast<float*>(lse), dctx, dqkv, drow,
+                         const_cast<void*>(keep), B, max_seq, A, H, dropout_p, seed, stream_id);
+    if (rc) return rc;
+    VB_REQUIRE(ctx && lse && dctx && drow, "attention varlen: null pointer");
+    if ((rc = set_varlen(p, cu_seqlens, total, qkv, dqkv))) return rc;
+    if (total == 0) return 0;
+    return attn_bwd_launch(p, st, delta_ready);
 }
 
 }  // namespace vb
@@ -595,5 +664,17 @@ int vb_attention_bwd(const void* qkv, const float* mask_bias, const void* ctx, c
                      int32_t hidden, float dropout_p, uint64_t dropout_seed, uint32_t dropout_stream, void* stream) {
     return vb::attn_bwd(qkv, mask_bias, ctx, lse, keep_mask, dctx, dqkv, drow, batch, seq, heads, hidden, dropout_p,
                         dropout_seed, dropout_stream, static_cast<cudaStream_t>(stream), false);
+}
+int vb_attention_fwd_varlen(const void* qkv, const int32_t* cu_seqlens, void* ctx, float* lse, void* keep_mask, int32_t batch,
+                            int32_t max_seq, int32_t total, int32_t heads, int32_t hidden, float dropout_p, uint64_t dropout_seed,
+                            uint32_t dropout_stream, void* stream) {
+    return vb::attn_fwd_varlen(qkv, cu_seqlens, ctx, lse, keep_mask, batch, max_seq, total, heads, hidden, dropout_p, dropout_seed,
+                               dropout_stream, static_cast<cudaStream_t>(stream), false);
+}
+int vb_attention_bwd_varlen(const void* qkv, const int32_t* cu_seqlens, const void* ctx, const float* lse, const void* keep_mask,
+                            const void* dctx, void* dqkv, float* drow, int32_t batch, int32_t max_seq, int32_t total, int32_t heads,
+                            int32_t hidden, float dropout_p, uint64_t dropout_seed, uint32_t dropout_stream, void* stream) {
+    return vb::attn_bwd_varlen(qkv, cu_seqlens, ctx, lse, keep_mask, dctx, dqkv, drow, batch, max_seq, total, heads, hidden,
+                               dropout_p, dropout_seed, dropout_stream, static_cast<cudaStream_t>(stream), false);
 }
 }

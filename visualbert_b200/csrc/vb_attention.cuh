@@ -29,7 +29,43 @@ struct AttnParams {
     float drop_scale;  // 1/(1-p) or 0
     unsigned drop_thresh16;  // attention: 8-bit threshold, round(p * 256)
     unsigned drop_seed;
+    // variable-length ("unpadded") calls: sequence b owns the packed rows [cu_seqlens[b], cu_seqlens[b+1]) of `total`; S is then
+    // the longest sequence (it sizes the grid and the keep-mask layout), lse / drow are [A, total], and mask_bias is unused
+    const int* cu_seqlens;  // device [B + 1]; nullptr for dense calls
+    int total;
 };
+
+// The rows one (sequence b, head h) works on: the first packed row, the sequence length and the base of its lse / drow
+// entries. Dense: (b S, S, (b A + h) S). Varlen: (cu[b], len_b, h total + cu[b]), with the table clamped so that a bad
+// cu_seqlens cannot send a kernel outside [0, total) rows or past S rows per sequence.
+struct SeqSpan {
+    long long row0;
+    int len;
+    long long stat0;
+};
+template <bool VL>
+__device__ __forceinline__ SeqSpan seq_span(const AttnParams& p, int b, int h) {
+    SeqSpan s;
+    if constexpr (VL) {
+        int lo = __ldg(p.cu_seqlens + b), hi = __ldg(p.cu_seqlens + b + 1);
+        lo = min(max(lo, 0), p.total);
+        hi = min(max(hi, lo), p.total);
+        s.row0 = lo;
+        s.len = min(hi - lo, p.S);
+        s.stat0 = static_cast<long long>(h) * p.total + lo;
+    } else {
+        s.row0 = static_cast<long long>(b) * p.S;
+        s.len = p.S;
+        s.stat0 = (static_cast<long long>(b) * p.A + h) * p.S;
+    }
+    return s;
+}
+// additive key bias in the exp2 domain: the caller's mask when dense; every key of the sequence is valid when varlen
+template <bool VL>
+__device__ __forceinline__ float key_bias2(const AttnParams& p, int b, int key, int len) {
+    if constexpr (VL) return key < len ? 0.f : -INFINITY;
+    else return key < p.S ? p.mask_bias[static_cast<long long>(b) * p.S + key] * kLog2e : -INFINITY;
+}
 
 // ------------------------------------------------------------------------------------------------
 // small device helpers
@@ -269,6 +305,8 @@ constexpr int kMaxSub = 4;  // 64-row tiles per resident stage
 // whole-head persistent kernels (vb_attention_head.cu); nkb = ceil(S / 64) <= kMaxSub.
 // mask_ready: the keep bits were already drawn (attn_mask_async); delta_ready: p.drow already holds D = rowsum(dO * O)
 // (written by the epilogue of the GEMM that produced dO, vb_gemm_args.delta_out).
+// Every launcher serves dense calls and, when p.cu_seqlens != nullptr, variable-length ones (a separate instantiation of each
+// kernel, so the dense code is unchanged).
 int attn_fwd_head(const AttnParams& p, int nkb, cudaStream_t st, bool mask_ready);
 int attn_bwd_head(const AttnParams& p, int nkb, cudaStream_t st, bool delta_ready);
 int attn_keep_mask(const AttnParams& p, int nkb, cudaStream_t st);

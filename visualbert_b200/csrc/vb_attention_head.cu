@@ -163,7 +163,7 @@ __device__ __forceinline__ void fwd_block(const AttnParams& p, float (&o)[8][4],
 // ------------------------------------------------------------------------------------------------
 // forward
 // ------------------------------------------------------------------------------------------------
-template <int NW>
+template <int NW, bool VL = false>
 __global__ void __launch_bounds__(NW * 32, 1)
 attn_fwd_head_kernel(const AttnParams p, const int nkb) {
     constexpr int NT = NW * 32;
@@ -181,15 +181,16 @@ attn_fwd_head_kernel(const AttnParams p, const int nkb) {
 
     auto issue = [&](int item, int buf) {
         const int b = item / p.A, h = item % p.A;
-        const bf16* qbase = p.qkv + static_cast<long long>(b) * S * ld + h * kHd;
+        const SeqSpan sp = seq_span<VL>(p, b, h);
+        const int nkv = VL ? (sp.len + kBlk - 1) / kBlk : nkb;  // tiles past the sequence's end are not loaded
+        const bf16* qbase = p.qkv + sp.row0 * ld + h * kHd;
         const uint32_t base = smem_u32(dsmem) + buf * buf_bytes;
-        load_rows<NT>(base, qbase, ld, nkb, S, tid);
-        load_rows<NT>(base + nkb * kTileBytes, qbase + p.H, ld, nkb, S, tid);
-        load_rows<NT>(base + 2 * nkb * kTileBytes, qbase + 2 * p.H, ld, nkb, S, tid);
+        load_rows<NT>(base, qbase, ld, nkv, sp.len, tid);
+        load_rows<NT>(base + nkb * kTileBytes, qbase + p.H, ld, nkv, sp.len, tid);
+        load_rows<NT>(base + 2 * nkb * kTileBytes, qbase + 2 * p.H, ld, nkv, sp.len, tid);
         cp_async_commit();
         float* sb = sbias_all + buf * nkb * kBlk;
-        for (int i = tid; i < nkb * kBlk; i += NT)
-            sb[i] = i < S ? p.mask_bias[static_cast<long long>(b) * S + i] * kLog2e : -INFINITY;
+        for (int i = tid; i < nkb * kBlk; i += NT) sb[i] = key_bias2<VL>(p, b, i, sp.len);
     };
 
     int item = blockIdx.x;
@@ -207,28 +208,31 @@ attn_fwd_head_kernel(const AttnParams p, const int nkb) {
             cp_async_wait<0>();
         }
         __syncthreads();
-        if (active) {
-            const int b = item / p.A, h = item % p.A;
+        const int b = item / p.A, h = item % p.A;
+        const SeqSpan sp = seq_span<VL>(p, b, h);
+        const int len = sp.len;
+        if (VL ? qrow0 < len : active) {  // warps past the sequence's end skip the head
             const unsigned bh = static_cast<unsigned>(item);
             const uint32_t base = smem_u32(dsmem) + buf * buf_bytes;
             const float* sb = sbias_all + buf * nkb * kBlk;
+            const int nkv = VL ? (len + kBlk - 1) / kBlk : nkb;
             uint32_t qf[4][4];
             load_afrag(qf, base + (warp >> 2) * kTileBytes, (warp & 3) * 16, lane);
             float m[2] = {-INFINITY, -INFINITY}, l[2] = {0.f, 0.f};
             float o[8][4];
             zero_acc(o);
-            for (int kb = 0; kb < nkb; ++kb) {
-                const int kvalid = min(kBlk, S - kb * kBlk);
+            for (int kb = 0; kb < nkv; ++kb) {
+                const int kvalid = min(kBlk, len - kb * kBlk);
                 fwd_block(p, o, m, l, qf, base + (nkb + kb) * kTileBytes, base + (2 * nkb + kb) * kTileBytes,
                           sb + kb * kBlk, kb, kvalid, qrow0, bh, nkb, lane, sc2);
             }
             const float dscale = p.drop_scale != 0.f ? p.drop_scale : 1.f;  // survivors' 1/(1-p), see fwd_block
             const float inv0 = dscale / l[0], inv1 = dscale / l[1];
-            store_acc(p.ctx + static_cast<long long>(b) * S * p.H + h * kHd, p.H, qrow0, S, o, lane, inv0, inv1);
+            store_acc(p.ctx + sp.row0 * p.H + h * kHd, p.H, qrow0, len, o, lane, inv0, inv1);
             if (t == 0 && p.lse != nullptr) {
-                float* lse = p.lse + static_cast<long long>(item) * S;
-                if (qrow0 + g < S) lse[qrow0 + g] = (m[0] + log2f(l[0])) * 0.6931471805599453f;
-                if (qrow0 + g + 8 < S) lse[qrow0 + g + 8] = (m[1] + log2f(l[1])) * 0.6931471805599453f;
+                float* lse = p.lse + (VL ? sp.stat0 : static_cast<long long>(item) * S);
+                if (qrow0 + g < len) lse[qrow0 + g] = (m[0] + log2f(l[0])) * 0.6931471805599453f;
+                if (qrow0 + g + 8 < len) lse[qrow0 + g + 8] = (m[1] + log2f(l[1])) * 0.6931471805599453f;
             }
         }
         __syncthreads();  // buffer `buf` is free again: the prefetch two iterations ahead may overwrite it
@@ -238,6 +242,8 @@ attn_fwd_head_kernel(const AttnParams p, const int nkb) {
 // ------------------------------------------------------------------------------------------------
 // backward: delta pre-kernel  D[b, h, q] = sum_d dO[b, q, h, d] * O[b, q, h, d]
 // ------------------------------------------------------------------------------------------------
+// VL (variable-length calls): rows are the `total` packed tokens and drow is [A, total] (B = 1, S = total below)
+template <bool VL = false>
 __global__ void __launch_bounds__(256)
 attn_delta_kernel(const bf16* __restrict__ o, const bf16* __restrict__ d_o, float* __restrict__ drow, int B, int S,
                   int A, int H) {
@@ -246,7 +252,7 @@ attn_delta_kernel(const bf16* __restrict__ o, const bf16* __restrict__ d_o, floa
     pdl_trigger();
     pdl_wait();
     if (row >= static_cast<long long>(B) * S) return;
-    const int b = static_cast<int>(row / S), q = static_cast<int>(row % S);
+    const int b = VL ? 0 : static_cast<int>(row / S), q = VL ? static_cast<int>(row) : static_cast<int>(row % S);
     const int chunks = H >> 3;  // 8 chunks of 8 elements per head
     for (int c0 = 0; c0 < chunks; c0 += 32) {  // warp-uniform trip count: the shuffles below need all lanes
         const int ch = c0 + lane;
@@ -272,7 +278,7 @@ attn_delta_kernel(const bf16* __restrict__ o, const bf16* __restrict__ d_o, floa
 // backward: fused dQ + dK/dV for one (batch, head) per CTA iteration
 // smem per buffer: Q | K | V | dO tiles (nkb each) ; then per buffer fp32 arrays lse2[nkb*64], D[nkb*64], bias2[nkb*64]
 // ------------------------------------------------------------------------------------------------
-template <int NW>
+template <int NW, bool VL = false>
 __global__ void __launch_bounds__(NW * 32, 1)
 attn_bwd_head_kernel(const AttnParams p, const int nkb, const int nbuf) {
     constexpr int NT = NW * 32;
@@ -291,21 +297,24 @@ attn_bwd_head_kernel(const AttnParams p, const int nkb, const int nbuf) {
 
     auto issue = [&](int item, int buf) {
         const int b = item / p.A, h = item % p.A;
-        const bf16* qbase = p.qkv + static_cast<long long>(b) * S * ld + h * kHd;
-        const bf16* dobase = p.dctx + static_cast<long long>(b) * S * p.H + h * kHd;
+        const SeqSpan sp = seq_span<VL>(p, b, h);
+        const int len = sp.len, nkv = VL ? (len + kBlk - 1) / kBlk : nkb;
+        const bf16* qbase = p.qkv + sp.row0 * ld + h * kHd;
+        const bf16* dobase = p.dctx + sp.row0 * p.H + h * kHd;
         const uint32_t base = smem_u32(dsmem) + buf * buf_bytes;
-        load_rows<NT>(base, qbase, ld, nkb, S, tid);
-        load_rows<NT>(base + nkb * kTileBytes, qbase + p.H, ld, nkb, S, tid);
-        load_rows<NT>(base + 2 * nkb * kTileBytes, qbase + 2 * p.H, ld, nkb, S, tid);
-        load_rows<NT>(base + 3 * nkb * kTileBytes, dobase, p.H, nkb, S, tid);
+        load_rows<NT>(base, qbase, ld, nkv, len, tid);
+        load_rows<NT>(base + nkb * kTileBytes, qbase + p.H, ld, nkv, len, tid);
+        load_rows<NT>(base + 2 * nkb * kTileBytes, qbase + 2 * p.H, ld, nkv, len, tid);
+        load_rows<NT>(base + 3 * nkb * kTileBytes, dobase, p.H, nkv, len, tid);
         cp_async_commit();
         float* sv = svec_all + buf * 3 * np64;
-        const float* lsep = p.lse + static_cast<long long>(item) * S;
-        const float* drp = p.drow + static_cast<long long>(item) * S;
+        const long long stat0 = VL ? sp.stat0 : static_cast<long long>(item) * S;
+        const float* lsep = p.lse + stat0;
+        const float* drp = p.drow + stat0;
         for (int i = tid; i < np64; i += NT) {
-            sv[i] = i < S ? lsep[i] * kLog2e : INFINITY;                       // +inf => p = 0 for padded queries
-            sv[np64 + i] = i < S ? drp[i] : 0.f;
-            sv[2 * np64 + i] = i < S ? p.mask_bias[static_cast<long long>(b) * S + i] * kLog2e : -INFINITY;
+            sv[i] = i < len ? lsep[i] * kLog2e : INFINITY;                       // +inf => p = 0 for padded queries
+            sv[np64 + i] = i < len ? drp[i] : 0.f;
+            sv[2 * np64 + i] = key_bias2<VL>(p, b, i, len);
         }
     };
 
@@ -325,8 +334,10 @@ attn_bwd_head_kernel(const AttnParams p, const int nkb, const int nbuf) {
             cp_async_wait<0>();
         }
         __syncthreads();
-        if (active) {
-            const int b = item / p.A, h = item % p.A;
+        const int b = item / p.A, h = item % p.A;
+        const SeqSpan sp = seq_span<VL>(p, b, h);
+        const int len = sp.len, nkv = VL ? (len + kBlk - 1) / kBlk : nkb;
+        if (VL ? row0 < len : active) {
             const unsigned bh = static_cast<unsigned>(item);
             const uint32_t base = smem_u32(dsmem) + buf * buf_bytes;
             const uint32_t sQ = base, sK = base + nkb * kTileBytes, sV = base + 2 * nkb * kTileBytes, sdO = base + 3 * nkb * kTileBytes;
@@ -335,7 +346,7 @@ attn_bwd_head_kernel(const AttnParams p, const int nkb, const int nbuf) {
             const float* sbias = slse + 2 * np64;
             const bool drop = p.drop_scale != 0.f;
             const float ds = drop ? p.drop_scale : 1.f;
-            bf16* dbase = p.dqkv + static_cast<long long>(b) * S * ld + h * kHd;
+            bf16* dbase = p.dqkv + sp.row0 * ld + h * kHd;
             const int mytile = warp >> 2, myrow = (warp & 3) * 16;
 
             // ---------------- phase A: dQ for query rows row0 .. row0+15 ----------------
@@ -347,8 +358,8 @@ attn_bwd_head_kernel(const AttnParams p, const int nkb, const int nbuf) {
                 const float d0 = sD[row0 + g], d1 = sD[row0 + g + 8];
                 float dq[8][4];
                 zero_acc(dq);
-                for (int kb = 0; kb < nkb; ++kb) {
-                    const int kvalid = min(kBlk, S - kb * kBlk);
+                for (int kb = 0; kb < nkv; ++kb) {
+                    const int kvalid = min(kBlk, len - kb * kBlk);
                     unsigned long long keep_a = ~0ull, keep_c = ~0ull;
                     if (drop) {
                         const unsigned long long* kp = p.keep + (static_cast<unsigned long long>(bh) * np64) * nkb;
@@ -382,7 +393,7 @@ attn_bwd_head_kernel(const AttnParams p, const int nkb, const int nbuf) {
                     acc_to_afrag(dsf, s);
                     gemm_nn(dq, dsf, sK + kb * kTileBytes, lane, kvalid);
                 }
-                store_acc(dbase, ld, row0, S, dq, lane, p.scale, p.scale);
+                store_acc(dbase, ld, row0, len, dq, lane, p.scale, p.scale);
             }
             // ---------------- phase B: dK, dV for key rows row0 .. row0+15 ----------------
             {
@@ -391,8 +402,8 @@ attn_bwd_head_kernel(const AttnParams p, const int nkb, const int nbuf) {
                 float dk[8][4], dv[8][4];
                 zero_acc(dk);
                 zero_acc(dv);
-                for (int qb = 0; qb < nkb; ++qb) {
-                    const int qvalid = min(kBlk, S - qb * kBlk);
+                for (int qb = 0; qb < nkv; ++qb) {
+                    const int qvalid = min(kBlk, len - qb * kBlk);
                     uint32_t af[4][4];
                     float st[8][4];
                     zero_acc(st);
@@ -455,8 +466,8 @@ attn_bwd_head_kernel(const AttnParams p, const int nkb, const int nbuf) {
                     acc_to_afrag(af, st);
                     gemm_nn(dk, af, sQ + qb * kTileBytes, lane, qvalid);  // dK += dS^T Q
                 }
-                store_acc(dbase + p.H, ld, row0, S, dk, lane, p.scale, p.scale);
-                store_acc(dbase + 2 * p.H, ld, row0, S, dv, lane, 1.f, 1.f);
+                store_acc(dbase + p.H, ld, row0, len, dk, lane, p.scale, p.scale);
+                store_acc(dbase + 2 * p.H, ld, row0, len, dv, lane, 1.f, 1.f);
             }
         }
         __syncthreads();
@@ -479,7 +490,7 @@ attn_bwd_head_kernel(const AttnParams p, const int nkb, const int nbuf) {
 // the next head cannot be double-buffered entirely: its K and V tiles (not needed by phase B) and its vectors are
 // prefetched during phase B, Q and dO at the top of its own iteration.
 // ------------------------------------------------------------------------------------------------
-template <int NW>
+template <int NW, bool VL = false>
 __global__ void __launch_bounds__(NW * 32, 1)
 attn_bwd_head_ps_kernel(const AttnParams p, const int nkb, const int colsP) {
     constexpr int NT = NW * 32;
@@ -506,23 +517,28 @@ attn_bwd_head_ps_kernel(const AttnParams p, const int nkb, const int colsP) {
 
     auto issue_kv = [&](int item, int vb) {
         const int b = item / p.A, h = item % p.A;
-        const bf16* qbase = p.qkv + static_cast<long long>(b) * S * ld + h * kHd;
-        load_rows<NT>(sK, qbase + p.H, ld, nkb, S, tid);
-        load_rows<NT>(sV, qbase + 2 * p.H, ld, nkb, S, tid);
+        const SeqSpan sp = seq_span<VL>(p, b, h);
+        const int len = sp.len, nkv = VL ? (len + kBlk - 1) / kBlk : nkb;
+        const bf16* qbase = p.qkv + sp.row0 * ld + h * kHd;
+        load_rows<NT>(sK, qbase + p.H, ld, nkv, len, tid);
+        load_rows<NT>(sV, qbase + 2 * p.H, ld, nkv, len, tid);
         cp_async_commit();
         float* sv = svec_all + vb * 3 * np64;
-        const float* lsep = p.lse + static_cast<long long>(item) * S;
-        const float* drp = p.drow + static_cast<long long>(item) * S;
+        const long long stat0 = VL ? sp.stat0 : static_cast<long long>(item) * S;
+        const float* lsep = p.lse + stat0;
+        const float* drp = p.drow + stat0;
         for (int i = tid; i < np64; i += NT) {
-            sv[i] = i < S ? lsep[i] * kLog2e : INFINITY;  // +inf => p = 0 for padded queries
-            sv[np64 + i] = i < S ? drp[i] : 0.f;
-            sv[2 * np64 + i] = i < S ? p.mask_bias[static_cast<long long>(b) * S + i] * kLog2e : -INFINITY;
+            sv[i] = i < len ? lsep[i] * kLog2e : INFINITY;  // +inf => p = 0 for padded queries
+            sv[np64 + i] = i < len ? drp[i] : 0.f;
+            sv[2 * np64 + i] = key_bias2<VL>(p, b, i, len);
         }
     };
     auto issue_qdo = [&](int item) {
         const int b = item / p.A, h = item % p.A;
-        load_rows<NT>(sQ, p.qkv + static_cast<long long>(b) * S * ld + h * kHd, ld, nkb, S, tid);
-        load_rows<NT>(sdO, p.dctx + static_cast<long long>(b) * S * p.H + h * kHd, p.H, nkb, S, tid);
+        const SeqSpan sp = seq_span<VL>(p, b, h);
+        const int len = sp.len, nkv = VL ? (len + kBlk - 1) / kBlk : nkb;
+        load_rows<NT>(sQ, p.qkv + sp.row0 * ld + h * kHd, ld, nkv, len, tid);
+        load_rows<NT>(sdO, p.dctx + sp.row0 * p.H + h * kHd, p.H, nkv, len, tid);
         cp_async_commit();
     };
 
@@ -537,15 +553,20 @@ attn_bwd_head_ps_kernel(const AttnParams p, const int nkb, const int colsP) {
         cp_async_wait<0>();
         __syncthreads();
         const int b = item / p.A, h = item % p.A;
+        const SeqSpan sp = seq_span<VL>(p, b, h);
+        const int len = sp.len, nkv = VL ? (len + kBlk - 1) / kBlk : nkb;
+        // rows of P / dS that phase A writes (every warp with a row of the sequence writes its 16 rows)
+        const int rowsv = VL ? (len + 15) / 16 * 16 : rowsP;
+        const bool act = VL ? row0 < len : active;
         const unsigned bh = static_cast<unsigned>(item);
         const float* slse = svec_all + vb * 3 * np64;
         const float* sD = slse + np64;
         const float* sbias = slse + 2 * np64;
-        bf16* dbase = p.dqkv + static_cast<long long>(b) * S * ld + h * kHd;
+        bf16* dbase = p.dqkv + sp.row0 * ld + h * kHd;
         const int mytile = warp >> 2, myrow = (warp & 3) * 16;
 
         // ---------------- phase A: S, P, dP, dS once; dQ; P_drop / dS -> shared memory ----------------
-        if (active) {
+        if (act) {
             uint32_t qf[4][4], dof[4][4];
             load_afrag(qf, sQ + mytile * kTileBytes, myrow, lane);
             load_afrag(dof, sdO + mytile * kTileBytes, myrow, lane);
@@ -554,8 +575,8 @@ attn_bwd_head_ps_kernel(const AttnParams p, const int nkb, const int colsP) {
             const uint32_t prow0 = (row0 + g) * pitch, prow1 = (row0 + g + 8) * pitch;
             float dq[8][4];
             zero_acc(dq);
-            for (int kb = 0; kb < nkb; ++kb) {
-                const int kvalid = min(kBlk, S - kb * kBlk);
+            for (int kb = 0; kb < nkv; ++kb) {
+                const int kvalid = min(kBlk, len - kb * kBlk);
                 unsigned long long keep_a = ~0ull, keep_c = ~0ull;
                 if (drop) {
                     const unsigned long long* kp = p.keep + (static_cast<unsigned long long>(bh) * np64) * nkb;
@@ -596,7 +617,7 @@ attn_bwd_head_ps_kernel(const AttnParams p, const int nkb, const int colsP) {
                 acc_to_afrag(dsf, s);
                 gemm_nn(dq, dsf, sK + kb * kTileBytes, lane, kvalid);
             }
-            store_acc(dbase, ld, row0, S, dq, lane, p.scale, p.scale);
+            store_acc(dbase, ld, row0, len, dq, lane, p.scale, p.scale);
         }
         __syncthreads();  // P / dS complete; K and V tiles are dead from here on
 
@@ -604,14 +625,14 @@ attn_bwd_head_ps_kernel(const AttnParams p, const int nkb, const int colsP) {
         if (next < total) issue_kv(next, vb ^ 1);  // overlaps phase B
 
         // ---------------- phase B: dV = P_drop^T dO, dK = dS^T Q for key rows row0 .. row0+15 ----------------
-        if (active) {
+        if (act) {
             float dk[8][4], dv[8][4];
             zero_acc(dk);
             zero_acc(dv);
             // ldmatrix.trans address of this lane: matrix i = lane >> 3 -> (query half i >> 1, key half i & 1)
             const uint32_t a_off = (((lane >> 4) & 1) * 8 + (lane & 7)) * pitch + (row0 + ((lane >> 3) & 1) * 8) * 2;
-            for (int qb = 0; qb < nkb; ++qb) {
-                const int qvalid = min(kBlk, rowsP - qb * kBlk);
+            for (int qb = 0; qb < nkv; ++qb) {
+                const int qvalid = min(kBlk, rowsv - qb * kBlk);
                 if (qvalid <= 0) break;
                 uint32_t af[4][4];
 #pragma unroll
@@ -625,23 +646,27 @@ attn_bwd_head_ps_kernel(const AttnParams p, const int nkb, const int colsP) {
                         ldsm_x4_t(sDS + (qb * kBlk + ks * 16) * pitch + a_off, af[ks][0], af[ks][1], af[ks][2], af[ks][3]);
                 gemm_nn(dk, af, sQ + qb * kTileBytes, lane, qvalid);
             }
-            store_acc(dbase + p.H, ld, row0, S, dk, lane, p.scale, p.scale);
-            store_acc(dbase + 2 * p.H, ld, row0, S, dv, lane, 1.f, 1.f);
+            store_acc(dbase + p.H, ld, row0, len, dk, lane, p.scale, p.scale);
+            store_acc(dbase + 2 * p.H, ld, row0, len, dv, lane, 1.f, 1.f);
         }
         __syncthreads();  // Q / dO tiles and P / dS are free for the next head
     }
 }
 
-template <int NW>
-static int launch_fwd(const AttnParams& p, int nkb, cudaStream_t st) {
+template <int NW, bool VL>
+static int launch_fwd_t(const AttnParams& p, int nkb, cudaStream_t st) {
     const int smem = 2 * 3 * nkb * kTileBytes + 2 * nkb * kBlk * 4;
     static int configured[kMaxDevices] = {0};
-    VB_CHECK_CUDA(ensure_dyn_smem(attn_fwd_head_kernel<NW>, smem, configured));
+    VB_CHECK_CUDA(ensure_dyn_smem(attn_fwd_head_kernel<NW, VL>, smem, configured));
     const int total = p.B * p.A;
     const int grid = total < num_sms() ? total : num_sms();
     ProfScope ps(st, PROF_ATTN_FWD, 4.0 * p.B * p.A * p.S * p.S * kHd, 1);
-    VB_CHECK_CUDA(launch_pdl(attn_fwd_head_kernel<NW>, dim3(grid), dim3(NW * 32), smem, st, p, nkb));
+    VB_CHECK_CUDA(launch_pdl(attn_fwd_head_kernel<NW, VL>, dim3(grid), dim3(NW * 32), smem, st, p, nkb));
     return 0;
+}
+template <int NW>
+static int launch_fwd(const AttnParams& p, int nkb, cudaStream_t st) {
+    return p.cu_seqlens ? launch_fwd_t<NW, true>(p, nkb, st) : launch_fwd_t<NW, false>(p, nkb, st);
 }
 
 // draws the attention-dropout keep bits of the whole layer call (no-op without dropout)
@@ -669,30 +694,38 @@ int attn_fwd_head(const AttnParams& p, int nkb, cudaStream_t st, bool mask_ready
     return 0;
 }
 
-template <int NW>
-static int launch_bwd(const AttnParams& p, int nkb, cudaStream_t st) {
+template <int NW, bool VL>
+static int launch_bwd_t(const AttnParams& p, int nkb, cudaStream_t st) {
     const int per_buf = 4 * nkb * kTileBytes + 3 * nkb * kBlk * 4;
     const int nbuf = 2 * per_buf <= 200 * 1024 ? 2 : 1;
     const int smem = nbuf * per_buf;
     static int configured[kMaxDevices] = {0};
-    VB_CHECK_CUDA(ensure_dyn_smem(attn_bwd_head_kernel<NW>, smem, configured));
+    VB_CHECK_CUDA(ensure_dyn_smem(attn_bwd_head_kernel<NW, VL>, smem, configured));
     const int total = p.B * p.A;
     const int grid = total < num_sms() ? total : num_sms();
     ProfScope ps(st, PROF_ATTN_DKV, 7.0 * p.B * p.A * p.S * p.S * kHd, 1);
-    VB_CHECK_CUDA(launch_pdl(attn_bwd_head_kernel<NW>, dim3(grid), dim3(NW * 32), smem, st, p, nkb, nbuf));
+    VB_CHECK_CUDA(launch_pdl(attn_bwd_head_kernel<NW, VL>, dim3(grid), dim3(NW * 32), smem, st, p, nkb, nbuf));
     return 0;
+}
+template <int NW>
+static int launch_bwd(const AttnParams& p, int nkb, cudaStream_t st) {
+    return p.cu_seqlens ? launch_bwd_t<NW, true>(p, nkb, st) : launch_bwd_t<NW, false>(p, nkb, st);
 }
 
 // P/dS-in-shared-memory variant: only when the whole head fits (S <= ~176); VB_ATTN_BWD_PS=0 disables it
-template <int NW>
-static int launch_bwd_ps(const AttnParams& p, int nkb, int colsP, int smem, cudaStream_t st) {
+template <int NW, bool VL>
+static int launch_bwd_ps_t(const AttnParams& p, int nkb, int colsP, int smem, cudaStream_t st) {
     static int configured[kMaxDevices] = {0};
-    VB_CHECK_CUDA(ensure_dyn_smem(attn_bwd_head_ps_kernel<NW>, smem, configured));
+    VB_CHECK_CUDA(ensure_dyn_smem(attn_bwd_head_ps_kernel<NW, VL>, smem, configured));
     const int total = p.B * p.A;
     const int grid = total < num_sms() ? total : num_sms();
     ProfScope ps(st, PROF_ATTN_DKV, 5.0 * p.B * p.A * p.S * p.S * kHd, 1);
-    VB_CHECK_CUDA(launch_pdl(attn_bwd_head_ps_kernel<NW>, dim3(grid), dim3(NW * 32), smem, st, p, nkb, colsP));
+    VB_CHECK_CUDA(launch_pdl(attn_bwd_head_ps_kernel<NW, VL>, dim3(grid), dim3(NW * 32), smem, st, p, nkb, colsP));
     return 0;
+}
+template <int NW>
+static int launch_bwd_ps(const AttnParams& p, int nkb, int colsP, int smem, cudaStream_t st) {
+    return p.cu_seqlens ? launch_bwd_ps_t<NW, true>(p, nkb, colsP, smem, st) : launch_bwd_ps_t<NW, false>(p, nkb, colsP, smem, st);
 }
 
 static int bwd_ps_smem(const AttnParams& p, int nkb, int* colsP) {
@@ -709,10 +742,16 @@ static int bwd_ps_smem(const AttnParams& p, int nkb, int* colsP) {
 }
 
 // D[b, h, q] = sum_d dO * O  (the softmax-backward row term), HBM-bound pre-pass shared by the backward kernels
+// (varlen: over the `total` packed rows, drow [A, total])
 int attn_delta(const AttnParams& p, cudaStream_t st) {
-    const long long rows = static_cast<long long>(p.B) * p.S;
     ProfScope ps(st, PROF_ATTN_DQ, 1.0 * p.B * p.A * p.S * p.S * kHd, 1);
-    VB_CHECK_CUDA(launch_pdl(attn_delta_kernel, dim3(static_cast<int>((rows + 7) / 8)), dim3(256), 0, st, p.ctx, p.dctx, p.drow, p.B,
+    if (p.cu_seqlens != nullptr) {
+        VB_CHECK_CUDA(launch_pdl(attn_delta_kernel<true>, dim3(static_cast<int>((p.total + 7LL) / 8)), dim3(256), 0, st, p.ctx, p.dctx,
+                                 p.drow, 1, p.total, p.A, p.H));
+        return 0;
+    }
+    const long long rows = static_cast<long long>(p.B) * p.S;
+    VB_CHECK_CUDA(launch_pdl(attn_delta_kernel<false>, dim3(static_cast<int>((rows + 7) / 8)), dim3(256), 0, st, p.ctx, p.dctx, p.drow, p.B,
                              p.S, p.A, p.H));
     return 0;
 }

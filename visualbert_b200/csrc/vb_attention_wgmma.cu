@@ -12,6 +12,10 @@
 //             the epilogue of the GEMM that produced dO, or from attn_delta.
 // Rows and keys >= S inside the last 64-row tile: keys get a -inf bias (probability 0), queries are never stored and, in
 // the backward, get lse = +inf (probability 0), so whatever the tile holds there contributes nothing.
+// Variable-length calls (VL): the CTA of (b, h) loads the packed rows cu[b] + 64 kb .. from a tensor map of `total` rows, only
+// for the key blocks kb < ceil(len / 64) of its own sequence. Tile rows past len belong to the next sequence (or are TMA's
+// zero fill past `total`): the same -inf bias / +inf lse rule makes them contribute nothing, and no ctx, dQ, dK or dV row past
+// len is stored. Warpgroups whose 64-row block starts past len issue no MMAs.
 #include "vb_attention.cuh"
 
 namespace vb {
@@ -68,7 +72,7 @@ __device__ __forceinline__ void store_tile(uint32_t tile, int r, const float (&x
 // ------------------------------------------------------------------------------------------------
 // forward
 // ------------------------------------------------------------------------------------------------
-template <int NKB>
+template <int NKB, bool VL = false>
 __global__ void __launch_bounds__(NKB * 128, 1)
 attn_fwd_wgmma_kernel(const __grid_constant__ CUtensorMap tmQKV, const AttnParams p) {
     extern __shared__ uint8_t smem_raw[];
@@ -79,8 +83,13 @@ attn_fwd_wgmma_kernel(const __grid_constant__ CUtensorMap tmQKV, const AttnParam
     float* sbias = reinterpret_cast<float*>(smem + 3 * NKB * kWgTile);
     const uint32_t bar = base + 3 * NKB * kWgTile + NKB * kBlk * 4;
     const int tid = threadIdx.x, wg = tid >> 7, warp = (tid >> 5) & 3, lane = tid & 31, g = lane >> 2, t = lane & 3;
-    const int item = blockIdx.x, b = item / p.A, h = item % p.A, S = p.S;
+    const int item = blockIdx.x, b = item / p.A, h = item % p.A;
     const unsigned bh = static_cast<unsigned>(item);
+    const SeqSpan sp = seq_span<VL>(p, b, h);
+    const int S = sp.len;                                 // rows of this sequence
+    const int nkv = VL ? (S + kBlk - 1) / kBlk : NKB;     // its key blocks
+    const int row0 = VL ? static_cast<int>(sp.row0) : b * S;
+    if (VL && S == 0) return;                             // an empty sequence writes nothing
 
     if (tid == 0) {
         tma_prefetch_desc(&tmQKV);
@@ -91,13 +100,14 @@ attn_fwd_wgmma_kernel(const __grid_constant__ CUtensorMap tmQKV, const AttnParam
     pdl_trigger();
     pdl_wait();
     if (tid == 0) {
-        mbar_arrive_expect_tx(bar, 3 * NKB * kWgTile);
+        mbar_arrive_expect_tx(bar, 3 * nkv * kWgTile);
 #pragma unroll
         for (int m = 0; m < 3; ++m)
 #pragma unroll
-            for (int kb = 0; kb < NKB; ++kb) tma_load_2d(base + (m * NKB + kb) * kWgTile, &tmQKV, bar, m * p.H + h * kHd, b * S + kb * kBlk);
+            for (int kb = 0; kb < NKB; ++kb)
+                if (!VL || kb < nkv) tma_load_2d(base + (m * NKB + kb) * kWgTile, &tmQKV, bar, m * p.H + h * kHd, row0 + kb * kBlk);
     }
-    for (int i = tid; i < NKB * kBlk; i += NKB * 128) sbias[i] = i < S ? p.mask_bias[static_cast<long long>(b) * S + i] * kLog2e : -INFINITY;
+    for (int i = tid; i < NKB * kBlk; i += NKB * 128) sbias[i] = key_bias2<VL>(p, b, i, S);
     const int q0 = wg * kBlk + warp * 16 + g;   // this lane's rows: q0, q0 + 8
     unsigned long long keep[NKB][2];
 #pragma unroll
@@ -106,12 +116,14 @@ attn_fwd_wgmma_kernel(const __grid_constant__ CUtensorMap tmQKV, const AttnParam
         keep[kb][1] = keep_word(p, bh, q0 + 8, kb, NKB, t);
     }
     __syncthreads();
+    if (VL && wg >= nkv) return;   // query block past the sequence's end (warpgroup 0 stays and waits for the loads)
     mbar_wait(bar, 0);
 
     float s[NKB][32];
     wgmma_fence();
 #pragma unroll
-    for (int kb = 0; kb < NKB; ++kb) qk_block<NKB>(s[kb], sQ, sK, wg, kb);
+    for (int kb = 0; kb < NKB; ++kb)
+        if (!VL || kb < nkv) qk_block<NKB>(s[kb], sQ, sK, wg, kb);
     wgmma_commit();
     wgmma_wait<0>();
 
@@ -122,6 +134,7 @@ attn_fwd_wgmma_kernel(const __grid_constant__ CUtensorMap tmQKV, const AttnParam
     for (int kb = 0; kb < NKB; ++kb)
 #pragma unroll
         for (int j = 0; j < 8; ++j) {
+            if (VL && kb >= nkv) break;
             const float b0 = sbias[kb * kBlk + 8 * j + 2 * t], b1 = sbias[kb * kBlk + 8 * j + 2 * t + 1];
             s[kb][4 * j] = fmaf(s[kb][4 * j], sc2, b0); s[kb][4 * j + 1] = fmaf(s[kb][4 * j + 1], sc2, b1);
             s[kb][4 * j + 2] = fmaf(s[kb][4 * j + 2], sc2, b0); s[kb][4 * j + 3] = fmaf(s[kb][4 * j + 3], sc2, b1);
@@ -140,6 +153,7 @@ attn_fwd_wgmma_kernel(const __grid_constant__ CUtensorMap tmQKV, const AttnParam
         for (int j = 0; j < 8; ++j)
 #pragma unroll
             for (int c = 0; c < 4; ++c) {
+                if (VL && kb >= nkv) break;
                 const int r = c >> 1;
                 float e = fast_ex2(s[kb][4 * j + c] - mx[r]);
                 l[r] += e;
@@ -158,21 +172,23 @@ attn_fwd_wgmma_kernel(const __grid_constant__ CUtensorMap tmQKV, const AttnParam
 #pragma unroll
     for (int kb = 0; kb < NKB; ++kb)
 #pragma unroll
-        for (int kk = 0; kk < 4; ++kk) pack_afrag(pa[kb][kk], s[kb], kk);
+        for (int kk = 0; kk < 4; ++kk)
+            if (!VL || kb < nkv) pack_afrag(pa[kb][kk], s[kb], kk);
     float o[32];
     wgmma_fence();
 #pragma unroll
     for (int kb = 0; kb < NKB; ++kb)
 #pragma unroll
         for (int kk = 0; kk < 4; ++kk)
-            wgmma_m64n64k16_rs<1>(o, pa[kb][kk], tile_desc(sV + kb * kWgTile + kk * 2048), (kb > 0 || kk > 0) ? 1u : 0u);
+            if (!VL || kb < nkv)
+                wgmma_m64n64k16_rs<1>(o, pa[kb][kk], tile_desc(sV + kb * kWgTile + kk * 2048), (kb > 0 || kk > 0) ? 1u : 0u);
     wgmma_commit();
     wgmma_wait<0>();
 
     const float dscale = p.drop_scale != 0.f ? p.drop_scale : 1.f;
-    store_rows(p.ctx + static_cast<long long>(b) * S * p.H + h * kHd, p.H, q0, S, o, t, dscale / l[0], dscale / l[1]);
+    store_rows(p.ctx + (VL ? sp.row0 : static_cast<long long>(b) * S) * p.H + h * kHd, p.H, q0, S, o, t, dscale / l[0], dscale / l[1]);
     if (t == 0 && p.lse != nullptr) {
-        float* lse = p.lse + static_cast<long long>(item) * S;
+        float* lse = p.lse + (VL ? sp.stat0 : static_cast<long long>(item) * S);
         if (q0 < S) lse[q0] = (mx[0] + log2f(l[0])) * 0.6931471805599453f;
         if (q0 + 8 < S) lse[q0 + 8] = (mx[1] + log2f(l[1])) * 0.6931471805599453f;
     }
@@ -181,7 +197,7 @@ attn_fwd_wgmma_kernel(const __grid_constant__ CUtensorMap tmQKV, const AttnParam
 // ------------------------------------------------------------------------------------------------
 // backward
 // ------------------------------------------------------------------------------------------------
-template <int NKB>
+template <int NKB, bool VL = false>
 __global__ void __launch_bounds__(NKB * 128, 1)
 attn_bwd_wgmma_kernel(const __grid_constant__ CUtensorMap tmQKV, const __grid_constant__ CUtensorMap tmDO, const AttnParams p) {
     extern __shared__ uint8_t smem_raw[];
@@ -193,9 +209,18 @@ attn_bwd_wgmma_kernel(const __grid_constant__ CUtensorMap tmQKV, const __grid_co
     float* sbias = reinterpret_cast<float*>(smem + (4 * NKB + NKB * NKB) * kWgTile);
     const uint32_t bar = base + (4 * NKB + NKB * NKB) * kWgTile + NKB * kBlk * 4;
     const int tid = threadIdx.x, wg = tid >> 7, warp = (tid >> 5) & 3, lane = tid & 31, g = lane >> 2, t = lane & 3;
-    const int item = blockIdx.x, b = item / p.A, h = item % p.A, S = p.S;
+    const int item = blockIdx.x, b = item / p.A, h = item % p.A;
     const unsigned bh = static_cast<unsigned>(item);
     const long long ld = 3LL * p.H;
+    const SeqSpan sp = seq_span<VL>(p, b, h);
+    const int S = sp.len;
+    const int nkv = VL ? (S + kBlk - 1) / kBlk : NKB;
+    const int row0 = VL ? static_cast<int>(sp.row0) : b * S;
+    const long long stat0 = VL ? sp.stat0 : static_cast<long long>(item) * S;
+    if (VL && S == 0) return;
+    // warpgroups whose 64-row block (of queries in pass 1 / 2, of keys for dV / dK) starts past the sequence's end issue no MMAs
+    // but stay for the block-wide barriers
+    const bool wg_live = !VL || wg < nkv;
 
     if (tid == 0) {
         tma_prefetch_desc(&tmQKV);
@@ -207,23 +232,24 @@ attn_bwd_wgmma_kernel(const __grid_constant__ CUtensorMap tmQKV, const __grid_co
     pdl_trigger();
     pdl_wait();
     if (tid == 0) {
-        mbar_arrive_expect_tx(bar, 4 * NKB * kWgTile);
+        mbar_arrive_expect_tx(bar, 4 * nkv * kWgTile);
 #pragma unroll
         for (int kb = 0; kb < NKB; ++kb) {
+            if (VL && kb >= nkv) break;
 #pragma unroll
-            for (int m = 0; m < 3; ++m) tma_load_2d(base + (m * NKB + kb) * kWgTile, &tmQKV, bar, m * p.H + h * kHd, b * S + kb * kBlk);
-            tma_load_2d(sDO + kb * kWgTile, &tmDO, bar, h * kHd, b * S + kb * kBlk);
+            for (int m = 0; m < 3; ++m) tma_load_2d(base + (m * NKB + kb) * kWgTile, &tmQKV, bar, m * p.H + h * kHd, row0 + kb * kBlk);
+            tma_load_2d(sDO + kb * kWgTile, &tmDO, bar, h * kHd, row0 + kb * kBlk);
         }
     }
-    for (int i = tid; i < NKB * kBlk; i += NKB * 128) sbias[i] = i < S ? p.mask_bias[static_cast<long long>(b) * S + i] * kLog2e : -INFINITY;
+    for (int i = tid; i < NKB * kBlk; i += NKB * 128) sbias[i] = key_bias2<VL>(p, b, i, S);
     const int r0 = warp * 16 + g;   // row of this lane inside its warpgroup's 64-row block (and r0 + 8)
     const int q0 = wg * kBlk + r0;
     float lse2[2], dr[2];
 #pragma unroll
     for (int r = 0; r < 2; ++r) {
         const int q = q0 + 8 * r;
-        lse2[r] = q < S ? p.lse[static_cast<long long>(item) * S + q] * kLog2e : INFINITY;   // +inf: probability 0
-        dr[r] = q < S ? p.drow[static_cast<long long>(item) * S + q] : 0.f;
+        lse2[r] = q < S ? p.lse[stat0 + q] * kLog2e : INFINITY;   // +inf: probability 0
+        dr[r] = q < S ? p.drow[stat0 + q] : 0.f;
     }
     unsigned long long keep[NKB][2];
 #pragma unroll
@@ -244,11 +270,12 @@ attn_bwd_wgmma_kernel(const __grid_constant__ CUtensorMap tmQKV, const __grid_co
                 s[4 * j + c] = fast_ex2(fmaf(s[4 * j + c], sc2, sbias[kb * kBlk + 8 * j + 2 * t + (c & 1)]) - lse2[c >> 1]);
     };
     auto kept = [&](int kb, int j, int c) { return ((keep[kb][c >> 1] >> (8 * j + (c & 1))) & 1ull) != 0; };
-    bf16* dqkv = p.dqkv + static_cast<long long>(b) * S * ld + h * kHd;
+    bf16* dqkv = p.dqkv + (VL ? sp.row0 : static_cast<long long>(b) * S) * ld + h * kHd;
 
     // ---- pass 1: P_drop -> shared memory; dV of this warpgroup's key block = P_drop^T dO ----
 #pragma unroll
     for (int kb = 0; kb < NKB; ++kb) {
+        if (VL && (!wg_live || kb >= nkv)) break;
         float s[32];
         wgmma_fence();
         qk_block<NKB>(s, sQ, sK, wg, kb);
@@ -263,15 +290,16 @@ attn_bwd_wgmma_kernel(const __grid_constant__ CUtensorMap tmQKV, const __grid_co
     }
     fence_proxy_async_smem();   // generic-proxy stores -> visible to the wgmma (async proxy) reads below
     __syncthreads();
-    {
+    if (wg_live) {
         float acc[32];
         wgmma_fence();
 #pragma unroll
         for (int qb = 0; qb < NKB; ++qb)
 #pragma unroll
             for (int kk = 0; kk < 4; ++kk)
-                wgmma_m64n64k16_ss<1, 1>(acc, tile_desc(sPS + (qb * NKB + wg) * kWgTile + kk * 2048), tile_desc(sDO + qb * kWgTile + kk * 2048),
-                                         (qb > 0 || kk > 0) ? 1u : 0u);
+                if (!VL || qb < nkv)
+                    wgmma_m64n64k16_ss<1, 1>(acc, tile_desc(sPS + (qb * NKB + wg) * kWgTile + kk * 2048),
+                                             tile_desc(sDO + qb * kWgTile + kk * 2048), (qb > 0 || kk > 0) ? 1u : 0u);
         wgmma_commit();
         wgmma_wait<0>();
         store_rows(dqkv + 2 * p.H, ld, q0, S, acc, t, 1.f, 1.f);   // rows of this warpgroup's block are keys here
@@ -282,6 +310,7 @@ attn_bwd_wgmma_kernel(const __grid_constant__ CUtensorMap tmQKV, const __grid_co
     float dq[32];
 #pragma unroll
     for (int kb = 0; kb < NKB; ++kb) {
+        if (VL && (!wg_live || kb >= nkv)) break;
         float s[32], dp[32];
         wgmma_fence();
         qk_block<NKB>(s, sQ, sK, wg, kb);
@@ -309,18 +338,19 @@ attn_bwd_wgmma_kernel(const __grid_constant__ CUtensorMap tmQKV, const __grid_co
         wgmma_commit();
         wgmma_wait<0>();   // the A fragments live in registers that the next block overwrites
     }
-    store_rows(dqkv, ld, q0, S, dq, t, p.scale, p.scale);
+    if (wg_live) store_rows(dqkv, ld, q0, S, dq, t, p.scale, p.scale);
     fence_proxy_async_smem();
     __syncthreads();
-    {
+    if (wg_live) {
         float acc[32];
         wgmma_fence();
 #pragma unroll
         for (int qb = 0; qb < NKB; ++qb)
 #pragma unroll
             for (int kk = 0; kk < 4; ++kk)
-                wgmma_m64n64k16_ss<1, 1>(acc, tile_desc(sPS + (qb * NKB + wg) * kWgTile + kk * 2048), tile_desc(sQ + qb * kWgTile + kk * 2048),
-                                         (qb > 0 || kk > 0) ? 1u : 0u);
+                if (!VL || qb < nkv)
+                    wgmma_m64n64k16_ss<1, 1>(acc, tile_desc(sPS + (qb * NKB + wg) * kWgTile + kk * 2048),
+                                             tile_desc(sQ + qb * kWgTile + kk * 2048), (qb > 0 || kk > 0) ? 1u : 0u);
         wgmma_commit();
         wgmma_wait<0>();
         store_rows(dqkv + p.H, ld, q0, S, acc, t, p.scale, p.scale);
@@ -335,18 +365,18 @@ bool attn_wgmma_supported(const AttnParams& p) {
            (p.dctx == nullptr || (reinterpret_cast<uintptr_t>(p.dctx) & 15) == 0);
 }
 
-template <int NKB>
+template <int NKB, bool VL = false>
 static int launch_fwd_wgmma(const AttnParams& p, const CUtensorMap& tq, cudaStream_t st) {
-    auto kern = attn_fwd_wgmma_kernel<NKB>;
+    auto kern = attn_fwd_wgmma_kernel<NKB, VL>;
     static int configured[kMaxDevices] = {0};
     VB_CHECK_CUDA(ensure_dyn_smem(kern, AttnSmem<NKB>::FWD_BYTES, configured));
     ProfScope ps(st, PROF_ATTN_FWD, 4.0 * p.B * p.A * p.S * p.S * kHd, 1);
     VB_CHECK_CUDA(launch_pdl(kern, dim3(p.B * p.A), dim3(NKB * 128), AttnSmem<NKB>::FWD_BYTES, st, tq, p));
     return 0;
 }
-template <int NKB>
+template <int NKB, bool VL = false>
 static int launch_bwd_wgmma(const AttnParams& p, const CUtensorMap& tq, const CUtensorMap& td, cudaStream_t st) {
-    auto kern = attn_bwd_wgmma_kernel<NKB>;
+    auto kern = attn_bwd_wgmma_kernel<NKB, VL>;
     static int configured[kMaxDevices] = {0};
     VB_CHECK_CUDA(ensure_dyn_smem(kern, AttnSmem<NKB>::BWD_BYTES, configured));
     ProfScope ps(st, PROF_ATTN_DKV, 10.0 * p.B * p.A * p.S * p.S * kHd, 1);
@@ -361,9 +391,15 @@ int attn_fwd_wgmma(const AttnParams& p, cudaStream_t st, bool mask_ready) {
         if (rc) return rc;
     }
     CUtensorMap tq;
-    int rc = make_tmap_bf16(&tq, p.qkv, 3ull * p.H, static_cast<uint64_t>(p.B) * p.S, 3ull * p.H, kBlk);
+    const bool vl = p.cu_seqlens != nullptr;
+    const uint64_t rows = vl ? static_cast<uint64_t>(p.total) : static_cast<uint64_t>(p.B) * p.S;
+    int rc = make_tmap_bf16(&tq, p.qkv, 3ull * p.H, rows, 3ull * p.H, kBlk);
     if (rc) return rc;
-    if (nkb == 1) rc = launch_fwd_wgmma<1>(p, tq, st);
+    if (vl) {
+        if (nkb == 1) rc = launch_fwd_wgmma<1, true>(p, tq, st);
+        else if (nkb == 2) rc = launch_fwd_wgmma<2, true>(p, tq, st);
+        else rc = launch_fwd_wgmma<3, true>(p, tq, st);
+    } else if (nkb == 1) rc = launch_fwd_wgmma<1>(p, tq, st);
     else if (nkb == 2) rc = launch_fwd_wgmma<2>(p, tq, st);
     else rc = launch_fwd_wgmma<3>(p, tq, st);
     if (rc) return rc;
@@ -379,11 +415,17 @@ int attn_bwd_wgmma(const AttnParams& p, cudaStream_t st, bool delta_ready) {
         if (rc) return rc;
     }
     CUtensorMap tq, td;
-    rc = make_tmap_bf16(&tq, p.qkv, 3ull * p.H, static_cast<uint64_t>(p.B) * p.S, 3ull * p.H, kBlk);
+    const bool vl = p.cu_seqlens != nullptr;
+    const uint64_t rows = vl ? static_cast<uint64_t>(p.total) : static_cast<uint64_t>(p.B) * p.S;
+    rc = make_tmap_bf16(&tq, p.qkv, 3ull * p.H, rows, 3ull * p.H, kBlk);
     if (rc) return rc;
-    rc = make_tmap_bf16(&td, p.dctx, static_cast<uint64_t>(p.H), static_cast<uint64_t>(p.B) * p.S, static_cast<uint64_t>(p.H), kBlk);
+    rc = make_tmap_bf16(&td, p.dctx, static_cast<uint64_t>(p.H), rows, static_cast<uint64_t>(p.H), kBlk);
     if (rc) return rc;
-    if (nkb == 1) rc = launch_bwd_wgmma<1>(p, tq, td, st);
+    if (vl) {
+        if (nkb == 1) rc = launch_bwd_wgmma<1, true>(p, tq, td, st);
+        else if (nkb == 2) rc = launch_bwd_wgmma<2, true>(p, tq, td, st);
+        else rc = launch_bwd_wgmma<3, true>(p, tq, td, st);
+    } else if (nkb == 1) rc = launch_bwd_wgmma<1>(p, tq, td, st);
     else if (nkb == 2) rc = launch_bwd_wgmma<2>(p, tq, td, st);
     else rc = launch_bwd_wgmma<3>(p, tq, td, st);
     if (rc) return rc;

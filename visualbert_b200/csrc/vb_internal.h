@@ -20,6 +20,13 @@ int attn_mask_async(void* keep, int B, int S, int A, int H, float dropout_p, uns
 int attn_bwd(const void* qkv, const float* mask_bias, const void* ctx, const float* lse, const void* keep,
              const void* dctx, void* dqkv, float* drow, int B, int S, int A, int H, float dropout_p,
              unsigned long long seed, unsigned stream_id, cudaStream_t st, bool delta_ready = false);
+// variable-length attention: sequence b owns packed rows [cu_seqlens[b], cu_seqlens[b+1]) (device), at most max_seq of them;
+// lse / drow are [A, total]
+int attn_fwd_varlen(const void* qkv, const int* cu_seqlens, void* ctx, float* lse, void* keep, int B, int max_seq, int total,
+                    int A, int H, float dropout_p, unsigned long long seed, unsigned stream_id, cudaStream_t st, bool mask_ready = false);
+int attn_bwd_varlen(const void* qkv, const int* cu_seqlens, const void* ctx, const float* lse, const void* keep,
+                    const void* dctx, void* dqkv, float* drow, int B, int max_seq, int total, int A, int H, float dropout_p,
+                    unsigned long long seed, unsigned stream_id, cudaStream_t st, bool delta_ready = false);
 // true when attn_bwd for this shape runs the kernel that takes D = rowsum(dO * O) from `drow` (so a caller may provide it)
 bool attn_bwd_takes_delta(const void* qkv, const void* dctx, void* dqkv, int B, int S, int A, int H);
 long long attn_keep_bytes(int B, int S, int A);

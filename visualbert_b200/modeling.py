@@ -208,7 +208,18 @@ class BertEncoder(nn.Module):
         self.layer = nn.ModuleList([BertLayer(config, i) for i in range(config.num_hidden_layers)])
         self.output_attention_weights = getattr(config, "output_attention_weights", False)
 
-    def forward(self, hidden_states, attention_mask, output_all_encoded_layers=True, seed=0):
+    def forward(self, hidden_states, attention_mask, output_all_encoded_layers=True, seed=0, varlen=None):
+        """varlen (ops.unpad_plan): unpadded call — hidden_states are the [total, H] packed valid rows, attention_mask is
+        ignored, and every returned layer is [total, H]. It always runs the whole-encoder call (there is no per-layer
+        varlen path), so it cannot serve attention weights or gradients through intermediate layers."""
+        if varlen is not None:
+            if self.output_attention_weights or (output_all_encoded_layers and torch.is_grad_enabled() and self.training):
+                raise ValueError("unpadded encoder: attention weights and gradients through intermediate layers need the "
+                                 "padded per-layer path")
+            if len(self.layer) == 0:
+                return [hidden_states]
+            ys = ops.bert_encoder(hidden_states.to(torch.bfloat16), None, self._fused_meta(seed, varlen), self._fused_params())
+            return list(ys) if output_all_encoded_layers else [ys[-1]]
         if attention_mask.dim() == 4:
             attention_mask = attention_mask[:, 0, 0, :]
         fused = (not self.output_attention_weights and hidden_states.is_cuda and len(self.layer) > 0
@@ -216,17 +227,8 @@ class BertEncoder(nn.Module):
                  and os.environ.get("VB_ENCODER_FUSED", "1") != "0")
         if fused:
             # one C call for the whole stack (vb_encoder_fwd / vb_encoder_bwd, one activation arena)
-            l0 = self.layer[0]
-            train = self.training
-            plan = self.__dict__.get("_plan")
-            if plan is None:
-                plan = self.__dict__["_plan"] = ops.EncoderPlan()
-            meta = dict(heads=l0.attention.self.num_attention_heads, layer_index0=l0.layer_index,
-                        hidden_dropout=l0.hidden_dropout_prob if train else 0.0,
-                        attn_dropout=l0.attention_probs_dropout_prob if train else 0.0, seed=int(seed), train=train,
-                        caches=[l._weights for l in self.layer], plan=plan)
-            params = [p for l in self.layer for p in l._params()]
-            ys = ops.bert_encoder(hidden_states.to(torch.bfloat16), attention_mask.float().contiguous(), meta, params)
+            ys = ops.bert_encoder(hidden_states.to(torch.bfloat16), attention_mask.float().contiguous(), self._fused_meta(seed),
+                                  self._fused_params())
             return list(ys) if output_all_encoded_layers else [ys[-1]]
         outs, attn = [], []
         for layer in self.layer:
@@ -238,6 +240,23 @@ class BertEncoder(nn.Module):
         if not output_all_encoded_layers:
             outs.append(hidden_states)
         return (outs, attn) if self.output_attention_weights else outs
+
+    def _fused_meta(self, seed, varlen=None):
+        l0 = self.layer[0]
+        train = self.training
+        plan = self.__dict__.get("_plan")
+        if plan is None:
+            plan = self.__dict__["_plan"] = ops.EncoderPlan()
+        meta = dict(heads=l0.attention.self.num_attention_heads, layer_index0=l0.layer_index,
+                    hidden_dropout=l0.hidden_dropout_prob if train else 0.0,
+                    attn_dropout=l0.attention_probs_dropout_prob if train else 0.0, seed=int(seed), train=train,
+                    caches=[l._weights for l in self.layer], plan=plan)
+        if varlen is not None:
+            meta["varlen"] = varlen
+        return meta
+
+    def _fused_params(self):
+        return [p for l in self.layer for p in l._params()]
 
 
 class BertPooler(nn.Module):
@@ -460,6 +479,7 @@ class BertVisualModel(PreTrainedBertModel):
             self.additional_layer = BertLayer(config, config.num_hidden_layers)
         self.output_attention_weights = getattr(config, "output_attention_weights", False)
         self.apply(self.init_bert_weights)
+        self._unpadded = False
         self._step = 0
         # base of the counter-hash dropout streams: follows torch.manual_seed (so runs are reproducible the torch way);
         # the data-parallel rank is mixed in per forward (next_seed) so replicas draw different masks
@@ -515,6 +535,45 @@ class BertVisualModel(PreTrainedBertModel):
             self.__dict__["_bank"] = bank
         bank.refresh(force=self.training)
 
+    def set_unpadded(self, flag=True):
+        """Opt-in unpadded ("variable-length") encoder execution, off by default.
+
+        When on, forward packs the valid positions (attention_mask != 0 over cat(text mask, image mask); any pattern, the
+        rows of an example keep their order) into [total, H] rows, runs the encoder on those rows only through the
+        variable-length kernels (vb_encoder_fwd_varlen: no GEMM, LayerNorm or attention work on padding), and scatters every
+        returned layer back to [B, S, H]. Semantics:
+          - valid positions equal those of the padded path to within rounding: the padded path's key bias of -10000 gives
+            those keys exactly zero probability in fp32 softmax, so the valid rows see the same keys either way;
+          - masked positions are ZERO, where the padded path returns finite values (queries over the valid keys). This shows
+            in output_all_encoded_layers outputs, in the lazily built pretraining `logits` at masked positions, in the pooled
+            output of an example whose first position is masked, and for an example without any valid position, whose rows
+            are all zero.
+        One host synchronisation per forward (the longest sequence and the row count). Not available with
+        bypass_transformer or output_attention_weights, nor, in training mode under grad, with output_all_encoded_layers=True
+        (gradients through intermediate layers): those raise instead of running padded."""
+        flag = bool(flag)
+        if flag and self.bypass_transformer:
+            raise ValueError("set_unpadded: not supported with bypass_transformer")
+        if flag and self.output_attention_weights:
+            raise ValueError("set_unpadded: not supported with output_attention_weights")
+        self._unpadded = flag
+        return self
+
+    def _encode_unpadded(self, x, attention_mask, output_all_encoded_layers, seed):
+        if output_all_encoded_layers and torch.is_grad_enabled() and self.training:
+            raise ValueError("unpadded forward: output_all_encoded_layers=True in training mode under grad needs gradients "
+                             "through intermediate layers, which only the padded per-layer path provides")
+        B, S, H = x.shape
+        vl = ops.unpad_plan(attention_mask != 0)
+        if vl["total"] == 0:   # no valid position anywhere: every row is zero
+            z = x.to(torch.bfloat16) * 0
+            return [z] * (len(self.encoder.layer) if output_all_encoded_layers else 1)
+        idx = vl["index"]
+        packed = x.reshape(B * S, H).index_select(0, idx)
+        ys = self.encoder(packed, None, output_all_encoded_layers=output_all_encoded_layers, seed=seed, varlen=vl)
+        zero = torch.zeros(B * S, H, device=x.device, dtype=torch.bfloat16)
+        return [zero.index_copy(0, idx, y.to(torch.bfloat16)).view(B, S, H) for y in ys]
+
     def next_seed(self):
         """Per-forward dropout seed: forward and backward of one step share it; steps differ."""
         self._step += 1
@@ -542,7 +601,7 @@ class BertVisualModel(PreTrainedBertModel):
             token_type_ids = torch.zeros_like(input_ids)
         seed = self.next_seed() if self.training else 0
         self.refresh_compute_weights()
-        bias = ops.mask_bias(attention_mask, None)
+        bias = None if self._unpadded else ops.mask_bias(attention_mask, None)
         x = self.embeddings(input_ids, token_type_ids, visual_embeddings=visual_embeddings,
                             visual_embeddings_type=visual_embeddings_type, position_embeddings_visual=position_embeddings_visual,
                             image_text_alignment=image_text_alignment, confidence=confidence, seed=seed)
@@ -555,7 +614,11 @@ class BertVisualModel(PreTrainedBertModel):
             text = text[0][-1] if self.output_attention_weights else text[-1]
             final = self.additional_layer(torch.cat((text, x[:, T:]), dim=1), bias, seed)
             return final, self.pooler(final)
-        if self.output_attention_weights:
+        if self._unpadded:
+            if self.bypass_transformer or self.output_attention_weights:
+                raise ValueError("unpadded forward: not supported with bypass_transformer or output_attention_weights")
+            encoded_layers = self._encode_unpadded(x, attention_mask, output_all_encoded_layers, seed)
+        elif self.output_attention_weights:
             encoded_layers, attn = self.encoder(x, bias, output_all_encoded_layers=output_all_encoded_layers, seed=seed)
         else:
             encoded_layers = self.encoder(x, bias, output_all_encoded_layers=output_all_encoded_layers, seed=seed)

@@ -55,6 +55,32 @@ def _scratch(dev, M, H, I, B, A, S, need_drop):
     return w
 
 
+_varlen_scratch_cache = {}
+
+
+def _varlen_scratch(dev, M, H, I, A, need_drop):
+    """Backward scratch of an unpadded encoder call: views of the first M = total rows of buffers that are kept per device and
+    only grow (by at least 1/4, in whole 256-row steps) when a batch has more packed rows than any before. The row count of
+    unpadded batches changes from step to step; a cache keyed on it would reallocate every backward."""
+    key = (dev, H, I, A)
+    c = _varlen_scratch_cache.get(key)
+    if c is None or c["rows"] < M:
+        rows = M if c is None else max(M, c["rows"] + c["rows"] // 4)
+        rows = (rows + 255) // 256 * 256
+        for k in [k for k in _varlen_scratch_cache if k[0] == dev]:   # free the smaller buffers before allocating
+            del _varlen_scratch_cache[k]
+        c = dict(rows=rows, d_pre=torch.empty(rows, H, device=dev, dtype=_BF16), d_pre_drop=None,
+                 d_big=torch.empty(rows, max(I, 3 * H), device=dev, dtype=_BF16),
+                 d_x1=torch.empty(rows, H, device=dev, dtype=_BF16), d_ctx=torch.empty(rows, H, device=dev, dtype=_BF16),
+                 drow=torch.empty(A * rows, device=dev, dtype=torch.float32))
+        _varlen_scratch_cache[key] = c
+    if need_drop and c["d_pre_drop"] is None:
+        c["d_pre_drop"] = torch.empty(c["rows"], H, device=dev, dtype=_BF16)
+    w = {k: (c[k][:M] if c[k] is not None else None) for k in ("d_pre", "d_pre_drop", "d_big", "d_x1", "d_ctx")}
+    w["drow"] = c["drow"][:A * M]   # [heads, total]
+    return w
+
+
 def cast_to_bf16(src, out=None):
     """fp32 -> bf16 through vb_cast_f32_to_bf16 (numel must be a multiple of 8)."""
     _require_cuda(src, "cast_to_bf16")
@@ -291,10 +317,12 @@ class EncoderPlan:
     def __init__(self):
         self.key = None
 
-    def prepare(self, caches, params, B, S, H, A, I, mbias, meta):
+    def prepare(self, caches, params, B, S, H, A, I, mbias, meta, dev, varlen=None):
+        """varlen (unpadded calls): dict(cu_seqlens, max_seq, total); B is then the number of sequences, S = max_seq, and
+        mbias is None."""
         L = len(caches)
         weights = [c.get(*[params[16 * l + i] for i in (0, 2, 4, 6, 10, 12, 1, 3, 5)], train=meta["train"]) for l, c in enumerate(caches)]
-        key = (B, S, H, A, I, L, tuple(w[0].data_ptr() for w in weights), tuple(p.data_ptr() for p in params), mbias.device)
+        key = (B, S, H, A, I, L, tuple(w[0].data_ptr() for w in weights), tuple(p.data_ptr() for p in params), dev)
         if key != self.key:
             self.descs = (_lib.LayerDesc * L)()
             for l in range(L):
@@ -310,33 +338,56 @@ class EncoderPlan:
             d = self.descs[l]
             d.hidden_dropout, d.attn_dropout, d.seed = meta["hidden_dropout"], meta["attn_dropout"], meta["seed"]
             d.layer_index = meta["layer_index0"] + l
-            d.mask_bias = mbias.data_ptr()
+            d.mask_bias = _ptr(mbias)
         off = (ctypes.c_int64 * _lib.VB_ENCODER_ARENA_BUFFERS)()
-        stride = int(_lib.lib().vb_encoder_arena_layout(B, S, H, A, I, 1 if meta["attn_dropout"] > 0 else 0, off))
+        drop = 1 if meta["attn_dropout"] > 0 else 0
+        if varlen is None:
+            stride = int(_lib.lib().vb_encoder_arena_layout(B, S, H, A, I, drop, off))
+        else:
+            stride = int(_lib.lib().vb_encoder_arena_layout_varlen(B, S, varlen["total"], H, A, I, drop, off))
+            if stride < 0:
+                _lib.check(1, "vb_encoder_arena_layout_varlen")
         return weights, stride, list(off)
 
 
 class _EncoderFn(torch.autograd.Function):
-    """BertEncoder (M.py:344-371): all layers in ONE vb_encoder_fwd / vb_encoder_bwd call over one activation arena."""
+    """BertEncoder (M.py:344-371): all layers in ONE vb_encoder_fwd / vb_encoder_bwd call over one activation arena.
+
+    With meta["varlen"] = dict(cu_seqlens, batch, max_seq, total) the call is unpadded: x is [total, H], the packed valid rows
+    (sequence b at rows cu_seqlens[b] .. cu_seqlens[b + 1]), mbias is None, and every output is [total, H]
+    (vb_encoder_fwd_varlen / vb_encoder_bwd_varlen)."""
+
+    @staticmethod
+    def _shape(x, meta):
+        vl = meta.get("varlen")
+        if vl is None:
+            B, S, H = x.shape
+            return B, S, H, B * S, (B, S, H)
+        return vl["batch"], vl["max_seq"], x.shape[-1], vl["total"], (vl["total"], x.shape[-1])
 
     @staticmethod
     def forward(ctx, x, mbias, meta, *params):
         _require_cuda(x, "bert_encoder")
-        B, S, H = x.shape
+        B, S, H, M, oshape = _EncoderFn._shape(x, meta)
+        vl = meta.get("varlen")
         L = len(params) // 16
         I = params[10].shape[0]
         A = meta["heads"]
         x = x.contiguous()
         with torch.cuda.device(x.device):
-            weights, stride, off = meta["plan"].prepare(meta["caches"], params, B, S, H, A, I, mbias, meta)
+            weights, stride, off = meta["plan"].prepare(meta["caches"], params, B, S, H, A, I, mbias, meta, x.device, vl)
             arena = torch.empty(L * stride, device=x.device, dtype=torch.uint8)
             plan = meta["plan"]
-            _lib.check(_lib.lib().vb_encoder_fwd(plan.descs, L, ctypes.c_void_p(x.data_ptr()), ctypes.c_void_p(arena.data_ptr()), _stream()),
-                       "vb_encoder_fwd")
-        n = B * S * H * 2
-        outs = tuple(arena[l * stride + off[13]: l * stride + off[13] + n].view(_BF16).view(B, S, H) for l in range(L))
+            if vl is None:
+                _lib.check(_lib.lib().vb_encoder_fwd(plan.descs, L, ctypes.c_void_p(x.data_ptr()), ctypes.c_void_p(arena.data_ptr()),
+                                                     _stream()), "vb_encoder_fwd")
+            else:
+                _lib.check(_lib.lib().vb_encoder_fwd_varlen(plan.descs, L, vl["cu_seqlens"].data_ptr(), M, x.data_ptr(),
+                                                            arena.data_ptr(), _stream()), "vb_encoder_fwd_varlen")
+        n = M * H * 2
+        outs = tuple(arena[l * stride + off[13]: l * stride + off[13] + n].view(_BF16).view(oshape) for l in range(L))
         ctx.meta, ctx.arena, ctx.params, ctx.weights = meta, arena, params, weights
-        ctx.shape = (B, S, H, A, I, L)
+        ctx.shape = (B, S, H, A, I, L, M, oshape)
         ctx.save_for_backward(x, mbias)
         ctx.mark_non_differentiable(*outs[:-1])
         ctx.set_materialize_grads(False)   # or autograd hands backward a 64 MB zero tensor for each of the L - 1 unused outputs
@@ -346,8 +397,8 @@ class _EncoderFn(torch.autograd.Function):
     def backward(ctx, *douts):
         x, mbias = ctx.saved_tensors
         meta, params = ctx.meta, ctx.params
-        B, S, H, A, I, L = ctx.shape
-        M = B * S
+        B, S, H, A, I, L, M, oshape = ctx.shape
+        vl = meta.get("varlen")
         dev = x.device
         if douts[-1] is None:   # nothing downstream depends on the encoder output
             return (None,) * (3 + 16 * L)
@@ -378,17 +429,23 @@ class _EncoderFn(torch.autograd.Function):
                     o += sz
         hd = meta["hidden_dropout"] > 0
         with torch.cuda.device(dev):
-            w = _scratch(dev, M, H, I, B, A, S, hd)
+            # varlen: row-sized scratch for the `total` packed rows (grow-only cache), drow [heads, total]
+            w = _scratch(dev, M, H, I, B, A, S, hd) if vl is None else _varlen_scratch(dev, M, H, I, A, hd)
             sc = _lib.LayerScratch(**{k: _ptr(t) for k, t in w.items()})
-            dx = torch.empty(B, S, H, device=dev, dtype=_BF16)
+            dx = torch.empty(oshape, device=dev, dtype=_BF16)
             plan = meta["plan"]
             for l in range(L):  # same step, same dropout streams as the forward
                 d = plan.descs[l]
                 d.hidden_dropout, d.attn_dropout, d.seed = meta["hidden_dropout"], meta["attn_dropout"], meta["seed"]
-                d.layer_index, d.mask_bias = meta["layer_index0"] + l, mbias.data_ptr()
-            _lib.check(_lib.lib().vb_encoder_bwd(plan.descs, L, ctypes.c_void_p(x.data_ptr()), ctypes.c_void_p(ctx.arena.data_ptr()),
-                                                 ctypes.c_void_p(dy.data_ptr()), ctypes.c_void_p(dx.data_ptr()), grads, ctypes.byref(sc),
-                                                 _stream()), "vb_encoder_bwd")
+                d.layer_index, d.mask_bias = meta["layer_index0"] + l, _ptr(mbias)
+            if vl is None:
+                _lib.check(_lib.lib().vb_encoder_bwd(plan.descs, L, ctypes.c_void_p(x.data_ptr()), ctypes.c_void_p(ctx.arena.data_ptr()),
+                                                     ctypes.c_void_p(dy.data_ptr()), ctypes.c_void_p(dx.data_ptr()), grads,
+                                                     ctypes.byref(sc), _stream()), "vb_encoder_bwd")
+            else:
+                _lib.check(_lib.lib().vb_encoder_bwd_varlen(plan.descs, L, vl["cu_seqlens"].data_ptr(), M, x.data_ptr(),
+                                                            ctx.arena.data_ptr(), dy.data_ptr(), dx.data_ptr(), grads, ctypes.byref(sc),
+                                                            _stream()), "vb_encoder_bwd_varlen")
         ctx.arena = None
         if direct is not None:
             return (dx, None, None) + (None,) * (16 * L)
@@ -404,9 +461,25 @@ class _EncoderFn(torch.autograd.Function):
 
 def bert_encoder(x, mbias, meta, params):
     """All layers at once. meta: dict(heads, layer_index0, hidden_dropout, attn_dropout, seed, train, caches=[LayerWeights],
-    plan=EncoderPlan); params: 16 tensors per layer in bert_layer order. Returns the tuple of all layer outputs (only
-    the last one is differentiable: a caller that needs gradients through intermediate outputs uses bert_layer)."""
+    plan=EncoderPlan, optional varlen=unpad_plan(...)); params: 16 tensors per layer in bert_layer order. Returns the tuple of
+    all layer outputs (only the last one is differentiable: a caller that needs gradients through intermediate outputs uses
+    bert_layer)."""
     return _EncoderFn.apply(x, mbias, meta, *params)
+
+
+def unpad_plan(valid):
+    """Row bookkeeping of an unpadded call from a [B, S] validity mask (any pattern, not only prefixes): the flat indices
+    b * S + s of the valid positions in row-major order (each example keeps the order of its rows), cu_seqlens (int32
+    [B + 1]: example b owns packed rows cu[b] .. cu[b + 1]), max_seq and total. One host synchronisation (max_seq and total);
+    the index comes from a stable sort instead of nonzero, so it needs none."""
+    B, S = valid.shape
+    valid = valid.reshape(B, S).bool()
+    lens = valid.sum(1, dtype=torch.int32)
+    cu = torch.zeros(B + 1, device=valid.device, dtype=torch.int32)
+    torch.cumsum(lens, 0, dtype=torch.int32, out=cu[1:])
+    max_seq, total = (int(v) for v in torch.stack((lens.max(), cu[-1])).tolist())
+    order = torch.sort((~valid).reshape(-1).to(torch.uint8), stable=True).indices
+    return dict(index=order[:total], cu_seqlens=cu, batch=B, max_seq=max_seq, total=total)
 
 
 def bert_layer(x, mbias, meta, params):
