@@ -57,7 +57,7 @@ typedef struct {
     int32_t M, N, K;
     void* D; int64_t ldd;
     int32_t d_fp32;   /* 0: D is bf16; 1: D is fp32 and the result is ACCUMULATED into D (red.add) */
-    int32_t splits;   /* split-K factor (d_fp32 only; 0/1 = no split) */
+    int32_t splits;   /* unused: the split-K factor of a d_fp32 output is chosen from the shape (field kept for the ABI) */
     const float* bias;            /* fp32 [N] or NULL */
     const void* addend; int64_t ld_add; /* bf16 [M,N] added after bias/dropout (residual) or NULL */
     int32_t epilogue;             /* VB_EPI_* */

@@ -47,9 +47,6 @@ static vb_gemm_args wgrad_args(const void* dY, const void* X, float* dW, int M, 
     memset(&a, 0, sizeof(a));
     a.A = dY; a.lda = N; a.a_mn_major = 1; a.B = X; a.ldb = K; a.b_mn_major = 1;
     a.M = N; a.N = K; a.K = M; a.D = dW; a.ldd = K; a.d_fp32 = 1;
-    const int tiles = ((N + 127) / 128) * ((K + 255) / 256);
-    int splits = (2 * num_sms()) / tiles;
-    a.splits = splits < 1 ? 1 : splits;
     return a;
 }
 

@@ -116,14 +116,15 @@ bool gemm_delta_ok(int M, int N);
 struct TileCoord {
     int m_blk, n_blk, kb_begin, kb_end;
 };
-// Tile order: the split index runs fastest, then the dimension with FEWER blocks (m_fast: there are fewer m-blocks), so that the
-// tiles in flight at any time share the slabs of the operand that spans the dimension with MORE blocks — the big one, which
-// must not be fetched from DRAM once per block of the other dimension (FFN-down weight gradient: M = 768, N = 3072, B = gelu(u)
-// is several times the L2).
+// Tile order: the split index runs slowest, so that the CTAs in flight at any time work on one or two k-ranges; within a split
+// the dimension with FEWER blocks runs fastest (m_fast: there are fewer m-blocks), so that those CTAs share the slabs of the
+// operand that spans the dimension with MORE blocks — the big one, which must not be fetched from DRAM once per block of the
+// other dimension (FFN-down weight gradient: M = 768, N = 3072, B = gelu(u) is several times the L2).
 __device__ __forceinline__ TileCoord decode_tile(int t, int n_blocks, int splits, int k_blocks, int m_blocks, bool m_fast) {
     TileCoord c;
-    const int split = t % splits;
-    const int mn = t / splits;
+    const int tiles = m_blocks * n_blocks;
+    const int split = t / tiles;
+    const int mn = t - split * tiles;
     if (m_fast) {
         c.m_blk = mn % m_blocks;
         c.n_blk = mn / m_blocks;
@@ -163,8 +164,8 @@ __device__ __forceinline__ void store16_bf16(bf16* p, const float (&f)[16]) {
 // times larger than one specialised path, and instruction-cache misses then stall the epilogue. A specialised kernel carries
 // only its path.
 // _T: gelu'(u) is kept in the TILE-NATIVE layout (vb_gemm_args.gp_tiled): the only reader of that tensor is the epilogue of the
-// backward GEMM, where the same thread holds the same 16 columns — so it is written and read as whole 1 KB warp blocks
-// (lane l: 32 bytes at block + 32 l) instead of 32-byte pieces of 32 different rows.
+// backward GEMM, where the same thread holds the same 16 columns — so it is stored in 1 KB blocks (one per epilogue warp and
+// chunk, row r of the warp's 32 at block + 32 r bytes) that both epilogues access in contiguous pieces.
 // EPI_DELTA: plain bf16 store plus the attention backward's D[b, head, s] = sum_d dO[row, head, d] * O[row, head, d] (vb_gemm_args.delta_*):
 // the GEMM that PRODUCES dO (input gradient of attention.output.dense) has, in each epilogue thread, 128 consecutive columns of one row —
 // two whole heads — so the row-wise dot product with O needs no exchange; O is read like a residual operand.
@@ -318,7 +319,7 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
     float* sbias = reinterpret_cast<float*>(smem + C::BIAS_OFF);
     const bool has_bias = p.bias != nullptr;
     if (has_bias) {   // with split-K the bias belongs to the whole sum: only split 0 adds it, the other splits stage zeros
-        const bool mine = p.splits == 1 || (blockIdx.x % p.splits) == 0;
+        const bool mine = tc.kb_begin == 0;
         for (int i = et; i < BLOCK_N; i += kEpiWarps * 32) {
             const int col = tc.n_blk * BLOCK_N + i;
             sbias[i] = (mine && col < p.N) ? __ldg(p.bias + col) : 0.f;
@@ -357,34 +358,44 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
     }
 
     // ---------------- epilogue ----------------
-    // Thread -> element map: epilogue warp ew owns rows 32 (ew % 4) .. + 31 (one per lane) and the column half ew / 4 of the tile,
-    // in 16-column chunks. Operands read by the epilogue (residual / gelu') are requested before the accumulators are staged.
+    // Thread -> element map: epilogue warp ew owns rows 32 (ew % 4) .. + 31 and the column half ew / 4 of the tile, in 16-column
+    // chunks; in step j a thread holds one chunk of one row. By default lane l takes chunk l / RPI of row RPI j + l % RPI of the
+    // warp's 32, so that one warp access covers RPI whole half-rows (RPI x 256 contiguous bytes of a bf16 output instead of 32
+    // bytes of 32 rows), and the staging reads of a quarter-warp hit 8 distinct 4-bank groups (ACC_LD = 4 mod 32). EPI_DELTA keeps
+    // one row per lane and chunk j in step j: a thread then holds whole heads of its row.
+    // Operands read by the epilogue (residual / gelu') are requested before the accumulators are staged.
     const int ew = warp - 4;
     const int q = ew & 3, half = ew >> 2;
-    const int lrow = q * 32 + lane;
-    const int row = tc.m_blk * BLOCK_M + lrow;
     const int col0 = tc.n_blk * BLOCK_N + half * (BLOCK_N / 2);
     constexpr int NCH = BLOCK_N / 2 / 16;
-    // tile-native gelu'(u) (M, N multiples of 256; vbert_b200.h): 1 KB warp blocks, lane l at + 32 l bytes
-    const long long gp_tile_off =
-        ((((static_cast<long long>(tc.m_blk >> 1) * n_blocks + tc.n_blk) * 2 + (tc.m_blk & 1)) * kEpiWarps + ew) * NCH) * 512 + lane * 16;
-    const bf16* exb = nullptr;
-    long long ex_step = 16;
-    if constexpr (!OUT_F32) {
-        constexpr bool kWantAdd = EPI == EPI_RESID || EPI == EPI_DROP_RESID || EPI == EPI_DELTA;   // EPI_DELTA: addend = O
-        if (row < p.M) {
-            if (kWantAdd || (EPI == EPI_GENERIC && p.addend != nullptr)) exb = p.addend + static_cast<long long>(row) * p.ld_add + col0;
-            else if (EPI == EPI_DGELU_BWD || (EPI == EPI_GENERIC && p.epilogue == VB_EPI_DGELU))
-                exb = p.aux_in + static_cast<long long>(row) * p.ld_aux + col0;
-            else if (EPI == EPI_DGELU_BWD_T) { exb = p.aux_in + gp_tile_off; ex_step = 512; }
-        }
-    }
+    constexpr int RPI = 32 / NCH;
+    constexpr bool kRowPerLane = EPI == EPI_DELTA;
+    auto wrow_of = [&](int j) { return kRowPerLane ? lane : RPI * j + lane % RPI; };   // row within the warp's 32
+    auto chunk_of = [&](int j) { return kRowPerLane ? j : lane / RPI; };
+    // tile-native gelu'(u) (M, N multiples of 256; vbert_b200.h): 1 KB warp blocks per chunk, row r of the warp's 32 at + 32 r bytes
+    const long long gp_warp_off =
+        ((((static_cast<long long>(tc.m_blk >> 1) * n_blocks + tc.n_blk) * 2 + (tc.m_blk & 1)) * kEpiWarps + ew) * NCH) * 512;
+    auto gp_off = [&](int j) { return gp_warp_off + chunk_of(j) * 512 + wrow_of(j) * 16; };
     constexpr bool kEx = !OUT_F32 && EPI != EPI_BIAS && !epi_is_gelu(EPI);
     uint32_t ex[kEx ? NCH : 1][8];
     if constexpr (kEx) {
+        constexpr bool kWantAdd = EPI == EPI_RESID || EPI == EPI_DROP_RESID || EPI == EPI_DELTA;   // EPI_DELTA: addend = O
+        const int row0 = tc.m_blk * BLOCK_M + q * 32 + wrow_of(0), c0 = col0 + chunk_of(0) * 16;   // step j: row0 + (row step) j
+        const bf16* exb = nullptr;
+        long long ex_step = 0;
+        if (kWantAdd || (EPI == EPI_GENERIC && p.addend != nullptr)) {
+            exb = p.addend + static_cast<long long>(row0) * p.ld_add + c0;
+            ex_step = kRowPerLane ? 16 : RPI * p.ld_add;
+        } else if (EPI == EPI_DGELU_BWD || (EPI == EPI_GENERIC && p.epilogue == VB_EPI_DGELU)) {
+            exb = p.aux_in + static_cast<long long>(row0) * p.ld_aux + c0;
+            ex_step = kRowPerLane ? 16 : RPI * p.ld_aux;
+        } else if (EPI == EPI_DGELU_BWD_T) {
+            exb = p.aux_in + gp_off(0);
+            ex_step = kRowPerLane ? 512 : RPI * 16;
+        }
 #pragma unroll
-        for (int k = 0; k < NCH; ++k)
-            if (exb != nullptr && col0 + k * 16 < p.N) ldg_v8(exb + k * ex_step, ex[k]);
+        for (int j = 0; j < NCH; ++j)
+            if (exb != nullptr && tc.m_blk * BLOCK_M + q * 32 + wrow_of(j) < p.M && col0 + chunk_of(j) * 16 < p.N) ldg_v8(exb + j * ex_step, ex[j]);
     }
 
     // both warpgroups' MMAs have retired (and with them every read of the ring): stage the accumulators over the ring
@@ -403,25 +414,26 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
     }
     named_bar_sync(1, kEpiWarps * 32);
 
-    const float* srow = sacc + lrow * C::ACC_LD + half * (BLOCK_N / 2);
     [[maybe_unused]] float hsum = 0.f;
 #pragma unroll
     for (int k = 0; k < NCH; ++k) {
-        const int col = col0 + k * 16;
+        const int lrow = q * 32 + wrow_of(k), cc = half * (BLOCK_N / 2) + chunk_of(k) * 16;   // in the tile
+        const int row = tc.m_blk * BLOCK_M + lrow;
+        const int col = tc.n_blk * BLOCK_N + cc;
         if (row < p.M && col < p.N) {
             float x[16];
 #pragma unroll
             for (int i = 0; i < 4; ++i) {
-                const float4 v = *reinterpret_cast<const float4*>(srow + k * 16 + 4 * i);
+                const float4 v = *reinterpret_cast<const float4*>(sacc + lrow * C::ACC_LD + cc + 4 * i);
                 x[4 * i] = v.x; x[4 * i + 1] = v.y; x[4 * i + 2] = v.z; x[4 * i + 3] = v.w;
             }
-            const float* sb = has_bias ? sbias + half * (BLOCK_N / 2) + k * 16 : nullptr;
+            const float* sb = has_bias ? sbias + cc : nullptr;
             const uint32_t (&e)[8] = ex[kEx ? k : 0];
             if constexpr (EPI == EPI_GELU_FWD_T) {
-                // gelu'(u): one coalesced 1 KB warp store into the tile-native buffer; gelu(u): row-major
+                // gelu'(u) into the tile-native buffer, gelu(u) row-major
                 uint32_t o0[8], o1[8];
                 epilogue16<OUT_F32, EPI, true>(p, row, col, sb, e, x, o0, o1);
-                stg_v8(reinterpret_cast<bf16*>(p.D) + gp_tile_off + k * 512, o0);
+                stg_v8(reinterpret_cast<bf16*>(p.D) + gp_off(k), o0);
                 stg_v8(p.aux_out + static_cast<long long>(row) * p.ld_aux + col, o1);
             } else if constexpr (EPI == EPI_DELTA) {
                 uint32_t o0[8];
@@ -556,6 +568,22 @@ static int launch(const CUtensorMap& ta, const CUtensorMap& tb, const GemmParams
     return 0;
 }
 
+// Split-K factor of an fp32 (accumulating) output, from the shape: the k-range is cut into `splits` equal parts so that the
+// tiles * splits CTAs fill whole waves of one CTA per SM. It minimises the time of the busiest SM in k-blocks, waves * (k-blocks
+// per split + kCtaCost), where kCtaCost stands for what every CTA pays besides its main loop (launch, first TMA round trip,
+// red.add of its partial tile); the smallest such factor wins.
+static int wgrad_splits(long long tiles, int k_blocks) {
+    constexpr int kCtaCost = 4;
+    const long long sms = num_sms();
+    int best = 1;
+    long long best_cost = -1;
+    for (int s = 1; s <= k_blocks && s <= 32; ++s) {
+        const long long cost = (tiles * s + sms - 1) / sms * ((k_blocks + s - 1) / s + kCtaCost);
+        if (best_cost < 0 || cost < best_cost) { best = s; best_cost = cost; }
+    }
+    return best;
+}
+
 bool pdl_enabled() {
     static const bool on = [] {
         const char* e = getenv("VB_PDL");
@@ -603,10 +631,6 @@ int gemm(const vb_gemm_args& a, cudaStream_t st) {
     GemmParams p;
     memset(&p, 0, sizeof(p));
     p.M = a.M; p.N = a.N; p.K = a.K;
-    const int k_blocks = (a.K + BLOCK_K - 1) / BLOCK_K;
-    int splits = (a.d_fp32 && a.splits > 1) ? a.splits : 1;
-    if (splits > k_blocks) splits = k_blocks;
-    p.splits = splits;
     p.D = a.D; p.ldd = a.ldd;
     p.bias = a.bias;
     p.addend = static_cast<const bf16*>(a.addend); p.ld_add = a.ld_add;
@@ -634,6 +658,8 @@ int gemm(const vb_gemm_args& a, cudaStream_t st) {
     const int n_pad256 = (a.N + 255) / 256 * 256;
     const bool bn256 = (a.N >= 256) && ((n_pad256 - a.N) * 8 <= a.N);
     VB_REQUIRE(!a.delta_out || bn256, "vb_gemm: delta_out needs 256-wide tiles");
+    const long long tiles = static_cast<long long>((a.M + BLOCK_M - 1) / BLOCK_M) * ((a.N + (bn256 ? 255 : 127)) / (bn256 ? 256 : 128));
+    p.splits = a.d_fp32 ? wgrad_splits(tiles, (a.K + BLOCK_K - 1) / BLOCK_K) : 1;
 
     CUtensorMap ta, tb;
     int rc;
