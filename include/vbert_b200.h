@@ -104,7 +104,8 @@ int vb_layernorm_bwd(const void* dy, const void* x, const float* mean, const flo
 
 /* ---- BertSelfAttention core (M.py:241-256) ----------------------------------------------- */
 /* qkv bf16 [batch*seq, 3*hidden] (Q | K | V), mask_bias fp32 [batch, seq] additive key bias,
- * ctx bf16 [batch*seq, hidden], lse fp32 [batch, heads, seq]. head_dim must be 64.
+ * ctx bf16 [batch*seq, hidden], lse fp32 [batch, heads, seq]. head_dim must be 64. qkv, and in the backward ctx and dctx,
+ * must be 16-byte aligned (the kernels load them in 16-byte pieces); a call with one that is not returns an error.
  * keep_mask: vb_attention_keep_bytes(batch, seq, heads) bytes, written by forward and read by backward when
  * dropout_p > 0 (packed keep bits of the attention-probability dropout, M.py:251); may be NULL otherwise. */
 int64_t vb_attention_keep_bytes(int32_t batch, int32_t seq, int32_t heads);
@@ -119,8 +120,8 @@ int vb_attention_bwd(const void* qkv, const float* mask_bias, const void* ctx, c
  * owns rows [cu_seqlens[b], cu_seqlens[b+1]); cu_seqlens is int32 [batch + 1] in DEVICE memory; max_seq >= every length.
  * ctx bf16 [total, hidden], dqkv bf16 [total, 3*hidden], lse and drow fp32 [heads, total]; keep_mask as for the dense call
  * with seq = max_seq (vb_attention_keep_bytes(batch, max_seq, heads)). There is no mask: every row of a sequence is a valid
- * key. Only rows inside [cu[b], cu[b] + len_b) are written. The route (wgmma / whole-head / staged) and its environment
- * switches are chosen from max_seq as the dense call chooses them from seq.
+ * key. Only rows inside [cu[b], cu[b] + len_b) are written. The route (wgmma / whole-head / staged) is chosen from
+ * max_seq as the dense call chooses it from seq. The alignment rule of the dense call applies.
  * Caller contract (not checked, that would need a host synchronisation): cu_seqlens is non-decreasing from 0 to at most total
  * and no length exceeds max_seq. The kernels clamp every length to [0, max_seq] and every row range to [0, total), so a bad
  * table gives wrong values but no access outside the tensors. */

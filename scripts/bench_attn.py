@@ -1,6 +1,7 @@
 """Attention kernels alone at the benchmark shape (cfg2: B=256, S=164, A=12) through the C ABI: parity against a torch fp32
 restatement on a small slice, then CUDA-event timing of forward and backward (dropout on, like the training step).
-Usage: python scripts/bench_attn.py [B] [S] [A] [iters]   (VB_ATTN_STAGED=1 selects the staged kernels)"""
+Usage: python scripts/bench_attn.py [B] [S] [A] [iters]   (S picks the kernels: wgmma up to 192, whole-head up to 256, staged
+beyond)"""
 import ctypes, os, sys
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)

@@ -1,25 +1,17 @@
 """Every attention kernel against a plain fp64 restatement of the same op, through the C ABI (ctypes).
 
-The library has four attention paths; which one runs depends on the sequence length and on environment switches that
-are read once per process:
+The library has three attention paths; the sequence length alone picks one:
 
-    wgmma            S <= 192 (default)                 attn_fwd_wgmma_kernel / attn_bwd_wgmma_kernel
-    head, P/dS smem  S <= 176 with VB_ATTN_HEAD=1       attn_fwd_head_kernel  / attn_bwd_head_ps_kernel
-    head, recompute  193 <= S <= 256 (default), or      attn_fwd_head_kernel  / attn_bwd_head_kernel
-                     VB_ATTN_HEAD=1 with S > 176 or VB_ATTN_BWD_PS=0
-    staged           S > 256 (default), VB_ATTN_STAGED=1  attn_fwd_kernel / attn_bwd_dq_kernel + attn_bwd_dkv_kernel
+    wgmma    S <= 192          attn_fwd_wgmma_kernel / attn_bwd_wgmma_kernel
+    head     193 <= S <= 256   attn_fwd_head_kernel  / attn_bwd_head_kernel
+    staged   S > 256           attn_fwd_kernel / attn_bwd_dq_kernel + attn_bwd_dkv_kernel
 
-The parametrized tests below run the shapes of the route selected by the current environment; test_attention_switches
-reruns this file in a subprocess for each switch set. Each case checks ctx, lse, dQ, dK and dV separately against the
-reference, that every output element is written (outputs are pre-filled with NaN), that nothing is read or written
+Each case checks ctx, lse, dQ, dK and dV separately against the reference, that every output element is written (outputs are pre-filled with NaN), that nothing is read or written
 outside the tensors (they are views inside buffers whose guard bands hold NaN for inputs and a sentinel for outputs),
 and that two identical calls are bit-identical. With dropout, the reference applies the bits the forward stored in the
 keep buffer, so a match also shows that the forward applied exactly the stored bits."""
 import ctypes
-import os
 import re
-import subprocess
-import sys
 
 import pytest
 import torch
@@ -36,69 +28,32 @@ SENTINEL = -12345.0
 KEEP_SENTINEL = 0xA5
 P_FIRST = 0.1      # dropout of the reference comparisons (quantised to 26/256)
 
-ROUTES = {
-    "default": {},
-    "head": {"VB_ATTN_HEAD": "1"},
-    "head_recompute": {"VB_ATTN_HEAD": "1", "VB_ATTN_BWD_PS": "0"},
-    "staged": {"VB_ATTN_STAGED": "1"},
-}
 KERNELS = {
     "wgmma": {"attn_fwd_wgmma_kernel", "attn_delta_kernel", "attn_bwd_wgmma_kernel"},
-    "head_ps": {"attn_fwd_head_kernel", "attn_delta_kernel", "attn_bwd_head_ps_kernel"},
-    "head_recompute": {"attn_fwd_head_kernel", "attn_delta_kernel", "attn_bwd_head_kernel"},
+    "head": {"attn_fwd_head_kernel", "attn_delta_kernel", "attn_bwd_head_kernel"},
     "staged": {"attn_fwd_kernel", "attn_bwd_dq_kernel", "attn_bwd_dkv_kernel"},
 }
 
 
-def _route():
-    """The switch set of this process, as the library reads it (vb_attention.cu, vb_attention_head.cu)."""
-    def on(k):
-        try:
-            return int(os.environ.get(k, "0")) != 0
-        except ValueError:
-            return False
-    if on("VB_ATTN_STAGED"):
-        return "staged"
-    if on("VB_ATTN_HEAD"):
-        return "head_recompute" if os.environ.get("VB_ATTN_BWD_PS", "").startswith("0") else "head"
-    return "default"
+def _path(S):
+    """The implementation the library picks for sequence length S."""
+    return "wgmma" if S <= 192 else "head" if S <= 256 else "staged"
 
 
-def _path(route, S):
-    """The implementation the library picks for sequence length S (16-byte aligned operands)."""
-    if route == "staged" or S > 256:
-        return "staged"
-    if route == "default" and S <= 192:
-        return "wgmma"
-    if route == "head" and S <= 176:  # P and dS of a whole head fit in shared memory up to S = 176
-        return "head_ps"
-    return "head_recompute"
-
-
-# sequence lengths per route: tile edges (1, 63/64/65, 127/128/129, 191/192), the cut-overs 176/177, 192/193 and
-# 256/257, and 513 (staged: stages of 4, 4 and 1 key blocks)
-SEQS = {
-    "default": [1, 2, 17, 63, 64, 65, 100, 127, 128, 129, 164, 191, 192, 193, 200, 255, 256, 257, 320, 356, 513],
-    "head": [1, 17, 64, 65, 128, 129, 176, 177],
-    "head_recompute": [17, 65, 177, 192],
-    "staged": [1, 65, 192],
-}
+# sequence lengths: tile edges (1, 63/64/65, 127/128/129, 191/192), the cut-overs 192/193 and 256/257, and the staged
+# kernels' stages of up to 4 key blocks: a partial and a full last block (319, 320), two stages (384), a last block of one
+# row (449) and three stages (513)
+SEQS = [1, 2, 17, 63, 64, 65, 100, 127, 128, 129, 164, 191, 192, 193, 200, 255, 256, 257, 319, 320, 356, 384, 449, 513]
 # dropout comparisons: a partial and a full last tile per path
-DROP_SEQS = {
-    "default": [65, 128, 192, 200, 256, 257, 320, 356, 513],
-    "head": [65, 128, 176, 177, 192],
-    "head_recompute": [65, 192],
-    "staged": [65, 192],
-}
+DROP_SEQS = [65, 128, 192, 200, 256, 257, 320, 356, 384, 513]
 # persistent whole-head kernels: B*A = 288 heads, more than twice the SM count, so every CTA walks several heads
-WALK = {"default": [200], "head": [164], "head_recompute": [164], "staged": []}
+WALK = [200]
 # one shape per path for the routing test
-ROUTING_SEQS = {"default": [100, 200, 356], "head": [128, 177], "head_recompute": [65], "staged": [65]}
+ROUTING_SEQS = [100, 200, 356]
 
-ROUTE = _route()
-CASES = ([(B, S, A, 0.0) for S in SEQS[ROUTE] for B in (1, 3) for A in (1, 2, 12)]
-         + [(3, S, 12, P_FIRST) for S in DROP_SEQS[ROUTE]]
-         + [(24, S, 12, p) for S in WALK[ROUTE] for p in (0.0, P_FIRST)])
+CASES = ([(B, S, A, 0.0) for S in SEQS for B in (1, 3) for A in (1, 2, 12)]
+         + [(3, S, 12, P_FIRST) for S in DROP_SEQS]
+         + [(24, S, 12, p) for S in WALK for p in (0.0, P_FIRST)])
 
 
 def _setup():
@@ -221,7 +176,7 @@ def _check_case(B, S, A, p, seed, fully_masked):
     """One forward + backward against the reference, with all checks described in the module docstring."""
     _lib, L, dev, st = _setup()
     H = A * 64
-    where = f"{ROUTE}/{_path(ROUTE, S)} B={B} S={S} A={A} p={p}"
+    where = f"{_path(S)} B={B} S={S} A={A} p={p}"
     qkv, bias, dctx = _inputs(B, S, A, dev, seed, fully_masked)
     T = _run(L, _lib, st, qkv, bias, dctx, B, S, A, p, dev)
     T2 = _run(L, _lib, st, qkv, bias, dctx, B, S, A, p, dev, guarded=False)
@@ -249,7 +204,7 @@ def _check_case(B, S, A, p, seed, fully_masked):
         n = int(p * 256 + 0.5)
         q = n / 256
         bits = _keep_bits(keep, B, S, A)
-        if _path(ROUTE, S) != "staged":  # the mask kernel also writes the transpose (rows = keys); the staged path does not
+        if _path(S) != "staged":  # the mask kernel also writes the transpose (rows = keys); the staged path does not
             assert torch.equal(bits, _keep_bits(keep, B, S, A, half=1).transpose(1, 2)), f"{where}: transposed keep bits differ"
         assert abs(bits.float().mean().item() - (1 - q)) < 5e-3, f"{where}: keep rate {bits.float().mean().item():.4f}"
         for kb in range((S + 63) // 64):  # per 64-key block: 6 standard deviations of a binomial rate
@@ -284,7 +239,7 @@ def test_attention_dropout_consistent_between_fwd_and_bwd():
     preserved."""
     _check_case(2, 100, 2, 0.2, seed=7, fully_masked=False)
 
-@pytest.mark.parametrize("S", SEQS[ROUTE])
+@pytest.mark.parametrize("S", SEQS)
 def test_attention_dropout_words_are_distinct(S):
     """At p = 0.5 a keep decision is the top bit of an 8-bit hash value, so each stored 64-bit word of a valid row
     (query < S, every key block, all 64 bits) is 64 independent random bits: two of them are equal with probability
@@ -303,14 +258,14 @@ def test_attention_dropout_words_are_distinct(S):
     nkb = (S + 63) // 64
     words = keep.view(torch.int64).view(2, B * A, nkb * 64, nkb)[0, :, :S, :].reshape(-1)
     dup = words.numel() - torch.unique(words).numel()
-    assert dup == 0, f"{ROUTE}/{_path(ROUTE, S)} S={S}: {dup} repeated keep words of {words.numel()}"
+    assert dup == 0, f"{_path(S)} S={S}: {dup} repeated keep words of {words.numel()}"
     bits = _keep_bits(keep, B, S, A).float()
     for kb in range(nkb):
         blk = bits[:, :, kb * 64:(kb + 1) * 64]
         assert abs(blk.mean().item() - 0.5) < 6 * (0.25 / blk.numel()) ** 0.5, f"S={S}: keep rate {blk.mean().item():.4f} in block {kb}"
 
 
-@pytest.mark.parametrize("S", ROUTING_SEQS[ROUTE])
+@pytest.mark.parametrize("S", ROUTING_SEQS)
 def test_attention_routing(S):
     """The kernels one forward + backward launches are those of the expected path: a change to the dispatch must not send
     every case silently to one implementation."""
@@ -327,21 +282,7 @@ def test_attention_routing(S):
     if not names:
         pytest.skip("torch.profiler recorded no device kernels")
     ran = {m.group(1) for n in names for m in [re.search(r"\b(attn_\w+_kernel)\b", n)] if m}
-    path = _path(ROUTE, S)
+    path = _path(S)
     want = KERNELS[path] | ({"attn_keep_mask_kernel"} if path != "staged" else set())
-    assert ran == want, f"{ROUTE} S={S}: expected {sorted(want)}, ran {sorted(ran)}"
+    assert ran == want, f"S={S}: expected {sorted(want)}, ran {sorted(ran)}"
 
-
-@pytest.mark.parametrize("route", [r for r in ROUTES if r != "default"])
-def test_attention_switches(route):
-    """The whole-head mma.sync kernels (with their P/dS-in-shared-memory backward and with the recompute backward) and the
-    staged kernels, forced through the library's environment switches, must pass the same checks: the switches are read
-    once per process, so this file reruns in a subprocess per switch set."""
-    if ROUTE != "default":
-        pytest.skip("already running under a switch set")
-    env = {k: v for k, v in os.environ.items() if k not in ("VB_ATTN_HEAD", "VB_ATTN_BWD_PS", "VB_ATTN_STAGED")}
-    env.update(ROUTES[route])
-    r = subprocess.run([sys.executable, "-m", "pytest", os.path.abspath(__file__), "-m", "gpu", "-q", "-p", "no:cacheprovider",
-                        "-k", "not test_attention_switches"], env=env, capture_output=True, text=True, timeout=900)
-    assert r.returncode == 0, r.stdout[-3000:] + r.stderr[-2000:]
-    assert " passed" in r.stdout and " skipped" not in r.stdout.splitlines()[-1], r.stdout[-2000:]

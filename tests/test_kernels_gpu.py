@@ -149,19 +149,6 @@ def test_gemm_dropout_statistics_and_determinism():
     assert abs(D1.float().mean().item() - D0.float().mean().item()) < 0.02 * D0.float().abs().mean().item()
 
 
-@pytest.mark.parametrize("env", [{"VB_GEMM_GP_TILED": "0"}, {"VB_GEMM_TILE_ORDER": "0"}, {"VB_PDL": "0"}])
-def test_gemm_kernel_variants(env):
-    """The GEMM picks per launch the layout of gelu'(u) (row-major or tile-native) and the order of its tiles, and its
-    kernels are launched with or without programmatic dependent launch. Each choice must pass the same checks: they are
-    forced through the library's environment switches, read once per process, so the GEMM tests rerun in a subprocess."""
-    import os, subprocess, sys
-    root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-    r = subprocess.run([sys.executable, "-m", "pytest", os.path.join(root, "tests", "test_kernels_gpu.py"), "-m", "gpu", "-q",
-                        "-k", "test_gemm_tn or test_gemm_gelu or test_gemm_dgrad or test_gemm_dropout"],
-                       env=dict(os.environ, **env), capture_output=True, text=True, timeout=600)
-    assert r.returncode == 0, r.stdout[-2000:] + r.stderr[-2000:]
-
-
 @pytest.mark.parametrize("rows,H", [(1000, 768), (333, 1024), (77, 128), (64, 256)])
 def test_layernorm_fwd_bwd(rows, H):
     _lib, L, dev, st = _setup()

@@ -30,11 +30,16 @@ def test_varlen_arena_layout_is_aligned_and_sized():
     assert b"bad shape" in L.vb_last_error()
 
 
+def _aligned_buffer(n):
+    """A host buffer and a 16-byte aligned address inside it (stands in for device pointers the calls refuse before use)."""
+    buf = ctypes.create_string_buffer(n + 16)
+    return buf, (ctypes.addressof(buf) + 15) // 16 * 16
+
+
 def test_varlen_argument_validation_reports_through_vb_last_error():
     from visualbert_b200 import _lib
     L = _lib.lib()
-    buf = ctypes.create_string_buffer(64)
-    p = ctypes.addressof(buf)
+    buf, p = _aligned_buffer(64)
     # batch 0, max_seq 0, negative total, null cu_seqlens, head_dim != 64: refused before anything is launched
     assert L.vb_attention_fwd_varlen(p, p, p, p, None, 0, 10, 10, 1, 64, 0.0, 1, 0, None) != 0
     assert b"empty problem" in L.vb_last_error()
@@ -57,6 +62,29 @@ def test_varlen_argument_validation_reports_through_vb_last_error():
     assert b"total" in L.vb_last_error()
     assert L.vb_encoder_bwd_varlen(None, 1, p, 5, None, None, None, None, None, None, None) != 0
     assert b"null pointer" in L.vb_last_error()
+
+
+def test_attention_refuses_operands_that_are_not_16_byte_aligned():
+    """Every attention route reads qkv, and in the backward ctx and dctx, in 16-byte pieces: a pointer 2 bytes off that
+    alignment is refused before anything is launched."""
+    from visualbert_b200 import _lib
+    L = _lib.lib()
+    buf, a = _aligned_buffer(64)
+    p, off = ctypes.c_void_p(a), ctypes.c_void_p(a + 2)
+    B, S, A, H = 2, 100, 1, 64
+    tail = (B, S, A, H, ctypes.c_float(0.0), ctypes.c_uint64(1), 0, None)
+    assert L.vb_attention_fwd(off, p, p, p, None, *tail) != 0
+    assert b"16-byte aligned" in L.vb_last_error()
+    assert L.vb_attention_bwd(off, p, p, p, None, p, p, p, *tail) != 0   # qkv
+    assert b"16-byte aligned" in L.vb_last_error()
+    assert L.vb_attention_bwd(p, p, off, p, None, p, p, p, *tail) != 0   # ctx
+    assert b"16-byte aligned" in L.vb_last_error()
+    assert L.vb_attention_bwd(p, p, p, p, None, off, p, p, *tail) != 0   # dctx
+    assert b"16-byte aligned" in L.vb_last_error()
+    assert L.vb_attention_fwd_varlen(a + 2, a, a, a, None, 2, 10, 10, 1, 64, 0.0, 1, 0, None) != 0
+    assert b"16-byte aligned" in L.vb_last_error()
+    assert L.vb_attention_bwd_varlen(a, a, a, a, None, a + 2, a, a, 2, 10, 10, 1, 64, 0.0, 1, 0, None) != 0
+    assert b"16-byte aligned" in L.vb_last_error()
 
 
 def _loop_plan(valid):

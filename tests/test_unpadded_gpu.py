@@ -2,14 +2,10 @@
 restatement and against the dense kernels on the same data, and BertVisualModel.set_unpadded against the goldens, the oracle
 and the padded path.
 
-The attention route is chosen from max_seq with the same environment switches as the dense call; they are read once per
-process, so test_varlen_switches reruns this file in a subprocess per switch set (as test_attention_reference_gpu.py does)."""
+The attention route is chosen from max_seq as the dense call chooses it from seq."""
 import ctypes
 import math
-import os
 import re
-import subprocess
-import sys
 
 import numpy as np
 import pytest
@@ -24,35 +20,12 @@ CTX_TOL, GRAD_TOL, LSE_TOL = 1.0e-2, 2.0e-2, 2.0e-2   # as in test_attention_ref
 GUARD_ROWS, GUARD_FLAT, SENTINEL = 64, 256, -12345.0
 P_DROP = 0.1
 
-ROUTES = {"default": {}, "head": {"VB_ATTN_HEAD": "1"}, "head_recompute": {"VB_ATTN_HEAD": "1", "VB_ATTN_BWD_PS": "0"},
-          "staged": {"VB_ATTN_STAGED": "1"}}
-
-
-def _route():
-    def on(k):
-        try:
-            return int(os.environ.get(k, "0")) != 0
-        except ValueError:
-            return False
-    if on("VB_ATTN_STAGED"):
-        return "staged"
-    if on("VB_ATTN_HEAD"):
-        return "head_recompute" if os.environ.get("VB_ATTN_BWD_PS", "").startswith("0") else "head"
-    return "default"
-
-
-ROUTE = _route()
 # length mixes: the maximum selects the route (wgmma <= 192, whole-head <= 256, staged above); 0 and 1 are the empty and the
 # one-row sequence, the others sit on tile edges and route cut-overs
-MIXES = {
-    "default": [[0, 1, 63, 64, 65], [127, 128, 129, 1], [176, 177, 0, 191, 192], [193, 64, 0], [255, 256, 1, 100],
-                [257, 100, 0], [356, 0, 17, 200], [513, 64, 129]],
-    "head": [[0, 1, 64, 65], [176, 177, 3, 128], [129, 0, 17]],
-    "head_recompute": [[17, 65, 177, 192, 0], [100, 1]],
-    "staged": [[1, 65, 192, 0], [64, 63, 5]],
-}
-CASES = ([(tuple(m), A, 0.0) for m in MIXES[ROUTE] for A in (1, 12)]
-         + [(tuple(m), 12, P_DROP) for m in MIXES[ROUTE][:2]])
+MIXES = [[0, 1, 63, 64, 65], [127, 128, 129, 1], [176, 177, 0, 191, 192], [193, 64, 0], [255, 256, 1, 100],
+         [257, 100, 0], [356, 0, 17, 200], [513, 64, 129]]
+CASES = ([(tuple(m), A, 0.0) for m in MIXES for A in (1, 12)]
+         + [(tuple(m), 12, P_DROP) for m in MIXES[:2]])
 
 
 def _setup():
@@ -154,7 +127,7 @@ def _inputs(lens, A, seed):
 
 def _check(lens, A, p, seed):
     H = A * 64
-    where = f"{ROUTE} lens={list(lens)} A={A} p={p}"
+    where = f"lens={list(lens)} A={A} p={p}"
     qkv, dctx = _inputs(lens, A, seed)
     T = _run_varlen(lens, A, p, qkv, dctx)
     T2 = _run_varlen(lens, A, p, qkv, dctx, guarded=False)
@@ -184,7 +157,6 @@ def test_varlen_attention_matches_reference(lens, A, p):
     _check(lens, A, p, seed=sum(lens) * 7 + A)
 
 
-@pytest.mark.skipif(ROUTE in ("staged",), reason="persistent whole-head / wgmma shapes")
 def test_varlen_attention_many_heads():
     """B * A = 7 * 40 = 280 heads, more than twice the SM count: persistent whole-head CTAs walk several sequences."""
     g = torch.Generator().manual_seed(3)
@@ -193,7 +165,6 @@ def test_varlen_attention_many_heads():
     _check(tuple(lens), 7, 0.0, seed=11)
 
 
-@pytest.mark.skipif(ROUTE != "default", reason="dense comparison once")
 @pytest.mark.parametrize("lens", [(100, 37, 1, 64), (200, 150, 3), (356, 300, 17)])
 def test_varlen_matches_dense_on_same_data(lens):
     """The dense kernels with a -10000 key mask on padded rows and the varlen kernels on the packed rows agree on every valid
@@ -228,7 +199,6 @@ def test_varlen_matches_dense_on_same_data(lens):
     assert e_ctx < CTX_TOL and e_d < GRAD_TOL and e_lse < LSE_TOL
 
 
-@pytest.mark.skipif(ROUTE != "default", reason="routing of the default switch set")
 @pytest.mark.parametrize("S,want", [(100, "wgmma"), (200, "head"), (356, "staged")])
 def test_varlen_routing(S, want):
     from torch.profiler import ProfilerActivity, profile
@@ -247,17 +217,6 @@ def test_varlen_routing(S, want):
            "head": {"attn_keep_mask_kernel", "attn_fwd_head_kernel", "attn_delta_kernel", "attn_bwd_head_kernel"},
            "staged": {"attn_fwd_kernel", "attn_bwd_dq_kernel", "attn_bwd_dkv_kernel"}}[want]
     assert ran == fam, f"S={S}: expected {sorted(fam)}, ran {sorted(ran)}"
-
-
-@pytest.mark.parametrize("route", [r for r in ROUTES if r != "default"])
-def test_varlen_switches(route):
-    if ROUTE != "default":
-        pytest.skip("already running under a switch set")
-    env = {k: v for k, v in os.environ.items() if k not in ("VB_ATTN_HEAD", "VB_ATTN_BWD_PS", "VB_ATTN_STAGED")}
-    env.update(ROUTES[route])
-    r = subprocess.run([sys.executable, "-m", "pytest", os.path.abspath(__file__), "-m", "gpu", "-q", "-p", "no:cacheprovider",
-                        "-k", "test_varlen_attention"], env=env, capture_output=True, text=True, timeout=900)
-    assert r.returncode == 0, r.stdout[-3000:] + r.stderr[-2000:]
 
 
 # ------------------------------------------------------------------------------------------------------------------------

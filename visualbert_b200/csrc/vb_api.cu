@@ -78,27 +78,13 @@ int layer_fwd(const vb_layer_desc* d, const void* x_in, void* x_out, const vb_la
     const int M = vl ? rows.total : d->batch * d->seq, H = d->hidden, I = d->inter;
     vb_gemm_args a = fwd_args(x_in, d->w_qkv, s->qkv, M, 3 * H, H);
     a.bias = d->b_qkv;
-    // the attention-dropout bits depend on (seed, layer) only: they are drawn on a side stream UNDER the QKV GEMM (attn_mask_async)
-    static cudaEvent_t before_qkv[kMaxDevices] = {nullptr};
-    const int dev = current_device();
-    const bool want_mask = d->attn_dropout > 0.f && s->keep_mask != nullptr;
-    if (want_mask) {
-        if (before_qkv[dev] == nullptr) VB_CHECK_CUDA(cudaEventCreateWithFlags(&before_qkv[dev], cudaEventDisableTiming));
-        VB_CHECK_CUDA(cudaEventRecord(before_qkv[dev], st));
-    }
     VB_TRY(gemm(a, st));
-    int mask_ready = 0;
-    if (want_mask) {
-        mask_ready = attn_mask_async(s->keep_mask, d->batch, d->seq, d->heads, H, d->attn_dropout, d->seed,
-                                     drop_stream(d->layer_index, kSiteAttnProbs), before_qkv[dev], st);
-        if (mask_ready < 0) return 2;
-    }
     if (vl)
         VB_TRY(attn_fwd_varlen(s->qkv, rows.cu_seqlens, s->ctx, s->lse, s->keep_mask, d->batch, d->seq, rows.total, d->heads, H,
-                               d->attn_dropout, d->seed, drop_stream(d->layer_index, kSiteAttnProbs), st, mask_ready == 1));
+                               d->attn_dropout, d->seed, drop_stream(d->layer_index, kSiteAttnProbs), st));
     else
         VB_TRY(attn_fwd(s->qkv, d->mask_bias, s->ctx, s->lse, s->keep_mask, d->batch, d->seq, d->heads, H, d->attn_dropout, d->seed,
-                        drop_stream(d->layer_index, kSiteAttnProbs), st, mask_ready == 1));
+                        drop_stream(d->layer_index, kSiteAttnProbs), st));
     a = fwd_args(s->ctx, d->w_attn_out, s->pre1, M, H, H);
     a.bias = d->b_attn_out; a.addend = x_in; a.ld_add = H;
     a.dropout_p = d->hidden_dropout; a.dropout_seed = d->seed; a.dropout_stream = drop_stream(d->layer_index, kSiteAttnOut);
@@ -147,9 +133,9 @@ int layer_bwd(const vb_layer_desc* d, const void* x_in, const vb_layer_acts* s, 
                   drop_stream(d->layer_index, kSiteAttnOut), 0.f, 0, st));
     VB_TRY(gemm(wgrad_args(dpm, s->ctx, g->dw_attn_out, M, H, H), st));
     a = dgrad_args(dpm, d->w_attn_out, w->d_ctx, M, H, H);
-    // D = rowsum(dO * O) of the attention backward falls out of this GEMM's epilogue (a thread holds two whole heads of a row)
-    const bool fused_delta = gemm_delta_ok(M, H) && w->drow != nullptr &&
-                             attn_bwd_takes_delta(s->qkv, w->d_ctx, w->d_big, d->batch, d->seq, d->heads, H);
+    // D = rowsum(dO * O) of the attention backward falls out of this GEMM's epilogue (a thread holds two whole heads of a row);
+    // the staged attention kernels compute D themselves
+    const bool fused_delta = gemm_delta_ok(M, H) && w->drow != nullptr && attn_route(d->seq) != AttnRoute::Staged;
     // (varlen: drow is [heads, total], i.e. delta_out[0][h][row] with delta_seq = total)
     if (fused_delta) { a.delta_ctx = s->ctx; a.delta_out = w->drow; a.delta_seq = vl ? rows.total : d->seq; }
     VB_TRY(gemm(a, st));

@@ -16,6 +16,7 @@
 // Tensor-core path here is warp-level mma.sync (m16n8k16, bf16 -> fp32); the wgmma kernel of the
 // layer is in vb_gemm.cu, where > 96 % of the FLOPs are.
 #include "vb_attention.cuh"
+#include "vb_internal.h"
 
 namespace vb {
 
@@ -436,23 +437,7 @@ attn_bwd_dkv_kernel(const AttnParams p, const int nsub) {
 // ------------------------------------------------------------------------------------------------
 // host
 // ------------------------------------------------------------------------------------------------
-// VB_ATTN_STAGED=1 forces the generic staged kernels (testing / tuning)
-static bool staged_only() {
-    static int v = -1;
-    if (v < 0) { const char* e = getenv("VB_ATTN_STAGED"); v = (e != nullptr && atoi(e) != 0) ? 1 : 0; }
-    return v == 1;
-}
-
-// VB_ATTN_HEAD=1 forces the whole-head mma.sync kernels where the wgmma kernels would run (testing / tuning)
-static bool head_only() {
-    static int v = -1;
-    if (v < 0) { const char* e = getenv("VB_ATTN_HEAD"); v = (e != nullptr && atoi(e) != 0) ? 1 : 0; }
-    return v == 1;
-}
-// The wgmma kernels serve seq <= 192 (every reference config), the whole-head mma.sync kernels seq <= 256, the staged kernels
-// any length. Both fused paths take pre-drawn dropout bits and a pre-computed D = rowsum(dO * O).
-static bool head_path(int S) { return !staged_only() && (S + kBlk - 1) / kBlk <= kMaxSub; }
-static bool wgmma_path(const AttnParams& p) { return head_path(p.S) && !head_only() && attn_wgmma_supported(p); }
+static bool aligned16(const void* ptr) { return (reinterpret_cast<uintptr_t>(ptr) & 15) == 0; }
 
 static int fill_params(AttnParams& p, const void* qkv, const float* mask_bias, void* ctx, float* lse,
                        const void* dctx, void* dqkv, float* drow, void* keep, int B, int S, int A, int H,
@@ -462,6 +447,9 @@ static int fill_params(AttnParams& p, const void* qkv, const float* mask_bias, v
     VB_REQUIRE(A <= 65535 && B <= 65535, "attention: grid too large");
     VB_REQUIRE(dropout_p >= 0.f && dropout_p < 1.f, "attention: dropout_p out of range");
     VB_REQUIRE(dropout_p == 0.f || keep != nullptr, "attention: dropout needs the keep-mask buffer (vb_attention_keep_bytes)");
+    // every route reads qkv, and in the backward ctx and dctx, in 16-byte pieces (TMA, cp.async, vector loads)
+    VB_REQUIRE(aligned16(qkv) && (dctx == nullptr || (aligned16(ctx) && aligned16(dctx))),
+               "attention: qkv, ctx (backward) and dctx must be 16-byte aligned");
     p.keep = static_cast<unsigned long long*>(keep);
     p.qkv = static_cast<const bf16*>(qkv);
     p.mask_bias = mask_bias;
@@ -491,39 +479,6 @@ long long attn_keep_bytes(int B, int S, int A) {
     return 2 * static_cast<long long>(B) * A * (nkb * kBlk) * nkb * 8;  // query-major words + their transpose (key-major)
 }
 
-// Draws the attention-dropout keep bits of a layer on the library's SIDE stream, so that the ALU-only mask kernel (no memory
-// traffic, 32 registers, no shared memory) shares the SMs with the QKV projection GEMM instead of running alone:
-// call it right after enqueuing that GEMM with an event recorded on `main` BEFORE the GEMM (the bits depend on (seed, stream)
-// only). Returns 1 when the bits are on their way (`main` already waits for them: pass mask_ready = true to attn_fwd), 0 when
-// the caller's attn_fwd will draw them itself (no dropout, another attention implementation, not opted in), < 0 on error.
-// OPT-IN (VB_MASK_OVERLAP=1): the GEMM shares its SMs with the mask kernel, so whether it pays off depends on the GPU; the
-// default is the plain sequence.
-int attn_mask_async(void* keep, int B, int S, int A, int H, float dropout_p, unsigned long long seed, unsigned stream_id,
-                    cudaEvent_t before_gemm, cudaStream_t main) {
-    static const int off = [] { const char* e = getenv("VB_MASK_OVERLAP"); return (e != nullptr && atoi(e) == 1) ? 0 : 1; }();
-    if (off || dropout_p <= 0.f || keep == nullptr) return 0;
-    if (!head_path(S)) return 0;
-    AttnParams p;
-    if (fill_params(p, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, keep, B, S, A, H, dropout_p, seed, stream_id)) return -1;
-    static cudaStream_t side[kMaxDevices] = {nullptr};
-    static cudaEvent_t done[kMaxDevices] = {nullptr};
-    const int dev = current_device();
-    if (side[dev] == nullptr) {
-        if (cudaStreamCreateWithFlags(&side[dev], cudaStreamNonBlocking) != cudaSuccess ||
-            cudaEventCreateWithFlags(&done[dev], cudaEventDisableTiming) != cudaSuccess) {
-            set_error("attention mask: cannot create the side stream");
-            return -1;
-        }
-    }
-    if (cudaStreamWaitEvent(side[dev], before_gemm, 0) != cudaSuccess) { set_error("attention mask: stream wait failed"); return -1; }
-    if (attn_keep_mask(p, (S + kBlk - 1) / kBlk, side[dev])) return -1;
-    if (cudaEventRecord(done[dev], side[dev]) != cudaSuccess || cudaStreamWaitEvent(main, done[dev], 0) != cudaSuccess) {
-        set_error("attention mask: event record / wait failed");
-        return -1;
-    }
-    return 1;
-}
-
 // variable-length calls: the sequence table and the packed row count (what can be checked without reading device memory)
 static int set_varlen(AttnParams& p, const int* cu_seqlens, int total, const void* qkv, const void* out) {
     VB_REQUIRE(cu_seqlens != nullptr, "attention varlen: cu_seqlens is NULL");
@@ -535,11 +490,12 @@ static int set_varlen(AttnParams& p, const int* cu_seqlens, int total, const voi
     return 0;
 }
 
-static int attn_fwd_launch(const AttnParams& p, cudaStream_t st, bool mask_ready) {
+static int attn_fwd_launch(const AttnParams& p, cudaStream_t st) {
     const int B = p.B, S = p.S, A = p.A;
     dim3 grid((S + kBlk - 1) / kBlk, A, B);
-    if (wgmma_path(p)) return attn_fwd_wgmma(p, st, mask_ready);
-    if (head_path(S)) return attn_fwd_head(p, static_cast<int>(grid.x), st, mask_ready);
+    const AttnRoute route = attn_route(S);
+    if (route == AttnRoute::Wgmma) return attn_fwd_wgmma(p, st);
+    if (route == AttnRoute::Head) return attn_fwd_head(p, static_cast<int>(grid.x), st);
     const long long nkb = grid.x;
     VB_REQUIRE(p.drop_scale == 0.f || static_cast<long long>(B) * A * (nkb * kBlk) * nkb * 16 < (1LL << 32),
                "attention dropout: mask counter space exceeded (B*A*S too large)");
@@ -561,63 +517,48 @@ static int attn_fwd_launch(const AttnParams& p, cudaStream_t st, bool mask_ready
 }
 
 int attn_fwd(const void* qkv, const float* mask_bias, void* ctx, float* lse, void* keep, int B, int S, int A, int H,
-             float dropout_p, unsigned long long seed, unsigned stream_id, cudaStream_t st, bool mask_ready) {
+             float dropout_p, unsigned long long seed, unsigned stream_id, cudaStream_t st) {
     AttnParams p;
     int rc = fill_params(p, qkv, mask_bias, ctx, lse, nullptr, nullptr, nullptr, keep, B, S, A, H, dropout_p, seed, stream_id);
     if (rc) return rc;
-    return attn_fwd_launch(p, st, mask_ready);
+    return attn_fwd_launch(p, st);
 }
 
 int attn_fwd_varlen(const void* qkv, const int* cu_seqlens, void* ctx, float* lse, void* keep, int B, int max_seq, int total,
-                    int A, int H, float dropout_p, unsigned long long seed, unsigned stream_id, cudaStream_t st, bool mask_ready) {
+                    int A, int H, float dropout_p, unsigned long long seed, unsigned stream_id, cudaStream_t st) {
     AttnParams p;
     int rc = fill_params(p, qkv, nullptr, ctx, lse, nullptr, nullptr, nullptr, keep, B, max_seq, A, H, dropout_p, seed, stream_id);
     if (rc) return rc;
     VB_REQUIRE(lse != nullptr, "attention varlen: lse is NULL");
     if ((rc = set_varlen(p, cu_seqlens, total, qkv, ctx))) return rc;
     if (total == 0) return 0;  // no rows: nothing to compute or store
-    return attn_fwd_launch(p, st, mask_ready);
-}
-
-static int g_bwd_minb = 3;
-
-bool attn_bwd_takes_delta(const void* qkv, const void* dctx, void* dqkv, int B, int S, int A, int H) {
-    return B > 0 && S > 0 && A > 0 && H == A * kHd && head_path(S);
+    return attn_fwd_launch(p, st);
 }
 
 static int attn_bwd_launch(const AttnParams& p, cudaStream_t st, bool delta_ready) {
     const int B = p.B, S = p.S, A = p.A;
-    static int c0[kMaxDevices] = {0}, c1[kMaxDevices] = {0}, c2[kMaxDevices] = {0}, c3[kMaxDevices] = {0};
-    VB_CHECK_CUDA(ensure_dyn_smem(attn_bwd_dq_kernel<2>, (3 + 2 * kMaxSub) * kTileBytes, c0));
-    VB_CHECK_CUDA(ensure_dyn_smem(attn_bwd_dq_kernel<3>, (3 + 2 * kMaxSub) * kTileBytes, c1));
-    VB_CHECK_CUDA(ensure_dyn_smem(attn_bwd_dkv_kernel<2>, (2 + 2 * kMaxSub) * kTileBytes, c2));
-    VB_CHECK_CUDA(ensure_dyn_smem(attn_bwd_dkv_kernel<3>, (2 + 2 * kMaxSub) * kTileBytes, c3));
-    static bool env_read = false;
-    if (!env_read) {
-        const char* e = getenv("VB_ATTN_BWD_MINB");  // tuning knob: resident CTAs per SM the backward kernels are compiled for
-        if (e != nullptr) g_bwd_minb = atoi(e) == 2 ? 2 : 3;
-        env_read = true;
-    }
     dim3 grid((S + kBlk - 1) / kBlk, A, B);
-    if (wgmma_path(p)) return attn_bwd_wgmma(p, st, delta_ready);
-    if (head_path(S)) return attn_bwd_head(p, static_cast<int>(grid.x), st, delta_ready);
+    const AttnRoute route = attn_route(S);
+    if (route == AttnRoute::Wgmma) return attn_bwd_wgmma(p, st, delta_ready);
+    if (route == AttnRoute::Head) return attn_bwd_head(p, static_cast<int>(grid.x), st, delta_ready);
     const int nsub = static_cast<int>(grid.x) < kMaxSub ? static_cast<int>(grid.x) : kMaxSub;
     const bool vl = p.cu_seqlens != nullptr;
+    static int c0[kMaxDevices] = {0}, c1[kMaxDevices] = {0}, v0[kMaxDevices] = {0}, v1[kMaxDevices] = {0};
     if (vl) {
-        static int v0[kMaxDevices] = {0}, v1[kMaxDevices] = {0};
         VB_CHECK_CUDA(ensure_dyn_smem(attn_bwd_dq_kernel<3, true>, (3 + 2 * kMaxSub) * kTileBytes, v0));
         VB_CHECK_CUDA(ensure_dyn_smem(attn_bwd_dkv_kernel<3, true>, (2 + 2 * kMaxSub) * kTileBytes, v1));
+    } else {
+        VB_CHECK_CUDA(ensure_dyn_smem(attn_bwd_dq_kernel<3>, (3 + 2 * kMaxSub) * kTileBytes, c0));
+        VB_CHECK_CUDA(ensure_dyn_smem(attn_bwd_dkv_kernel<3>, (2 + 2 * kMaxSub) * kTileBytes, c1));
     }
     {   // algorithmic work of the backward = 2x forward (recompute not credited), split evenly over the two kernels
         ProfScope ps(st, PROF_ATTN_DQ, 4.0 * B * A * S * S * kHd, 1);
         if (vl) attn_bwd_dq_kernel<3, true><<<grid, 128, (3 + 2 * nsub) * kTileBytes, st>>>(p, nsub);
-        else if (g_bwd_minb == 2) attn_bwd_dq_kernel<2><<<grid, 128, (3 + 2 * nsub) * kTileBytes, st>>>(p, nsub);
         else attn_bwd_dq_kernel<3><<<grid, 128, (3 + 2 * nsub) * kTileBytes, st>>>(p, nsub);
     }
     {
         ProfScope ps(st, PROF_ATTN_DKV, 4.0 * B * A * S * S * kHd, 1);
         if (vl) attn_bwd_dkv_kernel<3, true><<<grid, 128, (2 + 2 * nsub) * kTileBytes, st>>>(p, nsub);
-        else if (g_bwd_minb == 2) attn_bwd_dkv_kernel<2><<<grid, 128, (2 + 2 * nsub) * kTileBytes, st>>>(p, nsub);
         else attn_bwd_dkv_kernel<3><<<grid, 128, (2 + 2 * nsub) * kTileBytes, st>>>(p, nsub);
     }
     VB_CHECK_CUDA(cudaGetLastError());
@@ -657,7 +598,7 @@ int vb_attention_fwd(const void* qkv, const float* mask_bias, void* ctx, float* 
                      int32_t seq, int32_t heads, int32_t hidden, float dropout_p, uint64_t dropout_seed,
                      uint32_t dropout_stream, void* stream) {
     return vb::attn_fwd(qkv, mask_bias, ctx, lse, keep_mask, batch, seq, heads, hidden, dropout_p, dropout_seed,
-                        dropout_stream, static_cast<cudaStream_t>(stream), false);
+                        dropout_stream, static_cast<cudaStream_t>(stream));
 }
 int vb_attention_bwd(const void* qkv, const float* mask_bias, const void* ctx, const float* lse, const void* keep_mask,
                      const void* dctx, void* dqkv, float* drow, int32_t batch, int32_t seq, int32_t heads,
@@ -669,7 +610,7 @@ int vb_attention_fwd_varlen(const void* qkv, const int32_t* cu_seqlens, void* ct
                             int32_t max_seq, int32_t total, int32_t heads, int32_t hidden, float dropout_p, uint64_t dropout_seed,
                             uint32_t dropout_stream, void* stream) {
     return vb::attn_fwd_varlen(qkv, cu_seqlens, ctx, lse, keep_mask, batch, max_seq, total, heads, hidden, dropout_p, dropout_seed,
-                               dropout_stream, static_cast<cudaStream_t>(stream), false);
+                               dropout_stream, static_cast<cudaStream_t>(stream));
 }
 int vb_attention_bwd_varlen(const void* qkv, const int32_t* cu_seqlens, const void* ctx, const float* lse, const void* keep_mask,
                             const void* dctx, void* dqkv, float* drow, int32_t batch, int32_t max_seq, int32_t total, int32_t heads,

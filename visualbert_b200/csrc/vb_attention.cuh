@@ -1,8 +1,7 @@
-// vb_attention.cuh — device helpers shared by the attention kernels (vb_attention.cu: staged kernels for any
-// sequence length; vb_attention_head.cu: persistent whole-head mma.sync kernels for seq <= 256; vb_attention_wgmma.cu:
-// wgmma / TMA kernels for seq <= 192, the default).
+// vb_attention.cuh — device helpers shared by the attention kernels. The sequence length alone picks the kernels
+// (attn_route, vb_internal.h): vb_attention_wgmma.cu: wgmma / TMA kernels for seq <= 192; vb_attention_head.cu:
+// persistent whole-head mma.sync kernels for 192 < seq <= 256; vb_attention.cu: staged kernels for seq > 256.
 #pragma once
-#include <stdlib.h>
 
 #include "../../include/vbert_b200.h"
 #include "vb_common.cuh"
@@ -302,18 +301,18 @@ __device__ __forceinline__ void store_acc(bf16* base, long long ld, int row0, in
 
 constexpr int kMaxSub = 4;  // 64-row tiles per resident stage
 
-// whole-head persistent kernels (vb_attention_head.cu); nkb = ceil(S / 64) <= kMaxSub.
-// mask_ready: the keep bits were already drawn (attn_mask_async); delta_ready: p.drow already holds D = rowsum(dO * O)
-// (written by the epilogue of the GEMM that produced dO, vb_gemm_args.delta_out).
+// The forward launchers of the two fused routes draw the dropout keep bits (attn_keep_mask) before their kernel.
+// delta_ready: p.drow already holds D = rowsum(dO * O) (written by the epilogue of the GEMM that produced dO,
+// vb_gemm_args.delta_out); otherwise the backward launchers run attn_delta first.
 // Every launcher serves dense calls and, when p.cu_seqlens != nullptr, variable-length ones (a separate instantiation of each
 // kernel, so the dense code is unchanged).
-int attn_fwd_head(const AttnParams& p, int nkb, cudaStream_t st, bool mask_ready);
+// whole-head persistent kernels (vb_attention_head.cu), 192 < seq <= 256; nkb = ceil(S / 64)
+int attn_fwd_head(const AttnParams& p, int nkb, cudaStream_t st);
 int attn_bwd_head(const AttnParams& p, int nkb, cudaStream_t st, bool delta_ready);
 int attn_keep_mask(const AttnParams& p, int nkb, cudaStream_t st);
 int attn_delta(const AttnParams& p, cudaStream_t st);
-// wgmma / TMA / mbarrier kernels (vb_attention_wgmma.cu), seq <= 192: the default where supported
-bool attn_wgmma_supported(const AttnParams& p);
-int attn_fwd_wgmma(const AttnParams& p, cudaStream_t st, bool mask_ready);
+// wgmma / TMA / mbarrier kernels (vb_attention_wgmma.cu), seq <= 192
+int attn_fwd_wgmma(const AttnParams& p, cudaStream_t st);
 int attn_bwd_wgmma(const AttnParams& p, cudaStream_t st, bool delta_ready);
 int make_tmap_bf16(CUtensorMap* m, const void* ptr, uint64_t inner, uint64_t outer, uint64_t ld_elems, uint32_t box_outer);
 

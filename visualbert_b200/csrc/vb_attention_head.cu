@@ -1,13 +1,13 @@
-// vb_attention_head.cu — persistent whole-head mma.sync attention kernels for seq <= 256 (the fallback of the wgmma
-// kernels in vb_attention_wgmma.cu: 192 < seq <= 256, or VB_ATTN_HEAD=1).
+// vb_attention_head.cu — persistent whole-head mma.sync attention kernels for 192 < seq <= 256 (beyond the wgmma kernels
+// of vb_attention_wgmma.cu, whose backward does not fit in shared memory there).
 //
 // The staged kernels in vb_attention.cu launch one short-lived CTA per (batch, head, 64-query block): each
-// re-loads the head's K/V and spends much of its short life waiting for that load. Here one CTA owns a whole (batch, head): NW = ceil(S/16) warps, each with 16 query rows
+// re-loads the head's K/V and spends much of its short life waiting for that load. Here one CTA owns a whole (batch, head): NW = 16 warps, each with 16 query rows
 // (and, in backward, 16 key rows); Q/K/V (and dO) tiles are loaded ONCE per head with cp.async, and the CTA is
 // persistent — it walks over heads and prefetches the next head's tiles into the second shared-memory buffer
 // while computing the current one, so the tensor pipe never waits for HBM/L2 latency.
 //
-//   forward   smem 2 x (Q, K, V) tiles          S=164: 2 x 72 KB   12 warps/CTA, 1 CTA/SM
+//   forward   smem 2 x (Q, K, V) tiles          S=256: 2 x 96 KB   16 warps/CTA, 1 CTA/SM
 //   backward  delta pre-kernel: D = rowsum(dO * O)  (HBM-bound, one warp per token)
 //             fused kernel: smem (Q, K, V, dO) x {1,2} buffers; phase A: dQ (rows = queries),
 //             phase B: dK, dV (rows = keys) — the tiles are shared by both phases (loaded once, not 2 x 3 times).
@@ -478,195 +478,20 @@ attn_bwd_head_kernel(const AttnParams p, const int nkb, const int nbuf) {
 // ------------------------------------------------------------------------------------------------
 // host
 // ------------------------------------------------------------------------------------------------
-// ------------------------------------------------------------------------------------------------
-// backward, "PS" variant: P and dS of the whole head are kept in shared memory between the two phases, so the dK/dV
-// phase neither recomputes S^T = K Q^T and dP^T = V dO^T (64 of its 128 HMMAs per 16x64 unit) nor the exp2 / mask /
-// dropout work: it is two GEMMs whose A operands come from shared memory with ldmatrix.trans.
-//   phase A (rows = queries): S, P, dP, dS once; dQ += dS K;  P_drop and dS -> smem as bf16 [q][key] (pitch = 2*cols+16 B:
-//            an odd number of 16-byte chunks, so the 4-byte accumulator stores and the 8-row ldmatrix reads are
-//            bank-conflict free)
-//   phase B (rows = keys):    dV += P_drop^T dO,  dK += dS^T Q
-// Shared memory: Q|K|V|dO tiles (single buffer) + 2 x (lse, D, bias) vectors + P + dS = 227 KB at S = 164 (the limit), so
-// the next head cannot be double-buffered entirely: its K and V tiles (not needed by phase B) and its vectors are
-// prefetched during phase B, Q and dO at the top of its own iteration.
-// ------------------------------------------------------------------------------------------------
-template <int NW, bool VL = false>
-__global__ void __launch_bounds__(NW * 32, 1)
-attn_bwd_head_ps_kernel(const AttnParams p, const int nkb, const int colsP) {
-    constexpr int NT = NW * 32;
-    extern __shared__ __align__(128) uint8_t dsmem[];
-    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-    const int g = lane >> 2, t = lane & 3;
-    const int S = p.S;
-    const long long ld = 3LL * p.H;
-    const int np64 = nkb * kBlk;
-    const int tile_bytes = 4 * nkb * kTileBytes;
-    const int pitch = colsP * 2 + 16;            // bytes per P / dS row
-    const int rowsP = colsP;                     // query rows kept (= ceil16(S))
-    float* svec_all = reinterpret_cast<float*>(dsmem + tile_bytes);              // [2][3][np64]
-    const uint32_t sbase = smem_u32(dsmem);
-    const uint32_t sQ = sbase, sK = sbase + nkb * kTileBytes, sV = sbase + 2 * nkb * kTileBytes, sdO = sbase + 3 * nkb * kTileBytes;
-    const uint32_t sP = sbase + tile_bytes + 2 * 3 * np64 * 4;
-    const uint32_t sDS = sP + rowsP * pitch;
-    const int total = p.B * p.A;
-    const float sc2 = p.scale * kLog2e;
-    const int row0 = warp * 16;
-    const bool active = row0 < S;
-    const bool drop = p.drop_scale != 0.f;
-    const float ds = drop ? p.drop_scale : 1.f;
+// These kernels serve 192 < S <= 256 (attn_route): ceil(S / 16) is 13 .. 16 warps, so every launch has 16; warps whose rows
+// start past S only help with the loads.
+constexpr int kHeadWarps = 16;
 
-    auto issue_kv = [&](int item, int vb) {
-        const int b = item / p.A, h = item % p.A;
-        const SeqSpan sp = seq_span<VL>(p, b, h);
-        const int len = sp.len, nkv = VL ? (len + kBlk - 1) / kBlk : nkb;
-        const bf16* qbase = p.qkv + sp.row0 * ld + h * kHd;
-        load_rows<NT>(sK, qbase + p.H, ld, nkv, len, tid);
-        load_rows<NT>(sV, qbase + 2 * p.H, ld, nkv, len, tid);
-        cp_async_commit();
-        float* sv = svec_all + vb * 3 * np64;
-        const long long stat0 = VL ? sp.stat0 : static_cast<long long>(item) * S;
-        const float* lsep = p.lse + stat0;
-        const float* drp = p.drow + stat0;
-        for (int i = tid; i < np64; i += NT) {
-            sv[i] = i < len ? lsep[i] * kLog2e : INFINITY;  // +inf => p = 0 for padded queries
-            sv[np64 + i] = i < len ? drp[i] : 0.f;
-            sv[2 * np64 + i] = key_bias2<VL>(p, b, i, len);
-        }
-    };
-    auto issue_qdo = [&](int item) {
-        const int b = item / p.A, h = item % p.A;
-        const SeqSpan sp = seq_span<VL>(p, b, h);
-        const int len = sp.len, nkv = VL ? (len + kBlk - 1) / kBlk : nkb;
-        load_rows<NT>(sQ, p.qkv + sp.row0 * ld + h * kHd, ld, nkv, len, tid);
-        load_rows<NT>(sdO, p.dctx + sp.row0 * p.H + h * kHd, p.H, nkv, len, tid);
-        cp_async_commit();
-    };
-
-    int item = blockIdx.x;
-    if (item >= total) return;
-    pdl_trigger();
-    pdl_wait();
-    issue_kv(item, 0);
-    int vb = 0;
-    for (; item < total; item += gridDim.x, vb ^= 1) {
-        issue_qdo(item);
-        cp_async_wait<0>();
-        __syncthreads();
-        const int b = item / p.A, h = item % p.A;
-        const SeqSpan sp = seq_span<VL>(p, b, h);
-        const int len = sp.len, nkv = VL ? (len + kBlk - 1) / kBlk : nkb;
-        // rows of P / dS that phase A writes (every warp with a row of the sequence writes its 16 rows)
-        const int rowsv = VL ? (len + 15) / 16 * 16 : rowsP;
-        const bool act = VL ? row0 < len : active;
-        const unsigned bh = static_cast<unsigned>(item);
-        const float* slse = svec_all + vb * 3 * np64;
-        const float* sD = slse + np64;
-        const float* sbias = slse + 2 * np64;
-        bf16* dbase = p.dqkv + sp.row0 * ld + h * kHd;
-        const int mytile = warp >> 2, myrow = (warp & 3) * 16;
-
-        // ---------------- phase A: S, P, dP, dS once; dQ; P_drop / dS -> shared memory ----------------
-        if (act) {
-            uint32_t qf[4][4], dof[4][4];
-            load_afrag(qf, sQ + mytile * kTileBytes, myrow, lane);
-            load_afrag(dof, sdO + mytile * kTileBytes, myrow, lane);
-            const float lse0 = slse[row0 + g], lse1 = slse[row0 + g + 8];
-            const float d0 = sD[row0 + g], d1 = sD[row0 + g + 8];
-            const uint32_t prow0 = (row0 + g) * pitch, prow1 = (row0 + g + 8) * pitch;
-            float dq[8][4];
-            zero_acc(dq);
-            for (int kb = 0; kb < nkv; ++kb) {
-                const int kvalid = min(kBlk, len - kb * kBlk);
-                unsigned long long keep_a = ~0ull, keep_c = ~0ull;
-                if (drop) {
-                    const unsigned long long* kp = p.keep + (static_cast<unsigned long long>(bh) * np64) * nkb;
-                    keep_a = kp[static_cast<long long>(row0 + g) * nkb + kb];
-                    keep_c = kp[static_cast<long long>(row0 + g + 8) * nkb + kb];
-                }
-                float s[8][4];
-                zero_acc(s);
-                gemm_nt(s, qf, sK + kb * kTileBytes, lane, kvalid);
-#pragma unroll
-                for (int hh = 0; hh < 2; ++hh) {  // dP = dO V^T in two 32-key halves (register pressure)
-                    float dp[4][4];
-#pragma unroll
-                    for (int i = 0; i < 4; ++i) dp[i][0] = dp[i][1] = dp[i][2] = dp[i][3] = 0.f;
-                    gemm_nt_half(dp, dof, sV + kb * kTileBytes, lane, hh, kvalid);
-#pragma unroll
-                    for (int n4 = 0; n4 < 4; ++n4) {
-                        const int nt = hh * 4 + n4, bit = nt * 8 + 2 * t;
-                        const float b0 = sbias[kb * kBlk + bit], b1 = sbias[kb * kBlk + bit + 1];
-                        const float p0 = fast_ex2(fmaf(s[nt][0], sc2, b0) - lse0), p1 = fast_ex2(fmaf(s[nt][1], sc2, b1) - lse0);
-                        const float p2 = fast_ex2(fmaf(s[nt][2], sc2, b0) - lse1), p3 = fast_ex2(fmaf(s[nt][3], sc2, b1) - lse1);
-                        const bool k0 = (keep_a >> bit) & 1ull, k1 = (keep_a >> (bit + 1)) & 1ull;
-                        const bool k2 = (keep_c >> bit) & 1ull, k3 = (keep_c >> (bit + 1)) & 1ull;
-                        const float e0 = k0 ? dp[n4][0] * ds : 0.f, e1 = k1 ? dp[n4][1] * ds : 0.f;
-                        const float e2 = k2 ? dp[n4][2] * ds : 0.f, e3 = k3 ? dp[n4][3] * ds : 0.f;
-                        s[nt][0] = p0 * (e0 - d0); s[nt][1] = p1 * (e1 - d0);
-                        s[nt][2] = p2 * (e2 - d1); s[nt][3] = p3 * (e3 - d1);
-                        const int col = kb * kBlk + bit;
-                        if (col < colsP) {  // warp-uniform per (kb, nt): colsP is a multiple of 16
-                            st_shared_u32(sP + prow0 + col * 2, pack_bf16x2(k0 ? p0 * ds : 0.f, k1 ? p1 * ds : 0.f));
-                            st_shared_u32(sP + prow1 + col * 2, pack_bf16x2(k2 ? p2 * ds : 0.f, k3 ? p3 * ds : 0.f));
-                            st_shared_u32(sDS + prow0 + col * 2, pack_bf16x2(s[nt][0], s[nt][1]));
-                            st_shared_u32(sDS + prow1 + col * 2, pack_bf16x2(s[nt][2], s[nt][3]));
-                        }
-                    }
-                }
-                uint32_t dsf[4][4];
-                acc_to_afrag(dsf, s);
-                gemm_nn(dq, dsf, sK + kb * kTileBytes, lane, kvalid);
-            }
-            store_acc(dbase, ld, row0, len, dq, lane, p.scale, p.scale);
-        }
-        __syncthreads();  // P / dS complete; K and V tiles are dead from here on
-
-        const int next = item + gridDim.x;
-        if (next < total) issue_kv(next, vb ^ 1);  // overlaps phase B
-
-        // ---------------- phase B: dV = P_drop^T dO, dK = dS^T Q for key rows row0 .. row0+15 ----------------
-        if (act) {
-            float dk[8][4], dv[8][4];
-            zero_acc(dk);
-            zero_acc(dv);
-            // ldmatrix.trans address of this lane: matrix i = lane >> 3 -> (query half i >> 1, key half i & 1)
-            const uint32_t a_off = (((lane >> 4) & 1) * 8 + (lane & 7)) * pitch + (row0 + ((lane >> 3) & 1) * 8) * 2;
-            for (int qb = 0; qb < nkv; ++qb) {
-                const int qvalid = min(kBlk, rowsv - qb * kBlk);
-                if (qvalid <= 0) break;
-                uint32_t af[4][4];
-#pragma unroll
-                for (int ks = 0; ks < 4; ++ks)
-                    if (ks * 16 < qvalid)
-                        ldsm_x4_t(sP + (qb * kBlk + ks * 16) * pitch + a_off, af[ks][0], af[ks][1], af[ks][2], af[ks][3]);
-                gemm_nn(dv, af, sdO + qb * kTileBytes, lane, qvalid);
-#pragma unroll
-                for (int ks = 0; ks < 4; ++ks)
-                    if (ks * 16 < qvalid)
-                        ldsm_x4_t(sDS + (qb * kBlk + ks * 16) * pitch + a_off, af[ks][0], af[ks][1], af[ks][2], af[ks][3]);
-                gemm_nn(dk, af, sQ + qb * kTileBytes, lane, qvalid);
-            }
-            store_acc(dbase + p.H, ld, row0, len, dk, lane, p.scale, p.scale);
-            store_acc(dbase + 2 * p.H, ld, row0, len, dv, lane, 1.f, 1.f);
-        }
-        __syncthreads();  // Q / dO tiles and P / dS are free for the next head
-    }
-}
-
-template <int NW, bool VL>
-static int launch_fwd_t(const AttnParams& p, int nkb, cudaStream_t st) {
+template <bool VL>
+static int launch_fwd(const AttnParams& p, int nkb, cudaStream_t st) {
     const int smem = 2 * 3 * nkb * kTileBytes + 2 * nkb * kBlk * 4;
     static int configured[kMaxDevices] = {0};
-    VB_CHECK_CUDA(ensure_dyn_smem(attn_fwd_head_kernel<NW, VL>, smem, configured));
+    VB_CHECK_CUDA(ensure_dyn_smem(attn_fwd_head_kernel<kHeadWarps, VL>, smem, configured));
     const int total = p.B * p.A;
     const int grid = total < num_sms() ? total : num_sms();
     ProfScope ps(st, PROF_ATTN_FWD, 4.0 * p.B * p.A * p.S * p.S * kHd, 1);
-    VB_CHECK_CUDA(launch_pdl(attn_fwd_head_kernel<NW, VL>, dim3(grid), dim3(NW * 32), smem, st, p, nkb));
+    VB_CHECK_CUDA(launch_pdl(attn_fwd_head_kernel<kHeadWarps, VL>, dim3(grid), dim3(kHeadWarps * 32), smem, st, p, nkb));
     return 0;
-}
-template <int NW>
-static int launch_fwd(const AttnParams& p, int nkb, cudaStream_t st) {
-    return p.cu_seqlens ? launch_fwd_t<NW, true>(p, nkb, st) : launch_fwd_t<NW, false>(p, nkb, st);
 }
 
 // draws the attention-dropout keep bits of the whole layer call (no-op without dropout)
@@ -681,64 +506,27 @@ int attn_keep_mask(const AttnParams& p, int nkb, cudaStream_t st) {
     return 0;
 }
 
-int attn_fwd_head(const AttnParams& p, int nkb, cudaStream_t st, bool mask_ready) {
-    const int nw = (p.S + 15) / 16;
-    int rc = mask_ready ? 0 : attn_keep_mask(p, nkb, st);
+int attn_fwd_head(const AttnParams& p, int nkb, cudaStream_t st) {
+    int rc = attn_keep_mask(p, nkb, st);
     if (rc) return rc;
-    if (nw <= 4) rc = launch_fwd<4>(p, nkb, st);
-    else if (nw <= 8) rc = launch_fwd<8>(p, nkb, st);
-    else if (nw <= 12) rc = launch_fwd<12>(p, nkb, st);
-    else rc = launch_fwd<16>(p, nkb, st);
+    rc = p.cu_seqlens ? launch_fwd<true>(p, nkb, st) : launch_fwd<false>(p, nkb, st);
     if (rc) return rc;
     VB_CHECK_CUDA(cudaGetLastError());
     return 0;
 }
 
-template <int NW, bool VL>
-static int launch_bwd_t(const AttnParams& p, int nkb, cudaStream_t st) {
+template <bool VL>
+static int launch_bwd(const AttnParams& p, int nkb, cudaStream_t st) {
     const int per_buf = 4 * nkb * kTileBytes + 3 * nkb * kBlk * 4;
     const int nbuf = 2 * per_buf <= 200 * 1024 ? 2 : 1;
     const int smem = nbuf * per_buf;
     static int configured[kMaxDevices] = {0};
-    VB_CHECK_CUDA(ensure_dyn_smem(attn_bwd_head_kernel<NW, VL>, smem, configured));
+    VB_CHECK_CUDA(ensure_dyn_smem(attn_bwd_head_kernel<kHeadWarps, VL>, smem, configured));
     const int total = p.B * p.A;
     const int grid = total < num_sms() ? total : num_sms();
     ProfScope ps(st, PROF_ATTN_DKV, 7.0 * p.B * p.A * p.S * p.S * kHd, 1);
-    VB_CHECK_CUDA(launch_pdl(attn_bwd_head_kernel<NW, VL>, dim3(grid), dim3(NW * 32), smem, st, p, nkb, nbuf));
+    VB_CHECK_CUDA(launch_pdl(attn_bwd_head_kernel<kHeadWarps, VL>, dim3(grid), dim3(kHeadWarps * 32), smem, st, p, nkb, nbuf));
     return 0;
-}
-template <int NW>
-static int launch_bwd(const AttnParams& p, int nkb, cudaStream_t st) {
-    return p.cu_seqlens ? launch_bwd_t<NW, true>(p, nkb, st) : launch_bwd_t<NW, false>(p, nkb, st);
-}
-
-// P/dS-in-shared-memory variant: only when the whole head fits (S <= ~176); VB_ATTN_BWD_PS=0 disables it
-template <int NW, bool VL>
-static int launch_bwd_ps_t(const AttnParams& p, int nkb, int colsP, int smem, cudaStream_t st) {
-    static int configured[kMaxDevices] = {0};
-    VB_CHECK_CUDA(ensure_dyn_smem(attn_bwd_head_ps_kernel<NW, VL>, smem, configured));
-    const int total = p.B * p.A;
-    const int grid = total < num_sms() ? total : num_sms();
-    ProfScope ps(st, PROF_ATTN_DKV, 5.0 * p.B * p.A * p.S * p.S * kHd, 1);
-    VB_CHECK_CUDA(launch_pdl(attn_bwd_head_ps_kernel<NW, VL>, dim3(grid), dim3(NW * 32), smem, st, p, nkb, colsP));
-    return 0;
-}
-template <int NW>
-static int launch_bwd_ps(const AttnParams& p, int nkb, int colsP, int smem, cudaStream_t st) {
-    return p.cu_seqlens ? launch_bwd_ps_t<NW, true>(p, nkb, colsP, smem, st) : launch_bwd_ps_t<NW, false>(p, nkb, colsP, smem, st);
-}
-
-static int bwd_ps_smem(const AttnParams& p, int nkb, int* colsP) {
-    static int enabled = -1;
-    if (enabled < 0) {
-        const char* e = getenv("VB_ATTN_BWD_PS");
-        enabled = (e && e[0] == '0') ? 0 : 1;
-    }
-    const int max_smem = 227 * 1024;  // sm_90a opt-in limit per block (the library targets this arch only)
-    if (!enabled) return 0;
-    *colsP = (p.S + 15) / 16 * 16;
-    const int smem = 4 * nkb * kTileBytes + 2 * 3 * nkb * kBlk * 4 + 2 * (*colsP) * ((*colsP) * 2 + 16);
-    return smem <= max_smem ? smem : 0;
 }
 
 // D[b, h, q] = sum_d dO * O  (the softmax-backward row term), HBM-bound pre-pass shared by the backward kernels
@@ -761,18 +549,7 @@ int attn_bwd_head(const AttnParams& p, int nkb, cudaStream_t st, bool delta_read
         int rc0 = attn_delta(p, st);
         if (rc0) return rc0;
     }
-    const int nw = (p.S + 15) / 16;
-    int rc, colsP = 0;
-    const int ps_smem = bwd_ps_smem(p, nkb, &colsP);
-    if (ps_smem > 0) {
-        if (nw <= 4) rc = launch_bwd_ps<4>(p, nkb, colsP, ps_smem, st);
-        else if (nw <= 8) rc = launch_bwd_ps<8>(p, nkb, colsP, ps_smem, st);
-        else if (nw <= 12) rc = launch_bwd_ps<12>(p, nkb, colsP, ps_smem, st);
-        else rc = launch_bwd_ps<16>(p, nkb, colsP, ps_smem, st);
-    } else if (nw <= 4) rc = launch_bwd<4>(p, nkb, st);
-    else if (nw <= 8) rc = launch_bwd<8>(p, nkb, st);
-    else if (nw <= 12) rc = launch_bwd<12>(p, nkb, st);
-    else rc = launch_bwd<16>(p, nkb, st);
+    const int rc = p.cu_seqlens ? launch_bwd<true>(p, nkb, st) : launch_bwd<false>(p, nkb, st);
     if (rc) return rc;
     VB_CHECK_CUDA(cudaGetLastError());
     return 0;

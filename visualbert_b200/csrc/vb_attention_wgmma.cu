@@ -21,7 +21,6 @@
 namespace vb {
 
 constexpr int kWgTile = kBlk * kHd * 2;   // one 64 x 64 bf16 tile, 128B-swizzled rows (8 KB)
-constexpr int kMaxWgmmaBlocks = 3;         // seq <= 192: the backward's Q, K, V, dO and P/dS tiles fit in shared memory
 
 template <int NKB>
 struct AttnSmem {
@@ -360,11 +359,6 @@ attn_bwd_wgmma_kernel(const __grid_constant__ CUtensorMap tmQKV, const __grid_co
 // ------------------------------------------------------------------------------------------------
 // host
 // ------------------------------------------------------------------------------------------------
-bool attn_wgmma_supported(const AttnParams& p) {
-    return p.S <= kMaxWgmmaBlocks * kBlk && (reinterpret_cast<uintptr_t>(p.qkv) & 15) == 0 && (p.H * 2) % 16 == 0 &&
-           (p.dctx == nullptr || (reinterpret_cast<uintptr_t>(p.dctx) & 15) == 0);
-}
-
 template <int NKB, bool VL = false>
 static int launch_fwd_wgmma(const AttnParams& p, const CUtensorMap& tq, cudaStream_t st) {
     auto kern = attn_fwd_wgmma_kernel<NKB, VL>;
@@ -384,16 +378,14 @@ static int launch_bwd_wgmma(const AttnParams& p, const CUtensorMap& tq, const CU
     return 0;
 }
 
-int attn_fwd_wgmma(const AttnParams& p, cudaStream_t st, bool mask_ready) {
+int attn_fwd_wgmma(const AttnParams& p, cudaStream_t st) {
     const int nkb = (p.S + kBlk - 1) / kBlk;
-    if (!mask_ready) {
-        int rc = attn_keep_mask(p, nkb, st);
-        if (rc) return rc;
-    }
+    int rc = attn_keep_mask(p, nkb, st);
+    if (rc) return rc;
     CUtensorMap tq;
     const bool vl = p.cu_seqlens != nullptr;
     const uint64_t rows = vl ? static_cast<uint64_t>(p.total) : static_cast<uint64_t>(p.B) * p.S;
-    int rc = make_tmap_bf16(&tq, p.qkv, 3ull * p.H, rows, 3ull * p.H, kBlk);
+    rc = make_tmap_bf16(&tq, p.qkv, 3ull * p.H, rows, 3ull * p.H, kBlk);
     if (rc) return rc;
     if (vl) {
         if (nkb == 1) rc = launch_fwd_wgmma<1, true>(p, tq, st);

@@ -41,8 +41,6 @@ enum { PROF_GEMM_FWD = 0, PROF_GEMM_DGRAD = 1, PROF_GEMM_WGRAD = 2, PROF_ATTN_FW
 // scheduled, and run their on-chip prologue (barrier init, tensor-map prefetch), while the previous
 // kernel's last CTAs drain. Every such kernel calls pdl_trigger() on entry and pdl_wait() BEFORE its first global
 // memory access (griddepcontrol.wait returns once the preceding grid has completed and its writes are visible).
-// VB_PDL=0 in the environment turns the attribute off (plain stream order).
-bool pdl_enabled();
 #ifdef __CUDACC__
 __device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
 __device__ __forceinline__ void pdl_trigger() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
@@ -57,7 +55,7 @@ inline cudaError_t launch_pdl(void (*kernel)(KArgs...), dim3 grid, dim3 block, s
     attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
     attr[0].val.programmaticStreamSerializationAllowed = 1;
     cfg.attrs = attr;
-    cfg.numAttrs = pdl_enabled() ? 1 : 0;
+    cfg.numAttrs = 1;
     return cudaLaunchKernelEx(&cfg, kernel, static_cast<KArgs>(args)...);
 }
 #endif

@@ -584,22 +584,12 @@ static int wgrad_splits(long long tiles, int k_blocks) {
     return best;
 }
 
-bool pdl_enabled() {
-    static const bool on = [] {
-        const char* e = getenv("VB_PDL");
-        return !(e && e[0] == '0');
-    }();
-    return on;
-}
-
 bool gemm_delta_ok(int M, int N) {
-    static const int off = [] { const char* e = getenv("VB_GEMM_DELTA"); return (e != nullptr && atoi(e) == 0) ? 1 : 0; }();
     const int n_pad256 = (N + 255) / 256 * 256;
-    return !off && M >= 256 && N >= 256 && N % 64 == 0 && (n_pad256 - N) * 8 <= N;
+    return M >= 256 && N >= 256 && N % 64 == 0 && (n_pad256 - N) * 8 <= N;
 }
 bool gemm_gp_tiled_ok(int M, int N) {
-    static const int off = [] { const char* e = getenv("VB_GEMM_GP_TILED"); return (e != nullptr && atoi(e) == 0) ? 1 : 0; }();
-    return !off && M >= 256 && M % 256 == 0 && N % 256 == 0;
+    return M >= 256 && M % 256 == 0 && N % 256 == 0;
 }
 
 int gemm(const vb_gemm_args& a, cudaStream_t st) {
@@ -642,10 +632,7 @@ int gemm(const vb_gemm_args& a, cudaStream_t st) {
         p.addend = static_cast<const bf16*>(a.delta_ctx); p.ld_add = a.N;
         p.delta_out = a.delta_out; p.delta_seq = a.delta_seq;
     }
-    {
-        static const int order_off = [] { const char* e = getenv("VB_GEMM_TILE_ORDER"); return (e != nullptr && atoi(e) == 0) ? 1 : 0; }();
-        p.m_fast = (!order_off && (a.M + BLOCK_M - 1) / BLOCK_M < (a.N + 255) / 256) ? 1 : 0;
-    }
+    p.m_fast = (a.M + BLOCK_M - 1) / BLOCK_M < (a.N + 255) / 256 ? 1 : 0;
     if (a.dropout_p > 0.0f) {
         const DropQ q = dropout_quantise(a.dropout_p);
         p.drop_scale = q.scale;

@@ -13,22 +13,23 @@ int ln_fwd(const void* x, long long ldx, const float* gamma, const float* beta, 
 int ln_bwd(const void* dy, const void* x, const float* mean, const float* rstd, const float* gamma, void* dx,
            void* dx_drop, float* dgamma, float* dbeta, float* dbias, int rows, int H, float dropout_p,
            unsigned long long seed, unsigned stream_id, float in_dropout_p, unsigned in_stream_id, cudaStream_t st);
+// The attention kernels that serve a call, from its sequence length (varlen calls: the longest one): the wgmma kernels up to
+// 192 (their backward keeps Q, K, V, dO and P/dS of the whole head in shared memory), the whole-head mma.sync kernels up to
+// 256, the staged kernels beyond. The two fused routes take a pre-computed D = rowsum(dO * O) (delta_ready below).
+enum class AttnRoute { Wgmma, Head, Staged };
+inline AttnRoute attn_route(int S) { return S <= 192 ? AttnRoute::Wgmma : S <= 256 ? AttnRoute::Head : AttnRoute::Staged; }
 int attn_fwd(const void* qkv, const float* mask_bias, void* ctx, float* lse, void* keep, int B, int S, int A, int H,
-             float dropout_p, unsigned long long seed, unsigned stream_id, cudaStream_t st, bool mask_ready = false);
-int attn_mask_async(void* keep, int B, int S, int A, int H, float dropout_p, unsigned long long seed, unsigned stream_id,
-                    cudaEvent_t before_gemm, cudaStream_t main);
+             float dropout_p, unsigned long long seed, unsigned stream_id, cudaStream_t st);
 int attn_bwd(const void* qkv, const float* mask_bias, const void* ctx, const float* lse, const void* keep,
              const void* dctx, void* dqkv, float* drow, int B, int S, int A, int H, float dropout_p,
              unsigned long long seed, unsigned stream_id, cudaStream_t st, bool delta_ready = false);
 // variable-length attention: sequence b owns packed rows [cu_seqlens[b], cu_seqlens[b+1]) (device), at most max_seq of them;
 // lse / drow are [A, total]
 int attn_fwd_varlen(const void* qkv, const int* cu_seqlens, void* ctx, float* lse, void* keep, int B, int max_seq, int total,
-                    int A, int H, float dropout_p, unsigned long long seed, unsigned stream_id, cudaStream_t st, bool mask_ready = false);
+                    int A, int H, float dropout_p, unsigned long long seed, unsigned stream_id, cudaStream_t st);
 int attn_bwd_varlen(const void* qkv, const int* cu_seqlens, const void* ctx, const float* lse, const void* keep,
                     const void* dctx, void* dqkv, float* drow, int B, int max_seq, int total, int A, int H, float dropout_p,
                     unsigned long long seed, unsigned stream_id, cudaStream_t st, bool delta_ready = false);
-// true when attn_bwd for this shape runs the kernel that takes D = rowsum(dO * O) from `drow` (so a caller may provide it)
-bool attn_bwd_takes_delta(const void* qkv, const void* dctx, void* dqkv, int B, int S, int A, int H);
 long long attn_keep_bytes(int B, int S, int A);
 int colsum(const void* x, long long ld, float* out, int M, int N, cudaStream_t st);
 int cast_f32_bf16(const float* src, void* dst, long long n, cudaStream_t st);

@@ -223,8 +223,7 @@ class BertEncoder(nn.Module):
         if attention_mask.dim() == 4:
             attention_mask = attention_mask[:, 0, 0, :]
         fused = (not self.output_attention_weights and hidden_states.is_cuda and len(self.layer) > 0
-                 and not (output_all_encoded_layers and torch.is_grad_enabled() and self.training)
-                 and os.environ.get("VB_ENCODER_FUSED", "1") != "0")
+                 and not (output_all_encoded_layers and torch.is_grad_enabled() and self.training))
         if fused:
             # one C call for the whole stack (vb_encoder_fwd / vb_encoder_bwd, one activation arena)
             ys = ops.bert_encoder(hidden_states.to(torch.bfloat16), attention_mask.float().contiguous(), self._fused_meta(seed),
