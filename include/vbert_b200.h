@@ -23,7 +23,7 @@
 extern "C" {
 #endif
 
-#define VB_ABI_VERSION 3
+#define VB_ABI_VERSION 4
 
 /* ---- library ---------------------------------------------------------------------------- */
 int vb_abi_version(void);
@@ -131,6 +131,14 @@ int vb_attention_fwd_varlen(const void* qkv, const int32_t* cu_seqlens, void* ct
 int vb_attention_bwd_varlen(const void* qkv, const int32_t* cu_seqlens, const void* ctx, const float* lse, const void* keep_mask,
                             const void* dctx, void* dqkv, float* drow, int32_t batch, int32_t max_seq, int32_t total, int32_t heads,
                             int32_t hidden, float dropout_p, uint64_t dropout_seed, uint32_t dropout_stream, void* stream);
+/* Attention maps (the tensor output_attention_weights returns, M.py:241-247, 258-259): probs fp32 [batch, heads, seq, seq],
+ * probs[b,h,i,j] = softmax_j(q_i . k_j / 8 + mask_bias[b,j]) from the bf16 Q and K of qkv (laid out as for vb_attention_fwd),
+ * BEFORE dropout. Every element is written; masked keys (-10000) come out as exact zeros, and an example whose keys are all
+ * masked gets softmax(QK^T / 8) over all keys. The kernel computes its own row statistics (it does not read the forward's
+ * lse), so the maps are accurate to fp32 rounding for every mask. The argument checks of vb_attention_fwd apply (head_dim 64,
+ * qkv 16-byte aligned). */
+int vb_attention_probs(const void* qkv, const float* mask_bias, float* probs, int32_t batch, int32_t seq, int32_t heads,
+                       int32_t hidden, void* stream);
 
 /* ---- helpers ----------------------------------------------------------------------------- */
 /* (1 - cat(input_mask, image_mask)) * -10000 -> fp32 [batch, text+regions]  (M.py:1417, 1286-1294);
@@ -240,6 +248,11 @@ int vb_encoder_fwd(const vb_layer_desc* descs, int32_t n_layers, const void* x_i
 /* dy: gradient w.r.t. the LAST layer's output; dx: gradient w.r.t. x_in; grads: HOST array [n_layers]. */
 int vb_encoder_bwd(const vb_layer_desc* descs, int32_t n_layers, const void* x_in, void* arena, const void* dy, void* dx,
                    const vb_layer_grads* grads, const vb_layer_scratch* scratch, void* stream);
+/* The attention maps of every layer of a dense vb_encoder_fwd call (analysis mode, M.py:1316-1324, 1430-1444): probs fp32
+ * [n_layers, batch, heads, seq, seq] = vb_attention_probs of each layer, from the qkv buffer of its arena slot and its
+ * descs[l].mask_bias. Call it on the arena and descriptors vb_encoder_fwd just used, before anything overwrites the arena;
+ * one launch per layer, no other arena buffer is read. */
+int vb_encoder_attention_probs(const vb_layer_desc* descs, int32_t n_layers, void* arena, float* probs, void* stream);
 /* Variable-length ("unpadded") encoder: the same calls over `total` packed rows (see vb_attention_fwd_varlen for cu_seqlens and
  * its caller contract). descs[l].batch is the number of sequences and descs[l].seq the longest length (max_seq); mask_bias is
  * ignored and may be NULL. x_in, dy, dx and every row-sized arena / scratch buffer have `total` rows; lse and scratch.drow are

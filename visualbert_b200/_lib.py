@@ -10,7 +10,7 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 # VB_LIB_PATH: load another build of the same library (A/B timing of kernel variants on one GPU, scripts/build_variant.sh)
 LIB_PATH = os.environ.get("VB_LIB_PATH") or os.path.join(_HERE, "lib", "libvbert_b200.so")
 
-ABI_VERSION = 3   # == VB_ABI_VERSION of include/vbert_b200.h (tests/test_abi.py keeps the two in step)
+ABI_VERSION = 4  # == VB_ABI_VERSION of include/vbert_b200.h (tests/test_abi.py keeps the two in step)
 VB_EPI_NONE, VB_EPI_GELU, VB_EPI_DGELU = 0, 1, 2
 
 c_void_p, c_int, c_i64, c_f32, c_u64, c_u32 = (
@@ -79,7 +79,7 @@ EXPORTS = [
     "vb_colsum_bf16", "vb_cross_entropy_fwd", "vb_cross_entropy_bwd", "vb_layer_fwd", "vb_layer_bwd", "vb_embed_fwd", "vb_embed_bwd",
     "vb_bert_adam_step", "vb_cast_multi", "vb_encoder_arena_layout", "vb_encoder_fwd", "vb_encoder_bwd",
     "vb_attention_fwd_varlen", "vb_attention_bwd_varlen", "vb_encoder_arena_layout_varlen", "vb_encoder_fwd_varlen",
-    "vb_encoder_bwd_varlen",
+    "vb_encoder_bwd_varlen", "vb_attention_probs", "vb_encoder_attention_probs",
 ]
 VB_ENCODER_ARENA_BUFFERS = 14
 ARENA_NAMES = ("qkv", "ctx", "lse", "pre1", "mean1", "rstd1", "x1", "u", "g", "pre2", "mean2", "rstd2", "keep_mask", "y")
@@ -113,6 +113,8 @@ def lib():
         h.vb_encoder_arena_layout_varlen.argtypes = [_I, _I, _I, _I, _I, _I, _I, _P]
         h.vb_encoder_fwd_varlen.argtypes = [_P, _I, _P, _I, _P, _P, _P]
         h.vb_encoder_bwd_varlen.argtypes = [_P, _I, _P, _I, _P, _P, _P, _P, _P, _P, _P]
+        h.vb_attention_probs.argtypes = [_P, _P, _P, _I, _I, _I, _I, _P]
+        h.vb_encoder_attention_probs.argtypes = [_P, _I, _P, _P, _P]
         _lib = h
     return _lib
 

@@ -224,6 +224,26 @@ int encoder_bwd(const vb_layer_desc* descs, int n, const void* x_in, void* arena
     return 0;
 }
 
+// the attention maps of every layer of a dense vb_encoder_fwd, from the qkv each layer slot of the arena holds
+int encoder_attention_probs(const vb_layer_desc* descs, int n, void* arena, float* probs, cudaStream_t st) {
+    VB_REQUIRE(descs && n > 0 && arena && probs, "encoder_attention_probs: null pointer / no layers");
+    for (int l = 0; l < n; ++l) {  // every descriptor is checked before the first launch: a refused call writes nothing
+        VB_TRY(check_layer(&descs[l], kDenseRows));
+        VB_REQUIRE(descs[l].batch == descs[0].batch && descs[l].seq == descs[0].seq && descs[l].hidden == descs[0].hidden &&
+                   descs[l].heads == descs[0].heads && descs[l].inter == descs[0].inter &&
+                   (descs[l].attn_dropout > 0.f) == (descs[0].attn_dropout > 0.f), "encoder_attention_probs: layers differ in shape");
+    }
+    const long long per_layer = static_cast<long long>(descs[0].batch) * descs[0].heads * descs[0].seq * descs[0].seq;
+    for (int l = 0; l < n; ++l) {
+        vb_layer_acts a;
+        void* y;
+        arena_acts(&descs[l], arena, l, &a, &y, kDenseRows);
+        VB_TRY(attn_probs(a.qkv, descs[l].mask_bias, probs + l * per_layer, descs[l].batch, descs[l].seq, descs[l].heads,
+                          descs[l].hidden, st));
+    }
+    return 0;
+}
+
 static int check_embed(const vb_embed_desc* d) {
     VB_REQUIRE(d != nullptr, "embed: null descriptor");
     VB_REQUIRE(d->batch > 0 && d->text_len > 0 && d->num_regions >= 0, "embed: bad shape");
@@ -317,6 +337,9 @@ int vb_encoder_fwd(const vb_layer_desc* descs, int32_t n_layers, const void* x_i
 int vb_encoder_bwd(const vb_layer_desc* descs, int32_t n_layers, const void* x_in, void* arena, const void* dy, void* dx,
                    const vb_layer_grads* grads, const vb_layer_scratch* scratch, void* stream) {
     return vb::encoder_bwd(descs, n_layers, x_in, arena, dy, dx, grads, scratch, static_cast<cudaStream_t>(stream));
+}
+int vb_encoder_attention_probs(const vb_layer_desc* descs, int32_t n_layers, void* arena, float* probs, void* stream) {
+    return vb::encoder_attention_probs(descs, n_layers, arena, probs, static_cast<cudaStream_t>(stream));
 }
 int64_t vb_encoder_arena_layout_varlen(int32_t batch, int32_t max_seq, int32_t total, int32_t hidden, int32_t heads, int32_t inter,
                                        int32_t attn_dropout_on, int64_t* offsets) {

@@ -31,6 +31,8 @@ int attn_bwd_varlen(const void* qkv, const int* cu_seqlens, const void* ctx, con
                     const void* dctx, void* dqkv, float* drow, int B, int max_seq, int total, int A, int H, float dropout_p,
                     unsigned long long seed, unsigned stream_id, cudaStream_t st, bool delta_ready = false);
 long long attn_keep_bytes(int B, int S, int A);
+// the pre-dropout attention maps softmax(QK^T / 8 + mask_bias) of a dense call, fp32 [B, A, S, S] (vb_attention_probs.cu)
+int attn_probs(const void* qkv, const float* mask_bias, float* probs, int B, int S, int A, int H, cudaStream_t st);
 int colsum(const void* x, long long ld, float* out, int M, int N, cudaStream_t st);
 int cast_f32_bf16(const float* src, void* dst, long long n, cudaStream_t st);
 int cast_bf16_f32(const void* src, float* dst, long long n, cudaStream_t st);

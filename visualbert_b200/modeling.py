@@ -171,35 +171,19 @@ class BertLayer(nn.Module):
         a = self.attention.self
         return ((a.query.weight, a.key.weight, a.value.weight), (a.query.bias, a.key.bias, a.value.bias))
 
-    def forward(self, hidden_states, attention_mask, seed=0):
+    def forward(self, hidden_states, attention_mask, seed=0, output_attention_probs=False):
         """hidden_states [B, S, H]; attention_mask: the fp32 additive key bias [B, S]
-        ((1 - mask) * -10000), or the reference's extended mask [B, 1, 1, S]."""
+        ((1 - mask) * -10000), or the reference's extended mask [B, 1, 1, S]. With output_attention_probs returns
+        (output, maps): maps = softmax(QK^T/sqrt(d) + mask) [B, A, S, S] in fp32 (M.py:241-247, 258-259), pre-dropout and
+        detached, computed by vb_attention_probs from the same bf16 Q and K the layer's attention used."""
         if attention_mask.dim() == 4:
             attention_mask = attention_mask[:, 0, 0, :]
         train = self.training
         meta = dict(heads=self.attention.self.num_attention_heads, layer_index=self.layer_index,
                     hidden_dropout=self.hidden_dropout_prob if train else 0.0,
                     attn_dropout=self.attention_probs_dropout_prob if train else 0.0,
-                    seed=int(seed), cache=self._weights, train=train)
+                    seed=int(seed), cache=self._weights, train=train, attn_maps=bool(output_attention_probs))
         return ops.bert_layer(hidden_states.to(torch.bfloat16), attention_mask.float().contiguous(), meta, self._params())
-
-    @torch.no_grad()
-    def attention_probabilities(self, hidden_states, attention_mask):
-        """softmax(QK^T/sqrt(d) + mask) [B, A, S, S] in fp32 — the tensor `output_attention_weights=True` asks for
-        (M.py:241-247, 258-259). The fused kernels never materialise it, so this analysis-only slow path recomputes it
-        with torch ops from the layer input; pre-dropout, detached."""
-        if attention_mask.dim() == 4:
-            attention_mask = attention_mask[:, 0, 0, :]
-        a = self.attention.self
-        x = hidden_states.float()
-        B, S, H = x.shape
-        A = a.num_attention_heads
-
-        def heads(lin):
-            return F.linear(x, lin.weight.float(), lin.bias.float()).view(B, S, A, H // A).permute(0, 2, 1, 3)
-
-        scores = torch.matmul(heads(a.query), heads(a.key).transpose(-1, -2)) / math.sqrt(H // A)
-        return torch.softmax(scores + attention_mask.float()[:, None, None, :], dim=-1)
 
 
 class BertEncoder(nn.Module):
@@ -208,12 +192,17 @@ class BertEncoder(nn.Module):
         self.layer = nn.ModuleList([BertLayer(config, i) for i in range(config.num_hidden_layers)])
         self.output_attention_weights = getattr(config, "output_attention_weights", False)
 
-    def forward(self, hidden_states, attention_mask, output_all_encoded_layers=True, seed=0, varlen=None):
+    def forward(self, hidden_states, attention_mask, output_all_encoded_layers=True, seed=0, varlen=None,
+                output_attention_weights=None):
         """varlen (ops.unpad_plan): unpadded call — hidden_states are the [total, H] packed valid rows, attention_mask is
         ignored, and every returned layer is [total, H]. It always runs the whole-encoder call (there is no per-layer
-        varlen path), so it cannot serve attention weights or gradients through intermediate layers."""
+        varlen path), so it cannot serve attention weights or gradients through intermediate layers.
+
+        output_attention_weights (default: the config's) returns (layers, maps), maps = one detached fp32 [B, A, S, S]
+        pre-dropout attention map per layer, written by the attention-probability kernel from each layer's own qkv."""
+        want_maps = self.output_attention_weights if output_attention_weights is None else output_attention_weights
         if varlen is not None:
-            if self.output_attention_weights or (output_all_encoded_layers and torch.is_grad_enabled() and self.training):
+            if want_maps or (output_all_encoded_layers and torch.is_grad_enabled() and self.training):
                 raise ValueError("unpadded encoder: attention weights and gradients through intermediate layers need the "
                                  "padded per-layer path")
             if len(self.layer) == 0:
@@ -222,23 +211,29 @@ class BertEncoder(nn.Module):
             return list(ys) if output_all_encoded_layers else [ys[-1]]
         if attention_mask.dim() == 4:
             attention_mask = attention_mask[:, 0, 0, :]
-        fused = (not self.output_attention_weights and hidden_states.is_cuda and len(self.layer) > 0
+        fused = (hidden_states.is_cuda and len(self.layer) > 0
                  and not (output_all_encoded_layers and torch.is_grad_enabled() and self.training))
         if fused:
-            # one C call for the whole stack (vb_encoder_fwd / vb_encoder_bwd, one activation arena)
-            ys = ops.bert_encoder(hidden_states.to(torch.bfloat16), attention_mask.float().contiguous(), self._fused_meta(seed),
-                                  self._fused_params())
-            return list(ys) if output_all_encoded_layers else [ys[-1]]
+            # one C call for the whole stack (vb_encoder_fwd / vb_encoder_bwd, one activation arena), and with maps one
+            # vb_encoder_attention_probs call over the same arena
+            meta = self._fused_meta(seed)
+            meta["attn_maps"] = want_maps
+            ys = ops.bert_encoder(hidden_states.to(torch.bfloat16), attention_mask.float().contiguous(), meta, self._fused_params())
+            L = len(self.layer)
+            outs = list(ys[:L]) if output_all_encoded_layers else [ys[L - 1]]
+            return (outs, list(ys[L:])) if want_maps else outs
         outs, attn = [], []
         for layer in self.layer:
-            if self.output_attention_weights:
-                attn.append(layer.attention_probabilities(hidden_states, attention_mask))
-            hidden_states = layer(hidden_states, attention_mask, seed)
+            if want_maps:
+                hidden_states, maps = layer(hidden_states, attention_mask, seed, output_attention_probs=True)
+                attn.append(maps)
+            else:
+                hidden_states = layer(hidden_states, attention_mask, seed)
             if output_all_encoded_layers:
                 outs.append(hidden_states)
         if not output_all_encoded_layers:
             outs.append(hidden_states)
-        return (outs, attn) if self.output_attention_weights else outs
+        return (outs, attn) if want_maps else outs
 
     def _fused_meta(self, seed, varlen=None):
         l0 = self.layer[0]
@@ -609,8 +604,9 @@ class BertVisualModel(PreTrainedBertModel):
             # rows of the embedding output are appended afterwards and one more BertLayer sees the whole sequence
             assert not output_all_encoded_layers  # "Don't support this for the bypass model" (M.py:1300)
             T = input_ids.size(1)
-            text = self.encoder(x[:, :T].contiguous(), bias[:, :T].contiguous(), output_all_encoded_layers=False, seed=seed)
-            text = text[0][-1] if self.output_attention_weights else text[-1]
+            # the text encoder's attention maps are not part of the bypass model's outputs: they are not computed
+            text = self.encoder(x[:, :T].contiguous(), bias[:, :T].contiguous(), output_all_encoded_layers=False, seed=seed,
+                                output_attention_weights=False)[-1]
             final = self.additional_layer(torch.cat((text, x[:, T:]), dim=1), bias, seed)
             return final, self.pooler(final)
         if self._unpadded:

@@ -216,12 +216,23 @@ class LayerWeights:
         return self.buf
 
 
+def attention_probs(qkv, mbias, B, S, A):
+    """Pre-dropout attention maps softmax(QK^T / 8 + mbias) as fp32 [B, A, S, S] from a layer's bf16 qkv [B*S, 3H]
+    (vb_attention_probs)."""
+    probs = torch.empty(B, A, S, S, device=qkv.device, dtype=torch.float32)
+    with torch.cuda.device(qkv.device):
+        _lib.check(_lib.lib().vb_attention_probs(qkv.data_ptr(), mbias.data_ptr(), probs.data_ptr(), B, S, A, qkv.shape[1] // 3,
+                                                 _stream()), "vb_attention_probs")
+    return probs
+
+
 class _LayerFn(torch.autograd.Function):
-    """BertLayer forward/backward (reference M.py:322-341) through vb_layer_fwd / vb_layer_bwd."""
+    """BertLayer forward/backward (reference M.py:322-341) through vb_layer_fwd / vb_layer_bwd. With meta["attn_maps"] the
+    forward also returns the layer's attention maps (attention_probs of its qkv), a non-differentiable second output."""
 
     @staticmethod
     def forward(ctx, x, mbias, meta, qw, qb, kw, kb, vw, vb, ow, ob, g1, b1, iw, ib, dw, db, g2, b2):
-        # meta: dict(heads, layer_index, hidden_dropout, attn_dropout, seed, cache=LayerWeights)
+        # meta: dict(heads, layer_index, hidden_dropout, attn_dropout, seed, cache=LayerWeights, optional attn_maps)
         _require_cuda(x, "bert_layer")
         B, S, H = x.shape
         I = iw.shape[0]
@@ -258,10 +269,14 @@ class _LayerFn(torch.autograd.Function):
         ctx.weights = (wqkv, wo, wi, wout, bqkv)
         ctx.weight_key = meta["cache"].key if meta["cache"].bank is None else None
         ctx.save_for_backward(x, mbias, ob, g1, b1, ib, db, g2, b2)
+        if meta.get("attn_maps"):
+            maps = attention_probs(acts["qkv"], mbias, B, S, A)
+            ctx.mark_non_differentiable(maps)
+            return y, maps
         return y
 
     @staticmethod
-    def backward(ctx, dy):
+    def backward(ctx, dy, *_maps_grad):
         x, mbias, ob, g1, b1, ib, db, g2, b2 = ctx.saved_tensors
         meta, acts = ctx.meta, ctx.acts
         if ctx.weight_key is not None and meta["cache"].key != ctx.weight_key:
@@ -355,7 +370,10 @@ class _EncoderFn(torch.autograd.Function):
 
     With meta["varlen"] = dict(cu_seqlens, batch, max_seq, total) the call is unpadded: x is [total, H], the packed valid rows
     (sequence b at rows cu_seqlens[b] .. cu_seqlens[b + 1]), mbias is None, and every output is [total, H]
-    (vb_encoder_fwd_varlen / vb_encoder_bwd_varlen)."""
+    (vb_encoder_fwd_varlen / vb_encoder_bwd_varlen).
+
+    With meta["attn_maps"] (dense calls only) the L layer outputs are followed by the L attention maps, fp32 [B, A, S, S] views
+    of one [L, B, A, S, S] tensor written by vb_encoder_attention_probs right after the forward; they are not differentiable."""
 
     @staticmethod
     def _shape(x, meta):
@@ -384,14 +402,22 @@ class _EncoderFn(torch.autograd.Function):
             else:
                 _lib.check(_lib.lib().vb_encoder_fwd_varlen(plan.descs, L, vl["cu_seqlens"].data_ptr(), M, x.data_ptr(),
                                                             arena.data_ptr(), _stream()), "vb_encoder_fwd_varlen")
+            maps = ()
+            if meta.get("attn_maps"):
+                if vl is not None:
+                    raise ValueError("bert_encoder: attention maps need a dense (padded) call")
+                probs = torch.empty(L, B, A, S, S, device=x.device, dtype=torch.float32)
+                _lib.check(_lib.lib().vb_encoder_attention_probs(plan.descs, L, arena.data_ptr(), probs.data_ptr(), _stream()),
+                           "vb_encoder_attention_probs")
+                maps = tuple(probs.unbind(0))
         n = M * H * 2
         outs = tuple(arena[l * stride + off[13]: l * stride + off[13] + n].view(_BF16).view(oshape) for l in range(L))
         ctx.meta, ctx.arena, ctx.params, ctx.weights = meta, arena, params, weights
         ctx.shape = (B, S, H, A, I, L, M, oshape)
         ctx.save_for_backward(x, mbias)
-        ctx.mark_non_differentiable(*outs[:-1])
+        ctx.mark_non_differentiable(*outs[:-1], *maps)
         ctx.set_materialize_grads(False)   # or autograd hands backward a 64 MB zero tensor for each of the L - 1 unused outputs
-        return outs
+        return outs + maps
 
     @staticmethod
     def backward(ctx, *douts):
@@ -400,9 +426,9 @@ class _EncoderFn(torch.autograd.Function):
         B, S, H, A, I, L, M, oshape = ctx.shape
         vl = meta.get("varlen")
         dev = x.device
-        if douts[-1] is None:   # nothing downstream depends on the encoder output
+        if douts[L - 1] is None:   # nothing downstream depends on the encoder output
             return (None,) * (3 + 16 * L)
-        dy = douts[-1].to(_BF16).contiguous()
+        dy = douts[L - 1].to(_BF16).contiguous()
         groups = []
         for l in range(L):
             qw, qb, kw, kb, vw, vb = params[16 * l: 16 * l + 6]
@@ -461,9 +487,9 @@ class _EncoderFn(torch.autograd.Function):
 
 def bert_encoder(x, mbias, meta, params):
     """All layers at once. meta: dict(heads, layer_index0, hidden_dropout, attn_dropout, seed, train, caches=[LayerWeights],
-    plan=EncoderPlan, optional varlen=unpad_plan(...)); params: 16 tensors per layer in bert_layer order. Returns the tuple of
-    all layer outputs (only the last one is differentiable: a caller that needs gradients through intermediate outputs uses
-    bert_layer)."""
+    plan=EncoderPlan, optional varlen=unpad_plan(...), optional attn_maps=True); params: 16 tensors per layer in bert_layer
+    order. Returns the tuple of all layer outputs (only the last one is differentiable: a caller that needs gradients through
+    intermediate outputs uses bert_layer), followed, with attn_maps, by the L detached fp32 [B, A, S, S] attention maps."""
     return _EncoderFn.apply(x, mbias, meta, *params)
 
 
@@ -484,7 +510,8 @@ def unpad_plan(valid):
 
 def bert_layer(x, mbias, meta, params):
     """params: the 16 tensors of one BertLayer in reference order (q.w, q.b, k.w, k.b, v.w, v.b, attention.output
-    dense.w/.b, LayerNorm.w/.b, intermediate.dense.w/.b, output.dense.w/.b, LayerNorm.w/.b)."""
+    dense.w/.b, LayerNorm.w/.b, intermediate.dense.w/.b, output.dense.w/.b, LayerNorm.w/.b). With meta["attn_maps"]
+    returns (output, detached fp32 [B, A, S, S] attention maps)."""
     return _LayerFn.apply(x, mbias, meta, *params)
 
 
