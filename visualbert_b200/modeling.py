@@ -147,8 +147,21 @@ class BertOutput(nn.Module):
         self.LayerNorm = BertLayerNorm(config.hidden_size, eps=1e-12)
 
 
+def _encoder_meta(owner, layers, seed, **more):
+    """meta of one ops.bert_encoder / ops.bert_layer call over `layers`, for the module that makes the call. Each such
+    module keeps its own ops.EncoderPlan: a plan shared between callers would be rebuilt at every call."""
+    l0, train = layers[0], owner.training
+    plan = owner.__dict__.get("_plan")
+    if plan is None:
+        plan = owner.__dict__["_plan"] = ops.EncoderPlan()
+    return dict(heads=l0.attention.self.num_attention_heads, layer_index0=l0.layer_index,
+                hidden_dropout=l0.hidden_dropout_prob if train else 0.0,
+                attn_dropout=l0.attention_probs_dropout_prob if train else 0.0, seed=int(seed), train=train,
+                caches=[l._weights for l in layers], plan=plan, **more)
+
+
 class BertLayer(nn.Module):
-    """One transformer block (M.py:322-341) = one vb_layer_fwd / vb_layer_bwd call."""
+    """One transformer block (M.py:322-341) = a one-layer vb_encoder_fwd / vb_encoder_bwd call."""
 
     def __init__(self, config, layer_index=0):
         super().__init__()
@@ -167,6 +180,12 @@ class BertLayer(nn.Module):
                 a.output.LayerNorm.weight, a.output.LayerNorm.bias, self.intermediate.dense.weight,
                 self.intermediate.dense.bias, o.dense.weight, o.dense.bias, o.LayerNorm.weight, o.LayerNorm.bias)
 
+    def _masters(self):
+        """The fp32 parameters that have a compute copy, in the order of ops.LayerWeights.items."""
+        a = self.attention
+        return [a.self.query.weight, a.self.key.weight, a.self.value.weight, a.output.dense.weight, self.intermediate.dense.weight,
+                self.output.dense.weight, a.self.query.bias, a.self.key.bias, a.self.value.bias]
+
     def _vb_adjacent_param_groups(self):
         a = self.attention.self
         return ((a.query.weight, a.key.weight, a.value.weight), (a.query.bias, a.key.bias, a.value.bias))
@@ -175,14 +194,10 @@ class BertLayer(nn.Module):
         """hidden_states [B, S, H]; attention_mask: the fp32 additive key bias [B, S]
         ((1 - mask) * -10000), or the reference's extended mask [B, 1, 1, S]. With output_attention_probs returns
         (output, maps): maps = softmax(QK^T/sqrt(d) + mask) [B, A, S, S] in fp32 (M.py:241-247, 258-259), pre-dropout and
-        detached, computed by vb_attention_probs from the same bf16 Q and K the layer's attention used."""
+        detached, computed by vb_encoder_attention_probs from the same bf16 Q and K the layer's attention used."""
         if attention_mask.dim() == 4:
             attention_mask = attention_mask[:, 0, 0, :]
-        train = self.training
-        meta = dict(heads=self.attention.self.num_attention_heads, layer_index=self.layer_index,
-                    hidden_dropout=self.hidden_dropout_prob if train else 0.0,
-                    attn_dropout=self.attention_probs_dropout_prob if train else 0.0,
-                    seed=int(seed), cache=self._weights, train=train, attn_maps=bool(output_attention_probs))
+        meta = _encoder_meta(self, [self], seed, attn_maps=bool(output_attention_probs))
         return ops.bert_layer(hidden_states.to(torch.bfloat16), attention_mask.float().contiguous(), meta, self._params())
 
 
@@ -207,7 +222,8 @@ class BertEncoder(nn.Module):
                                  "padded per-layer path")
             if len(self.layer) == 0:
                 return [hidden_states]
-            ys = ops.bert_encoder(hidden_states.to(torch.bfloat16), None, self._fused_meta(seed, varlen), self._fused_params())
+            meta = _encoder_meta(self, self.layer, seed, varlen=varlen)
+            ys = ops.bert_encoder(hidden_states.to(torch.bfloat16), None, meta, self._fused_params())
             return list(ys) if output_all_encoded_layers else [ys[-1]]
         if attention_mask.dim() == 4:
             attention_mask = attention_mask[:, 0, 0, :]
@@ -216,8 +232,7 @@ class BertEncoder(nn.Module):
         if fused:
             # one C call for the whole stack (vb_encoder_fwd / vb_encoder_bwd, one activation arena), and with maps one
             # vb_encoder_attention_probs call over the same arena
-            meta = self._fused_meta(seed)
-            meta["attn_maps"] = want_maps
+            meta = _encoder_meta(self, self.layer, seed, attn_maps=want_maps)
             ys = ops.bert_encoder(hidden_states.to(torch.bfloat16), attention_mask.float().contiguous(), meta, self._fused_params())
             L = len(self.layer)
             outs = list(ys[:L]) if output_all_encoded_layers else [ys[L - 1]]
@@ -234,20 +249,6 @@ class BertEncoder(nn.Module):
         if not output_all_encoded_layers:
             outs.append(hidden_states)
         return (outs, attn) if want_maps else outs
-
-    def _fused_meta(self, seed, varlen=None):
-        l0 = self.layer[0]
-        train = self.training
-        plan = self.__dict__.get("_plan")
-        if plan is None:
-            plan = self.__dict__["_plan"] = ops.EncoderPlan()
-        meta = dict(heads=l0.attention.self.num_attention_heads, layer_index0=l0.layer_index,
-                    hidden_dropout=l0.hidden_dropout_prob if train else 0.0,
-                    attn_dropout=l0.attention_probs_dropout_prob if train else 0.0, seed=int(seed), train=train,
-                    caches=[l._weights for l in self.layer], plan=plan)
-        if varlen is not None:
-            meta["varlen"] = varlen
-        return meta
 
     def _fused_params(self):
         return [p for l in self.layer for p in l._params()]
@@ -479,54 +480,32 @@ class BertVisualModel(PreTrainedBertModel):
         # the data-parallel rank is mixed in per forward (next_seed) so replicas draw different masks
         self.dropout_seed = (0x5EED ^ torch.initial_seed()) & 0xFFFFFFFF
 
-    def _bank_sources(self):
+    def _bank_holders(self):
+        """(ops weight holder, its fp32 masters) of everything the model's bank serves."""
         layers = list(self.encoder.layer) + ([self.additional_layer] if self.bypass_transformer else [])
-        srcs = []
-        for l in layers:
-            a = l.attention
-            srcs += [a.self.query.weight, a.self.key.weight, a.self.value.weight, a.output.dense.weight, l.intermediate.dense.weight,
-                     l.output.dense.weight, a.self.query.bias, a.self.key.bias, a.self.value.bias]
-        srcs.append(self.embeddings.projection.weight)
+        holders = [(l._weights, l._masters()) for l in layers]
+        holders.append((self.embeddings._weights, [self.embeddings.projection.weight]))
         extra = self.__dict__.get("_bank_extra")
         if extra is not None:
-            srcs += list(extra[0])
-        return layers, srcs
+            holders.append(extra)
+        return holders
 
     def refresh_compute_weights(self):
         """bf16 compute copies of all matrices of the encoder path <- fp32 masters, ONE launch (ops.WeightBank). Always
         in training mode (any optimizer, including the reference BertAdam's `p.data` updates, is picked up), on a
         version change in eval mode. Called by forward(); public so callers that edit weights mid-eval can force it."""
-        layers, srcs = self._bank_sources()
+        holders = self._bank_holders()
+        srcs = [p for _, masters in holders for p in masters]
         if not srcs[0].is_cuda:
             return
         bank = self.__dict__.get("_bank")
         if bank is None or not bank.bound_to(srcs):
-            bf16, dev = torch.bfloat16, srcs[0].device
-            bank = ops.WeightBank()
-            items, keep = [], []
-            for l in layers:
-                a = l.attention
-                H, I = a.output.dense.weight.shape[0], l.intermediate.dense.weight.shape[0]
-                wqkv = torch.empty(3 * H, H, device=dev, dtype=bf16)
-                wo = torch.empty(H, H, device=dev, dtype=bf16)
-                wi = torch.empty(I, H, device=dev, dtype=bf16)
-                wout = torch.empty(H, I, device=dev, dtype=bf16)
-                bqkv = torch.empty(3 * H, device=dev, dtype=torch.float32)
-                items += [(a.self.query.weight, wqkv[0:H], False), (a.self.key.weight, wqkv[H:2 * H], False),
-                          (a.self.value.weight, wqkv[2 * H:], False), (a.output.dense.weight, wo, False),
-                          (l.intermediate.dense.weight, wi, False), (l.output.dense.weight, wout, False),
-                          (a.self.query.bias, bqkv[0:H], True), (a.self.key.bias, bqkv[H:2 * H], True),
-                          (a.self.value.bias, bqkv[2 * H:], True)]
-                l._weights.buf, l._weights.bank = (wqkv, wo, wi, wout, bqkv), bank
-            pw = self.embeddings.projection.weight
-            pbuf = torch.empty(pw.shape, device=dev, dtype=bf16)
-            items.append((pw, pbuf, False))
-            self.embeddings._weights.buf, self.embeddings._weights.bank = pbuf, bank
-            extra = self.__dict__.get("_bank_extra")
-            if extra is not None:
-                items += extra[1](bank)
-            bank.bind(items, keep)
-            self.__dict__["_bank"] = bank
+            bank = self.__dict__["_bank"] = ops.WeightBank()
+            items = []
+            for holder, masters in holders:
+                items += holder.items(*masters)
+                holder.owner = bank
+            bank.bind(items)
         bank.refresh(force=self.training)
 
     def set_unpadded(self, flag=True):
@@ -767,16 +746,7 @@ class TrainVisualBERTObjective(PreTrainedBertModel):
         if self.training_head_type != "pretraining" or not hasattr(self, "cls"):
             return
         head = self.cls.predictions
-        E, b = head.decoder.weight, head.bias
-
-        def items(bank):
-            dw = self._decoder_cache()
-            table, bias_p = dw.alloc(E)
-            dw.bank = bank
-            V = E.shape[0]
-            return [(E, table[:V], False), (b, bias_p[:V], True)]
-
-        self.bert.__dict__["_bank_extra"] = ((E, b), items)
+        self.bert.__dict__["_bank_extra"] = (self._decoder_cache(), [head.decoder.weight, head.bias])
 
     def _masked_lm_loss(self, sequence_output, flat_labels, rows=None):
         """CrossEntropyLoss(ignore_index=-1) of the MLM head (M.py:1471-1473) evaluated on the labelled rows only:

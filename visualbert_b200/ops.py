@@ -5,7 +5,7 @@ encoder path runs in the sm_90a kernels. There is no fallback: on a machine with
 without a CUDA device these ops raise.
 
 Activations are bf16; parameters are the model's fp32 master weights, cast to bf16 "compute weights"
-by vb_cast_f32_to_bf16 (cached per parameter version). Parameter gradients come back in fp32.
+in a WeightBank by one vb_cast_multi launch per refresh. Parameter gradients come back in fp32.
 """
 import ctypes
 
@@ -33,51 +33,30 @@ def _require_cuda(t, what):
 # --------------------------------------------------------------------------------------------
 # workspaces: backward scratch is shared by all layers of a step (same stream, sequential use)
 # --------------------------------------------------------------------------------------------
-_scratch_cache = {}
+_bwd_scratch_cache = {}
 
 
-def _scratch(dev, M, H, I, B, A, S, need_drop):
-    key = (dev, M, H, I, B, A, S)
-    w = _scratch_cache.get(key)
-    if w is None:
-        w = dict(
-            d_pre=torch.empty(M, H, device=dev, dtype=_BF16),
-            d_pre_drop=None,
-            d_big=torch.empty(M, max(I, 3 * H), device=dev, dtype=_BF16),
-            d_x1=torch.empty(M, H, device=dev, dtype=_BF16),
-            d_ctx=torch.empty(M, H, device=dev, dtype=_BF16),
-            drow=torch.empty(B, A, S, device=dev, dtype=torch.float32))
-        for k in [k for k in _scratch_cache if k[0] == dev]:   # keep a single shape resident PER DEVICE
-            del _scratch_cache[k]
-        _scratch_cache[key] = w
-    if need_drop and w["d_pre_drop"] is None:
-        w["d_pre_drop"] = torch.empty(M, H, device=dev, dtype=_BF16)
-    return w
-
-
-_varlen_scratch_cache = {}
-
-
-def _varlen_scratch(dev, M, H, I, A, need_drop):
-    """Backward scratch of an unpadded encoder call: views of the first M = total rows of buffers that are kept per device and
-    only grow (by at least 1/4, in whole 256-row steps) when a batch has more packed rows than any before. The row count of
-    unpadded batches changes from step to step; a cache keyed on it would reallocate every backward."""
+def _bwd_scratch(dev, M, H, I, A, need_drop):
+    """Backward scratch of an encoder call over M rows (B * S dense, the packed total unpadded): views of the first M rows of
+    buffers that are kept per device and only grow (by at least 1/4, in whole 256-row steps) when a call has more rows than
+    any before. The row count of unpadded batches changes from step to step; a cache keyed on it would reallocate every
+    backward."""
     key = (dev, H, I, A)
-    c = _varlen_scratch_cache.get(key)
+    c = _bwd_scratch_cache.get(key)
     if c is None or c["rows"] < M:
         rows = M if c is None else max(M, c["rows"] + c["rows"] // 4)
         rows = (rows + 255) // 256 * 256
-        for k in [k for k in _varlen_scratch_cache if k[0] == dev]:   # free the smaller buffers before allocating
-            del _varlen_scratch_cache[k]
+        for k in [k for k in _bwd_scratch_cache if k[0] == dev]:   # free the smaller buffers before allocating
+            del _bwd_scratch_cache[k]
         c = dict(rows=rows, d_pre=torch.empty(rows, H, device=dev, dtype=_BF16), d_pre_drop=None,
                  d_big=torch.empty(rows, max(I, 3 * H), device=dev, dtype=_BF16),
                  d_x1=torch.empty(rows, H, device=dev, dtype=_BF16), d_ctx=torch.empty(rows, H, device=dev, dtype=_BF16),
                  drow=torch.empty(A * rows, device=dev, dtype=torch.float32))
-        _varlen_scratch_cache[key] = c
+        _bwd_scratch_cache[key] = c
     if need_drop and c["d_pre_drop"] is None:
         c["d_pre_drop"] = torch.empty(c["rows"], H, device=dev, dtype=_BF16)
     w = {k: (c[k][:M] if c[k] is not None else None) for k in ("d_pre", "d_pre_drop", "d_big", "d_x1", "d_ctx")}
-    w["drow"] = c["drow"][:A * M]   # [heads, total]
+    w["drow"] = c["drow"][:A * M]   # [B, A, S] dense, [heads, total] unpadded
     return w
 
 
@@ -143,17 +122,15 @@ class WeightBank:
         self.items = []       # (src parameter, dst tensor, dst_is_fp32)
         self.table = None
         self.n_chunks = 0
-        self.keep = []        # owners of the dst storage
         self.generation = 0
 
     def _signature(self, params):
         return tuple((p.data_ptr(), p._version) for p in params)
 
-    def bind(self, items, keep):
+    def bind(self, items):
         """items: list of (src fp32 parameter, dst tensor [contiguous view], dst_is_fp32)."""
         import numpy as np
         self.items = items
-        self.keep = keep
         arr = (_lib.CastItem * len(items))()
         chunk = 0
         for i, (src, dst, f32) in enumerate(items):
@@ -182,38 +159,59 @@ class WeightBank:
         self.generation += 1
 
 
-class LayerWeights:
-    """bf16 compute copies of one BertLayer's matrices. Normally views into the model's WeightBank (refreshed once per
-    forward by the model); a stand-alone BertLayer refreshes them itself — on every training-mode forward, or when the
-    masters' (data_ptr, _version) signature changes in eval mode."""
+class _BankViews:
+    """The compute weights of one module: views into a WeightBank. A model that owns the module lists `items()` in its own
+    bank, sets `owner` and refreshes that bank once per forward. A module used on its own gets a private bank over its own
+    masters at its first CUDA forward (again when the masters moved), refreshed on every get() by WeightBank.refresh's rule."""
 
     def __init__(self):
-        self.key = None
         self.buf = None
-        self.bank = None      # set by the owning model: buffers are bank views, refresh is the bank's job
+        self.owner = None     # the owning model's bank: refreshing is the model's job
+        self.bank = None      # the private bank of a module without an owner
 
-    def get(self, q, k, v, o, w1, w2, bq, bk, bv, train=False):
-        if self.bank is not None:
-            return self.buf
-        key = tuple((p.data_ptr(), p._version) for p in (q, k, v, o, w1, w2, bq, bk, bv))
-        if train or key != self.key:
-            H, I = o.shape[0], w1.shape[0]
-            dev = q.device
-            if self.buf is None or self.buf[0].device != dev:
-                self.buf = (torch.empty(3 * H, H, device=dev, dtype=_BF16), torch.empty(H, H, device=dev, dtype=_BF16),
-                            torch.empty(I, H, device=dev, dtype=_BF16), torch.empty(H, I, device=dev, dtype=_BF16),
-                            torch.empty(3 * H, device=dev, dtype=torch.float32))
-            wqkv, wo, wi, wout, bqkv = self.buf
-            with torch.no_grad():
-                cast_to_bf16(q.detach(), wqkv[0:H])
-                cast_to_bf16(k.detach(), wqkv[H:2 * H])
-                cast_to_bf16(v.detach(), wqkv[2 * H:3 * H])
-                cast_to_bf16(o.detach(), wo)
-                cast_to_bf16(w1.detach(), wi)
-                cast_to_bf16(w2.detach(), wout)
-                torch.cat((bq.detach(), bk.detach(), bv.detach()), out=bqkv)
-            self.key = key
+    def get(self, *masters, train=False):
+        if self.owner is None:
+            if self.bank is None or not self.bank.bound_to(masters):
+                self.bank = WeightBank()
+                self.bank.bind(self.items(*masters))
+            self.bank.refresh(force=train)
         return self.buf
+
+
+class LayerWeights(_BankViews):
+    """One BertLayer: buf = (packed q|k|v [3H, H], attention output [H, H], intermediate [I, H], output [H, I]) in bf16 and
+    the packed fp32 q|k|v bias [3H]."""
+
+    def items(self, q, k, v, o, w1, w2, bq, bk, bv):
+        H, I, dev = o.shape[0], w1.shape[0], q.device
+        wqkv = torch.empty(3 * H, H, device=dev, dtype=_BF16)
+        bqkv = torch.empty(3 * H, device=dev, dtype=torch.float32)
+        self.buf = (wqkv, torch.empty(H, H, device=dev, dtype=_BF16), torch.empty(I, H, device=dev, dtype=_BF16),
+                    torch.empty(H, I, device=dev, dtype=_BF16), bqkv)
+        return [(q, wqkv[0:H], False), (k, wqkv[H:2 * H], False), (v, wqkv[2 * H:], False), (o, self.buf[1], False),
+                (w1, self.buf[2], False), (w2, self.buf[3], False),
+                (bq, bqkv[0:H], True), (bk, bqkv[H:2 * H], True), (bv, bqkv[2 * H:], True)]
+
+
+class ProjectionWeights(_BankViews):
+    """The visual projection matrix of the embeddings: buf = its bf16 copy."""
+
+    def items(self, w):
+        self.buf = torch.empty(w.shape, device=w.device, dtype=_BF16)
+        return [(w, self.buf, False)]
+
+
+class DecoderWeights(_BankViews):
+    """The tied MLM decoder: buf = (bf16 copy of the word-embedding matrix with its rows padded to a multiple of 16, fp32
+    bias padded likewise). The padding rows are zero (the GEMMs address all of them) and their bias is -30000, so the
+    padding columns of the logits vanish in the softmax."""
+
+    def items(self, E, bias):
+        V = E.shape[0]
+        Vp = (V + 15) // 16 * 16
+        self.buf = (torch.zeros(Vp, E.shape[1], device=E.device, dtype=_BF16),
+                    torch.full((Vp,), -30000.0, device=E.device, dtype=torch.float32))
+        return [(E, self.buf[0][:V], False), (bias, self.buf[1][:V], True)]
 
 
 def attention_probs(qkv, mbias, B, S, A):
@@ -226,115 +224,72 @@ def attention_probs(qkv, mbias, B, S, A):
     return probs
 
 
-class _LayerFn(torch.autograd.Function):
-    """BertLayer forward/backward (reference M.py:322-341) through vb_layer_fwd / vb_layer_bwd. With meta["attn_maps"] the
-    forward also returns the layer's attention maps (attention_probs of its qkv), a non-differentiable second output."""
+_GRAD_FIELDS = ("dw_qkv", "db_qkv", "dw_attn_out", "db_attn_out", "dln1_gamma", "dln1_beta",
+                "dw_inter", "db_inter", "dw_out", "db_out", "dln2_gamma", "dln2_beta")   # vb_layer_grads
 
-    @staticmethod
-    def forward(ctx, x, mbias, meta, qw, qb, kw, kb, vw, vb, ow, ob, g1, b1, iw, ib, dw, db, g2, b2):
-        # meta: dict(heads, layer_index, hidden_dropout, attn_dropout, seed, cache=LayerWeights, optional attn_maps)
-        _require_cuda(x, "bert_layer")
-        B, S, H = x.shape
-        I = iw.shape[0]
-        M = B * S
-        A = meta["heads"]
-        dev = x.device
-        x = x.contiguous()
-        wqkv, wo, wi, wout, bqkv = meta["cache"].get(qw, kw, vw, ow, iw, dw, qb, kb, vb, train=meta.get("train", False))
-        f32 = torch.float32
-        acts = dict(
-            qkv=torch.empty(M, 3 * H, device=dev, dtype=_BF16), ctx=torch.empty(M, H, device=dev, dtype=_BF16),
-            lse=torch.empty(B, A, S, device=dev, dtype=f32), pre1=torch.empty(M, H, device=dev, dtype=_BF16),
-            mean1=torch.empty(M, device=dev, dtype=f32), rstd1=torch.empty(M, device=dev, dtype=f32),
-            x1=torch.empty(M, H, device=dev, dtype=_BF16), u=torch.empty(M, I, device=dev, dtype=_BF16),
-            g=torch.empty(M, I, device=dev, dtype=_BF16), pre2=torch.empty(M, H, device=dev, dtype=_BF16),
-            mean2=torch.empty(M, device=dev, dtype=f32), rstd2=torch.empty(M, device=dev, dtype=f32),
-            keep_mask=(torch.empty(int(_lib.lib().vb_attention_keep_bytes(B, S, A)), device=dev, dtype=torch.uint8)
-                       if meta["attn_dropout"] > 0 else None))
-        y = torch.empty(B, S, H, device=dev, dtype=_BF16)
-        d = _lib.LayerDesc(
-            batch=B, seq=S, hidden=H, heads=A, inter=I, hidden_dropout=meta["hidden_dropout"],
-            attn_dropout=meta["attn_dropout"], seed=meta["seed"], layer_index=meta["layer_index"],
-            w_qkv=wqkv.data_ptr(), w_attn_out=wo.data_ptr(), w_inter=wi.data_ptr(), w_out=wout.data_ptr(),
-            b_qkv=bqkv.data_ptr(), b_attn_out=ob.data_ptr(), ln1_gamma=g1.data_ptr(), ln1_beta=b1.data_ptr(),
-            b_inter=ib.data_ptr(), b_out=db.data_ptr(), ln2_gamma=g2.data_ptr(), ln2_beta=b2.data_ptr(),
-            mask_bias=mbias.data_ptr())
-        a = _lib.LayerActs(**{k: _ptr(t) for k, t in acts.items()})
-        with torch.cuda.device(dev):
-            _lib.check(_lib.lib().vb_layer_fwd(ctypes.byref(d), ctypes.c_void_p(x.data_ptr()), ctypes.c_void_p(y.data_ptr()),
-                                               ctypes.byref(a), _stream()), "vb_layer_fwd")
-        ctx.meta = meta
-        ctx.acts = acts
-        ctx.params = (qw, qb, kw, kb, vw, vb, ow, ob, g1, b1, iw, ib, dw, db, g2, b2)
-        ctx.weights = (wqkv, wo, wi, wout, bqkv)
-        ctx.weight_key = meta["cache"].key if meta["cache"].bank is None else None
-        ctx.save_for_backward(x, mbias, ob, g1, b1, ib, db, g2, b2)
-        if meta.get("attn_maps"):
-            maps = attention_probs(acts["qkv"], mbias, B, S, A)
-            ctx.mark_non_differentiable(maps)
-            return y, maps
-        return y
 
-    @staticmethod
-    def backward(ctx, dy, *_maps_grad):
-        x, mbias, ob, g1, b1, ib, db, g2, b2 = ctx.saved_tensors
-        meta, acts = ctx.meta, ctx.acts
-        if ctx.weight_key is not None and meta["cache"].key != ctx.weight_key:
-            raise RuntimeError("visualbert_b200: layer weights were modified between forward and backward")
-        wqkv, wo, wi, wout, bqkv = ctx.weights
-        B, S, H = x.shape
-        I = wi.shape[0]
-        M, A = B * S, meta["heads"]
-        dev = x.device
-        dy = dy.to(_BF16).contiguous()
-        qw, qb, kw, kb, vw, vb, ow, ob_, g1_, b1_, iw, ib_, dw, db_, g2_, b2_ = ctx.params
-        direct = _grad_targets(ctx.params, ((qw, kw, vw), (qb, kb, vb)))
-        gnames = ("dw_qkv", "db_qkv", "dw_attn_out", "db_attn_out", "dln1_gamma", "dln1_beta",
-                  "dw_inter", "db_inter", "dw_out", "db_out", "dln2_gamma", "dln2_beta")
-        if direct is not None:
-            tg = dict(zip(("qw", "qb", "kw", "kb", "vw", "vb", "ow", "ob", "g1", "b1", "iw", "ib", "dw", "db", "g2", "b2"), direct))
-            parts = [tg["qw"], tg["qb"], tg["ow"], tg["ob"], tg["g1"], tg["b1"], tg["iw"], tg["ib"], tg["dw"], tg["db"], tg["g2"], tg["b2"]]
-        else:
-            sizes = [3 * H * H, 3 * H, H * H, H, H, H, I * H, I, H * I, H, H, H]
-            flat = torch.zeros(sum(sizes), device=dev, dtype=torch.float32)
-            parts = list(torch.split(flat, sizes))
-        g = _lib.LayerGrads(**{n: t.data_ptr() for n, t in zip(gnames, parts)})
-        hd = meta["hidden_dropout"] > 0
-        w = _scratch(dev, M, H, I, B, A, S, hd)
-        sc = _lib.LayerScratch(**{k: _ptr(t) for k, t in w.items()})
-        d = _lib.LayerDesc(
-            batch=B, seq=S, hidden=H, heads=A, inter=I, hidden_dropout=meta["hidden_dropout"],
-            attn_dropout=meta["attn_dropout"], seed=meta["seed"], layer_index=meta["layer_index"],
-            w_qkv=wqkv.data_ptr(), w_attn_out=wo.data_ptr(), w_inter=wi.data_ptr(), w_out=wout.data_ptr(),
-            b_qkv=bqkv.data_ptr(), b_attn_out=ob.data_ptr(), ln1_gamma=g1.data_ptr(), ln1_beta=b1.data_ptr(),
-            b_inter=ib.data_ptr(), b_out=db.data_ptr(), ln2_gamma=g2.data_ptr(), ln2_beta=b2.data_ptr(),
-            mask_bias=mbias.data_ptr())
-        a = _lib.LayerActs(**{k: _ptr(t) for k, t in acts.items()})
-        dx = torch.empty(B, S, H, device=dev, dtype=_BF16)
-        with torch.cuda.device(dev):
-            _lib.check(_lib.lib().vb_layer_bwd(ctypes.byref(d), ctypes.c_void_p(x.data_ptr()), ctypes.byref(a),
-                                               ctypes.c_void_p(dy.data_ptr()), ctypes.c_void_p(dx.data_ptr()),
-                                               ctypes.byref(g), ctypes.byref(sc), _stream()), "vb_layer_bwd")
-        ctx.acts = None
-        if direct is not None:
-            return (dx, None, None) + (None,) * 16
-        dwqkv, dbqkv, dwo, dbo, dg1, db1, dwi, dbi, dwout, dbout, dg2, db2 = parts
+def _grad_sizes(H, I):
+    return [3 * H * H, 3 * H, H * H, H, H, H, I * H, I, H * I, H, H, H]
+
+
+def _layer_grads(params, L, H, I, dev):
+    """The vb_layer_grads array of an L-layer backward and the buffer behind it: None when every pointer is a parameter's own
+    `.grad` (_grad_targets; q|k|v are one packed output, so each layer's q, k, v weights and biases must be adjacent), else
+    one zeroed flat fp32 buffer that _autograd_grads cuts up."""
+    groups = []
+    for l in range(L):
+        qw, qb, kw, kb, vw, vb = params[16 * l: 16 * l + 6]
+        groups += [(qw, kw, vw), (qb, kb, vb)]
+    direct = _grad_targets(params, groups)
+    grads = (_lib.LayerGrads * L)()
+    if direct is not None:
+        for l in range(L):
+            t = direct[16 * l: 16 * l + 16]
+            for name, g in zip(_GRAD_FIELDS, (t[0], t[1]) + tuple(t[6:16])):
+                setattr(grads[l], name, g.data_ptr())
+        return grads, None
+    sizes = _grad_sizes(H, I)
+    flat = torch.zeros(L * sum(sizes), device=dev, dtype=torch.float32)
+    o = flat.data_ptr()
+    for l in range(L):
+        for name, sz in zip(_GRAD_FIELDS, sizes):
+            setattr(grads[l], name, o)
+            o += 4 * sz
+    return grads, flat
+
+
+def _autograd_grads(flat, L, H, I):
+    """The 16 parameter gradients per layer, in bert_layer order, as views of _layer_grads' flat buffer."""
+    out = []
+    for part in flat.view(L, -1).unbind(0):
+        dwqkv, dbqkv, dwo, dbo, dg1, db1, dwi, dbi, dwout, dbout, dg2, db2 = torch.split(part, _grad_sizes(H, I))
         dwq, dwk, dwv = dwqkv.view(3, H, H).unbind(0)
         dbq, dbk, dbv = dbqkv.view(3, H).unbind(0)
-        return (dx, None, None, dwq, dbq, dwk, dbk, dwv, dbv, dwo.view(H, H), dbo, dg1, db1,
-                dwi.view(I, H), dbi, dwout.view(H, I), dbout, dg2, db2)
+        out += [dwq, dbq, dwk, dbk, dwv, dbv, dwo.view(H, H), dbo, dg1, db1, dwi.view(I, H), dbi, dwout.view(H, I), dbout, dg2, db2]
+    return tuple(out)
+
+
+def _stamp(descs, L, meta, mbias):
+    """The per-step fields of a descriptor array: dropout, seed (so a backward draws its forward's dropout streams), mask."""
+    for l in range(L):
+        d = descs[l]
+        d.hidden_dropout, d.attn_dropout, d.seed = meta["hidden_dropout"], meta["attn_dropout"], meta["seed"]
+        d.layer_index, d.mask_bias = meta["layer_index0"] + l, _ptr(mbias)
 
 
 class EncoderPlan:
-    """Host-side state of the whole-encoder call (vb_encoder_fwd / vb_encoder_bwd): the ctypes descriptor and gradient
-    arrays are built once per (shape, weights) and only their per-step fields (seed, dropout) are touched afterwards."""
+    """Host-side state of the encoder call (vb_encoder_fwd / vb_encoder_bwd): the ctypes descriptor array is built once per
+    (shape, weights) and only its per-step fields (_stamp) are touched afterwards."""
 
     def __init__(self):
         self.key = None
 
     def prepare(self, caches, params, B, S, H, A, I, mbias, meta, dev, varlen=None):
-        """varlen (unpadded calls): dict(cu_seqlens, max_seq, total); B is then the number of sequences, S = max_seq, and
-        mbias is None."""
+        """-> (descs, weights, arena stride per layer, buffer offsets). varlen (unpadded calls): dict(cu_seqlens, max_seq,
+        total); B is then the number of sequences, S = max_seq, and mbias is None.
+
+        A forward keeps `descs` for its backward. So a new key gets a NEW array and the old one is never rewritten: a
+        backward that runs after a forward of another shape or other weights still describes its own forward's arena."""
         L = len(caches)
         weights = [c.get(*[params[16 * l + i] for i in (0, 2, 4, 6, 10, 12, 1, 3, 5)], train=meta["train"]) for l, c in enumerate(caches)]
         key = (B, S, H, A, I, L, tuple(w[0].data_ptr() for w in weights), tuple(p.data_ptr() for p in params), dev)
@@ -349,11 +304,7 @@ class EncoderPlan:
                 d.b_qkv, d.b_attn_out, d.ln1_gamma, d.ln1_beta = bqkv.data_ptr(), ob.data_ptr(), g1.data_ptr(), b1.data_ptr()
                 d.b_inter, d.b_out, d.ln2_gamma, d.ln2_beta = ib.data_ptr(), db.data_ptr(), g2.data_ptr(), b2.data_ptr()
             self.key = key
-        for l in range(L):
-            d = self.descs[l]
-            d.hidden_dropout, d.attn_dropout, d.seed = meta["hidden_dropout"], meta["attn_dropout"], meta["seed"]
-            d.layer_index = meta["layer_index0"] + l
-            d.mask_bias = _ptr(mbias)
+        _stamp(self.descs, L, meta, mbias)
         off = (ctypes.c_int64 * _lib.VB_ENCODER_ARENA_BUFFERS)()
         drop = 1 if meta["attn_dropout"] > 0 else 0
         if varlen is None:
@@ -362,7 +313,7 @@ class EncoderPlan:
             stride = int(_lib.lib().vb_encoder_arena_layout_varlen(B, S, varlen["total"], H, A, I, drop, off))
             if stride < 0:
                 _lib.check(1, "vb_encoder_arena_layout_varlen")
-        return weights, stride, list(off)
+        return self.descs, weights, stride, list(off)
 
 
 class _EncoderFn(torch.autograd.Function):
@@ -393,26 +344,25 @@ class _EncoderFn(torch.autograd.Function):
         A = meta["heads"]
         x = x.contiguous()
         with torch.cuda.device(x.device):
-            weights, stride, off = meta["plan"].prepare(meta["caches"], params, B, S, H, A, I, mbias, meta, x.device, vl)
+            descs, weights, stride, off = meta["plan"].prepare(meta["caches"], params, B, S, H, A, I, mbias, meta, x.device, vl)
             arena = torch.empty(L * stride, device=x.device, dtype=torch.uint8)
-            plan = meta["plan"]
             if vl is None:
-                _lib.check(_lib.lib().vb_encoder_fwd(plan.descs, L, ctypes.c_void_p(x.data_ptr()), ctypes.c_void_p(arena.data_ptr()),
+                _lib.check(_lib.lib().vb_encoder_fwd(descs, L, ctypes.c_void_p(x.data_ptr()), ctypes.c_void_p(arena.data_ptr()),
                                                      _stream()), "vb_encoder_fwd")
             else:
-                _lib.check(_lib.lib().vb_encoder_fwd_varlen(plan.descs, L, vl["cu_seqlens"].data_ptr(), M, x.data_ptr(),
+                _lib.check(_lib.lib().vb_encoder_fwd_varlen(descs, L, vl["cu_seqlens"].data_ptr(), M, x.data_ptr(),
                                                             arena.data_ptr(), _stream()), "vb_encoder_fwd_varlen")
             maps = ()
             if meta.get("attn_maps"):
                 if vl is not None:
                     raise ValueError("bert_encoder: attention maps need a dense (padded) call")
                 probs = torch.empty(L, B, A, S, S, device=x.device, dtype=torch.float32)
-                _lib.check(_lib.lib().vb_encoder_attention_probs(plan.descs, L, arena.data_ptr(), probs.data_ptr(), _stream()),
+                _lib.check(_lib.lib().vb_encoder_attention_probs(descs, L, arena.data_ptr(), probs.data_ptr(), _stream()),
                            "vb_encoder_attention_probs")
                 maps = tuple(probs.unbind(0))
         n = M * H * 2
         outs = tuple(arena[l * stride + off[13]: l * stride + off[13] + n].view(_BF16).view(oshape) for l in range(L))
-        ctx.meta, ctx.arena, ctx.params, ctx.weights = meta, arena, params, weights
+        ctx.meta, ctx.descs, ctx.arena, ctx.params, ctx.weights = meta, descs, arena, params, weights
         ctx.shape = (B, S, H, A, I, L, M, oshape)
         ctx.save_for_backward(x, mbias)
         ctx.mark_non_differentiable(*outs[:-1], *maps)
@@ -422,74 +372,39 @@ class _EncoderFn(torch.autograd.Function):
     @staticmethod
     def backward(ctx, *douts):
         x, mbias = ctx.saved_tensors
-        meta, params = ctx.meta, ctx.params
+        meta, descs = ctx.meta, ctx.descs
         B, S, H, A, I, L, M, oshape = ctx.shape
         vl = meta.get("varlen")
         dev = x.device
         if douts[L - 1] is None:   # nothing downstream depends on the encoder output
             return (None,) * (3 + 16 * L)
         dy = douts[L - 1].to(_BF16).contiguous()
-        groups = []
-        for l in range(L):
-            qw, qb, kw, kb, vw, vb = params[16 * l: 16 * l + 6]
-            groups += [(qw, kw, vw), (qb, kb, vb)]
-        direct = _grad_targets(params, groups)
-        sizes = [3 * H * H, 3 * H, H * H, H, H, H, I * H, I, H * I, H, H, H]
-        grads = (_lib.LayerGrads * L)()
-        gnames = ("dw_qkv", "db_qkv", "dw_attn_out", "db_attn_out", "dln1_gamma", "dln1_beta",
-                  "dw_inter", "db_inter", "dw_out", "db_out", "dln2_gamma", "dln2_beta")
-        if direct is not None:
-            for l in range(L):
-                t = direct[16 * l: 16 * l + 16]
-                ptrs = (t[0], t[1], t[6], t[7], t[8], t[9], t[10], t[11], t[12], t[13], t[14], t[15])
-                for nme, tt in zip(gnames, ptrs):
-                    setattr(grads[l], nme, tt.data_ptr())
-            flat = None
-        else:
-            per = sum(sizes)
-            flat = torch.zeros(L * per, device=dev, dtype=torch.float32)
-            for l in range(L):
-                o = l * per
-                for nme, sz in zip(gnames, sizes):
-                    setattr(grads[l], nme, flat.data_ptr() + 4 * o)
-                    o += sz
-        hd = meta["hidden_dropout"] > 0
+        grads, flat = _layer_grads(ctx.params, L, H, I, dev)
         with torch.cuda.device(dev):
-            # varlen: row-sized scratch for the `total` packed rows (grow-only cache), drow [heads, total]
-            w = _scratch(dev, M, H, I, B, A, S, hd) if vl is None else _varlen_scratch(dev, M, H, I, A, hd)
+            w = _bwd_scratch(dev, M, H, I, A, meta["hidden_dropout"] > 0)
             sc = _lib.LayerScratch(**{k: _ptr(t) for k, t in w.items()})
             dx = torch.empty(oshape, device=dev, dtype=_BF16)
-            plan = meta["plan"]
-            for l in range(L):  # same step, same dropout streams as the forward
-                d = plan.descs[l]
-                d.hidden_dropout, d.attn_dropout, d.seed = meta["hidden_dropout"], meta["attn_dropout"], meta["seed"]
-                d.layer_index, d.mask_bias = meta["layer_index0"] + l, _ptr(mbias)
+            _stamp(descs, L, meta, mbias)   # a later forward with the same plan key has stamped its own step since
             if vl is None:
-                _lib.check(_lib.lib().vb_encoder_bwd(plan.descs, L, ctypes.c_void_p(x.data_ptr()), ctypes.c_void_p(ctx.arena.data_ptr()),
+                _lib.check(_lib.lib().vb_encoder_bwd(descs, L, ctypes.c_void_p(x.data_ptr()), ctypes.c_void_p(ctx.arena.data_ptr()),
                                                      ctypes.c_void_p(dy.data_ptr()), ctypes.c_void_p(dx.data_ptr()), grads,
                                                      ctypes.byref(sc), _stream()), "vb_encoder_bwd")
             else:
-                _lib.check(_lib.lib().vb_encoder_bwd_varlen(plan.descs, L, vl["cu_seqlens"].data_ptr(), M, x.data_ptr(),
+                _lib.check(_lib.lib().vb_encoder_bwd_varlen(descs, L, vl["cu_seqlens"].data_ptr(), M, x.data_ptr(),
                                                             ctx.arena.data_ptr(), dy.data_ptr(), dx.data_ptr(), grads, ctypes.byref(sc),
                                                             _stream()), "vb_encoder_bwd_varlen")
         ctx.arena = None
-        if direct is not None:
+        if flat is None:
             return (dx, None, None) + (None,) * (16 * L)
-        out = []
-        per = sum(sizes)
-        for l in range(L):
-            dwqkv, dbqkv, dwo, dbo, dg1, db1, dwi, dbi, dwout, dbout, dg2, db2 = torch.split(flat[l * per: (l + 1) * per], sizes)
-            dwq, dwk, dwv = dwqkv.view(3, H, H).unbind(0)
-            dbq, dbk, dbv = dbqkv.view(3, H).unbind(0)
-            out += [dwq, dbq, dwk, dbk, dwv, dbv, dwo.view(H, H), dbo, dg1, db1, dwi.view(I, H), dbi, dwout.view(H, I), dbout, dg2, db2]
-        return (dx, None, None) + tuple(out)
+        return (dx, None, None) + _autograd_grads(flat, L, H, I)
 
 
 def bert_encoder(x, mbias, meta, params):
     """All layers at once. meta: dict(heads, layer_index0, hidden_dropout, attn_dropout, seed, train, caches=[LayerWeights],
     plan=EncoderPlan, optional varlen=unpad_plan(...), optional attn_maps=True); params: 16 tensors per layer in bert_layer
     order. Returns the tuple of all layer outputs (only the last one is differentiable: a caller that needs gradients through
-    intermediate outputs uses bert_layer), followed, with attn_maps, by the L detached fp32 [B, A, S, S] attention maps."""
+    intermediate outputs calls bert_layer once per layer), followed, with attn_maps, by the L detached fp32 [B, A, S, S]
+    attention maps."""
     return _EncoderFn.apply(x, mbias, meta, *params)
 
 
@@ -509,27 +424,13 @@ def unpad_plan(valid):
 
 
 def bert_layer(x, mbias, meta, params):
-    """params: the 16 tensors of one BertLayer in reference order (q.w, q.b, k.w, k.b, v.w, v.b, attention.output
-    dense.w/.b, LayerNorm.w/.b, intermediate.dense.w/.b, output.dense.w/.b, LayerNorm.w/.b). With meta["attn_maps"]
-    returns (output, detached fp32 [B, A, S, S] attention maps)."""
-    return _LayerFn.apply(x, mbias, meta, *params)
-
-
-class ProjectionWeights:
-    def __init__(self):
-        self.key = None
-        self.buf = None
-        self.bank = None
-
-    def get(self, w, train=False):
-        if self.bank is not None:
-            return self.buf
-        key = (w.data_ptr(), w._version)
-        if train or key != self.key:
-            with torch.no_grad():
-                self.buf = cast_to_bf16(w.detach(), self.buf if self.buf is not None and self.buf.device == w.device else None)
-            self.key = key
-        return self.buf
+    """One layer: bert_encoder over a single layer, so its output is differentiable. meta as for bert_encoder, with one
+    LayerWeights in caches, the layer's index as layer_index0 and a plan of the layer's own; params: the 16 tensors of one
+    BertLayer in reference order (q.w, q.b, k.w, k.b, v.w, v.b, attention.output dense.w/.b, LayerNorm.w/.b,
+    intermediate.dense.w/.b, output.dense.w/.b, LayerNorm.w/.b). With meta["attn_maps"] returns (output, detached fp32
+    [B, A, S, S] attention maps)."""
+    outs = _EncoderFn.apply(x, mbias, meta, *params)
+    return outs if meta.get("attn_maps") else outs[0]
 
 
 class _EmbedFn(torch.autograd.Function):
@@ -571,7 +472,7 @@ class _EmbedFn(torch.autograd.Function):
         with torch.cuda.device(dev):
             _lib.check(_lib.lib().vb_embed_fwd(ctypes.byref(d), ctypes.c_void_p(y.data_ptr()), ctypes.byref(a), _stream()),
                        "vb_embed_fwd")
-        ctx.meta = meta
+        ctx.desc = d   # the backward's too: it does not read visual_addend
         ctx.shape = (B, T, V, H, Dv)
         ctx.feats_need_grad = feats is not None and feats.requires_grad
         ctx.feats_dtype = None if feats is None else feats.dtype
@@ -585,7 +486,6 @@ class _EmbedFn(torch.autograd.Function):
     def backward(ctx, dy):
         ids, tt, vt, fb, wp, pb, word, pos, typ, typ_vis, pos_vis, gamma, beta, pre, mean, rstd = ctx.saved_tensors
         B, T, V, H, Dv = ctx.shape
-        meta = ctx.meta
         dev = word.device
         M = B * (T + V)
         dy = dy.to(_BF16).contiguous()
@@ -609,19 +509,13 @@ class _EmbedFn(torch.autograd.Function):
             d_feats = torch.empty(B * V, Dv, device=dev, dtype=_BF16) if ctx.feats_need_grad else None
         else:
             d_vis = d_feats = None
-        d = _lib.EmbedDesc(
-            batch=B, text_len=T, num_regions=V, hidden=H, visual_dim=Dv, vocab=word.shape[0], max_pos=pos.shape[0],
-            n_types=typ.shape[0], eps=1e-12, dropout=meta["dropout"], seed=meta["seed"],
-            input_ids=ids.data_ptr(), token_type_ids=tt.data_ptr(), visual_type=_ptr(vt), visual_feats=_ptr(fb),
-            w_proj=_ptr(wp), b_proj=_ptr(pb), word=word.data_ptr(), pos=pos.data_ptr(), type=typ.data_ptr(),
-            pos_vis=pos_vis.data_ptr(), type_vis=typ_vis.data_ptr(), gamma=gamma.data_ptr(), beta=beta.data_ptr())
         a = _lib.EmbedActs(vis_proj=0, pre=pre.data_ptr(), mean=mean.data_ptr(), rstd=rstd.data_ptr())
         g = _lib.EmbedGrads(
             dword=dword.data_ptr(), dpos=dpos.data_ptr(), dtype=dtyp.data_ptr(), dpos_vis=dpos_vis.data_ptr(),
             dtype_vis=dtyp_vis.data_ptr(), dw_proj=_ptr(dpw), db_proj=_ptr(dpb), dgamma=dgamma.data_ptr(),
             dbeta=dbeta.data_ptr(), d_pre=d_pre.data_ptr(), d_vis=_ptr(d_vis), d_feats=_ptr(d_feats))
         with torch.cuda.device(dev):
-            _lib.check(_lib.lib().vb_embed_bwd(ctypes.byref(d), ctypes.byref(a), ctypes.c_void_p(dy.data_ptr()),
+            _lib.check(_lib.lib().vb_embed_bwd(ctypes.byref(ctx.desc), ctypes.byref(a), ctypes.c_void_p(dy.data_ptr()),
                                                ctypes.byref(g), _stream()), "vb_embed_bwd")
         dfe = None
         if d_feats is not None:
@@ -651,43 +545,6 @@ def _gemm(dev, **kw):
         _lib.check(_lib.lib().vb_gemm(ctypes.byref(a), _stream()), "vb_gemm")
 
 
-class DecoderWeights:
-    """bf16 copy of the tied word-embedding matrix [vocab, H] and the fp32 bias padded to a multiple of 16 columns
-    (padding columns get -30000 so they vanish in the softmax), refreshed when the masters change."""
-
-    def __init__(self):
-        self.key = None
-        self.table = None
-        self.bias = None
-        self.bank = None
-
-    def alloc(self, E):
-        V = E.shape[0]
-        Vp = (V + 15) // 16 * 16
-        if self.table is None or self.table.device != E.device or self.table.shape[0] != Vp:
-            self.table = torch.zeros(Vp, E.shape[1], device=E.device, dtype=_BF16)
-            self.bias = torch.full((Vp,), -30000.0, device=E.device, dtype=torch.float32)
-        return self.table, self.bias
-
-    def get(self, E, bias, train=False):
-        if self.bank is not None:
-            return self.table, self.bias
-        key = (E.data_ptr(), E._version, bias.data_ptr(), bias._version)
-        if train or key != self.key:
-            V = E.shape[0]
-            Vp = (V + 15) // 16 * 16
-            with torch.no_grad():
-                # [Vp, H] with zero rows V..Vp-1: the GEMMs address all Vp rows of the table
-                if self.table is None or self.table.device != E.device or self.table.shape[0] != Vp:
-                    self.table = torch.zeros(Vp, E.shape[1], device=E.device, dtype=_BF16)
-                cast_to_bf16(E.detach(), self.table[:V])
-                if self.bias is None or self.bias.device != E.device or self.bias.numel() != Vp:
-                    self.bias = torch.full((Vp,), -30000.0, device=E.device, dtype=torch.float32)
-                self.bias[:V].copy_(bias.detach())
-            self.key = key
-        return self.table, self.bias
-
-
 class _MlmDecoderFn(torch.autograd.Function):
     """logits[n, Vp] = t[n, H] @ E[V, H]^T + bias (BertLMPredictionHead decoder, reference M.py:403-421) — forward,
     input-gradient and weight-gradient GEMMs all on gemm_wgmma_kernel; the weight gradient accumulates straight
@@ -698,8 +555,8 @@ class _MlmDecoderFn(torch.autograd.Function):
         _require_cuda(t, "mlm_decoder")
         n, H = t.shape
         V = E.shape[0]
-        Vp = (V + 15) // 16 * 16
         table, bias_p = cache.get(E, bias, train=train)
+        Vp = table.shape[0]
         t = t.to(_BF16).contiguous()
         logits = torch.empty(n, Vp, device=t.device, dtype=_BF16)
         _gemm(t.device, A=t.data_ptr(), lda=H, B=table.data_ptr(), ldb=H, M=n, N=Vp, K=H, D=logits.data_ptr(), ldd=Vp,
