@@ -45,6 +45,7 @@ int vb_profile_read(double* ms, double* work, int64_t* launches);
 #define VB_EPI_NONE 0
 #define VB_EPI_GELU 1  /* u = acc + bias: aux_out = gelu(u), D = gelu'(u)   — M.py:56-61, 302-305 */
 #define VB_EPI_DGELU 2 /* D = acc * aux_in  (aux_in = the gelu'(u) saved by VB_EPI_GELU) — backward of M.py:304 */
+/* VB_EPI_GELU and VB_EPI_DGELU take no dropout and no addend: vb_gemm refuses such a call. */
 
 typedef struct {
     /* D[M,N] = epilogue( sum_k A(m,k) * B(n,k) )

@@ -66,6 +66,31 @@ def test_argument_validation_reports_through_vb_last_error():
     assert L.vb_gemm(None, None) != 0
 
 
+# 32-byte aligned fake device pointers: every check in vb_gemm runs before its first CUDA call
+_FAKE = dict(A=0x10000, lda=256, B=0x20000, ldb=256, M=256, N=256, K=256, D=0x30000, ldd=256)
+
+
+def test_gemm_refuses_an_unknown_epilogue():
+    from visualbert_b200 import _lib
+    L = _lib.lib()
+    for epi in (3, -1, 9):
+        a = _lib.GemmArgs(epilogue=epi, aux_in=0x40000, aux_out=0x50000, ld_aux=256, **_FAKE)
+        assert L.vb_gemm(ctypes.byref(a), None) != 0
+        assert b"unknown epilogue" in L.vb_last_error()
+
+
+@pytest.mark.parametrize("epi", ["gelu", "dgelu"])
+@pytest.mark.parametrize("extra", ["dropout", "addend"])
+def test_gemm_refuses_gelu_epilogues_with_dropout_or_addend(epi, extra):
+    from visualbert_b200 import _lib
+    L = _lib.lib()
+    kw = dict(epilogue=_lib.VB_EPI_GELU, aux_out=0x50000) if epi == "gelu" else dict(epilogue=_lib.VB_EPI_DGELU, aux_in=0x40000)
+    kw.update(dict(dropout_p=0.1, dropout_seed=1) if extra == "dropout" else dict(addend=0x60000, ld_add=256))
+    a = _lib.GemmArgs(ld_aux=256, **kw, **_FAKE)
+    assert L.vb_gemm(ctypes.byref(a), None) != 0
+    assert b"take no dropout and no addend" in L.vb_last_error()
+
+
 @pytest.mark.skipif(torch.cuda.is_available(), reason="checks the no-GPU behaviour")
 def test_product_path_fails_loudly_without_cuda():
     from visualbert_b200 import BertConfig, TrainVisualBERTObjective, _lib, synthetic

@@ -456,9 +456,9 @@ def test_unpadded_train_mode_reproducible():
 def test_varlen_layer_train_mode_matches_reference_math_with_the_same_masks(lens, A, layer_index):
     """One layer through vb_encoder_fwd_varlen / _bwd_varlen with hidden and attention dropout on, against the reference
     arithmetic (M.py:231-341) in fp32 with THE SAME masks: the hidden-state masks are regenerated with the hash restatement of
-    test_train_parity_gpu.py over the packed [total, H] tensors, the attention bits are read back from the arena's keep buffer,
+    dropout_util.py over the packed [total, H] tensors, the attention bits are read back from the arena's keep buffer,
     and attention runs per sequence. Checks the layer output, the input gradient and every parameter gradient."""
-    from test_train_parity_gpu import hidden_keep
+    from dropout_util import hidden_keep
     from visualbert_b200 import _lib
     L = _lib.lib()
     dev = torch.device("cuda:0")

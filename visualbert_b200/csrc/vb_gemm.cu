@@ -223,9 +223,6 @@ __device__ __forceinline__ void epilogue16(const GemmParams& p, int row, int col
             }
             store16_bf16(d, gp);
             d = p.aux_out + static_cast<long long>(row) * p.ld_aux + col;
-        } else if (kGeneric && p.epilogue == 3) {  // debug/tuning only: two stores, no GELU math
-            store16_bf16(d, x);
-            d = p.aux_out + static_cast<long long>(row) * p.ld_aux + col;
         } else if (epi_is_dgelu(EPI) || (kGeneric && p.epilogue == VB_EPI_DGELU)) {
 #pragma unroll
             for (int i = 0; i < 8; ++i) {
@@ -601,10 +598,12 @@ int gemm(const vb_gemm_args& a, cudaStream_t st) {
     VB_REQUIRE((!a.aux_in && !a.aux_out) || a.ld_aux % 16 == 0, "vb_gemm: ld_aux must be a multiple of 16");
     VB_REQUIRE((reinterpret_cast<uintptr_t>(a.aux_in) & 31) == 0 && (reinterpret_cast<uintptr_t>(a.aux_out) & 31) == 0,
                "vb_gemm: aux_in / aux_out must be 32-byte aligned");
-    VB_REQUIRE(a.epilogue == VB_EPI_NONE || a.epilogue == VB_EPI_GELU || a.epilogue == VB_EPI_DGELU || a.epilogue == 3,
+    VB_REQUIRE(a.epilogue == VB_EPI_NONE || a.epilogue == VB_EPI_GELU || a.epilogue == VB_EPI_DGELU,
                "vb_gemm: unknown epilogue %d", a.epilogue);
     VB_REQUIRE(a.epilogue != VB_EPI_GELU || a.aux_out, "vb_gemm: GELU epilogue needs aux_out");
     VB_REQUIRE(a.epilogue != VB_EPI_DGELU || a.aux_in, "vb_gemm: DGELU epilogue needs aux_in");
+    VB_REQUIRE(a.epilogue == VB_EPI_NONE || (!a.addend && a.dropout_p == 0.0f),
+               "vb_gemm: the GELU / DGELU epilogues take no dropout and no addend");
     VB_REQUIRE(!a.d_fp32 || (a.epilogue == VB_EPI_NONE && !a.addend && a.dropout_p == 0.0f),
                "vb_gemm: fp32-accumulate output supports bias only");
     VB_REQUIRE(a.dropout_p >= 0.0f && a.dropout_p < 1.0f, "vb_gemm: dropout_p out of range");
@@ -661,12 +660,10 @@ int gemm(const vb_gemm_args& a, cudaStream_t st) {
         // specialised epilogues for the shapes of the layer (forward and input-gradient GEMMs); anything else: generic
         const bool drop = a.dropout_p > 0.0f, add = a.addend != nullptr;
         int epi = EPI_GENERIC;
-        if (a.epilogue == VB_EPI_GELU && !drop && !add) epi = a.gp_tiled ? EPI_GELU_FWD_T : EPI_GELU_FWD;
-        else if (a.epilogue == VB_EPI_DGELU && !drop && !add) epi = a.gp_tiled ? EPI_DGELU_BWD_T : EPI_DGELU_BWD;
-        else if (a.epilogue == VB_EPI_NONE) epi = add ? (drop ? EPI_DROP_RESID : EPI_RESID) : (drop ? EPI_GENERIC : EPI_BIAS);
+        if (a.epilogue == VB_EPI_GELU) epi = a.gp_tiled ? EPI_GELU_FWD_T : EPI_GELU_FWD;
+        else if (a.epilogue == VB_EPI_DGELU) epi = a.gp_tiled ? EPI_DGELU_BWD_T : EPI_DGELU_BWD;
+        else epi = add ? (drop ? EPI_DROP_RESID : EPI_RESID) : (drop ? EPI_GENERIC : EPI_BIAS);
         if (a.delta_out) epi = EPI_DELTA;
-        VB_REQUIRE(!a.gp_tiled || epi == EPI_GELU_FWD_T || epi == EPI_DGELU_BWD_T,
-                   "vb_gemm: gp_tiled needs a plain GELU / DGELU epilogue (no dropout, no addend)");
         if (!a.a_mn_major && !a.b_mn_major) {
             switch (epi) {
                 case EPI_BIAS: return launch<false, false, 256, false, EPI_BIAS>(ta, tb, p, st);
