@@ -45,7 +45,11 @@ int vb_profile_read(double* ms, double* work, int64_t* launches);
 #define VB_EPI_NONE 0
 #define VB_EPI_GELU 1  /* u = acc + bias: aux_out = gelu(u), D = gelu'(u)   — M.py:56-61, 302-305 */
 #define VB_EPI_DGELU 2 /* D = acc * aux_in  (aux_in = the gelu'(u) saved by VB_EPI_GELU) — backward of M.py:304 */
-/* VB_EPI_GELU and VB_EPI_DGELU take no dropout and no addend: vb_gemm refuses such a call. */
+/* 3 is retired and refused as unknown */
+#define VB_EPI_GELU_FWD 4 /* u = acc + bias: D = gelu(u) and nothing else (no aux_out, no aux_in, no gp_tiled) — the FFN-up GEMM of a
+                           * forward that no backward follows (evaluation under torch.no_grad(), train.py:292-325). D holds bit for
+                           * bit what VB_EPI_GELU writes to aux_out; K-major A and B and a bf16 D only. */
+/* The GELU epilogues take no dropout and no addend: vb_gemm refuses such a call. */
 
 typedef struct {
     /* D[M,N] = epilogue( sum_k A(m,k) * B(n,k) )
@@ -254,6 +258,23 @@ int vb_encoder_bwd(const vb_layer_desc* descs, int32_t n_layers, const void* x_i
  * descs[l].mask_bias. Call it on the arena and descriptors vb_encoder_fwd just used, before anything overwrites the arena;
  * one launch per layer, no other arena buffer is read. */
 int vb_encoder_attention_probs(const vb_layer_desc* descs, int32_t n_layers, void* arena, float* probs, void* stream);
+/* Forward-only encoder: the forward of a call that no backward follows — the reference's evaluation loop runs the model under
+ * torch.no_grad() (visualbert/models/train.py:292-325). Every layer runs through ONE caller-owned workspace the size of less
+ * than one arena slot, whatever n_layers is. Per layer the launches, their arguments and so every output bit are those of
+ * vb_encoder_fwd, except that nothing only a backward reads is stored: the FFN-up GEMM uses VB_EPI_GELU_FWD (no gelu'), the
+ * attention writes no lse and the LayerNorms no mean / rstd. Dropout (descs[l].hidden_dropout / attn_dropout / seed) is
+ * honoured as in vb_encoder_fwd, so the same seed gives the same output.
+ * vb_encoder_infer_workspace: bytes of that workspace (a multiple of 256; never more than the arena slot stride of the same
+ * shape); packed_rows < 0: dense (M = batch * seq rows), else the row count of a variable-length call with seq = max_seq.
+ * Returns -1 on a bad shape.
+ * y_last: bf16 [M, hidden], the last layer's output. y_all: NULL, or bf16 [n_layers, M, hidden] receiving every layer's
+ * output; y_last must then be NULL or the last slice of y_all. At least one of the two is given.
+ * probs: NULL, or fp32 [n_layers, batch, heads, seq, seq] attention maps (dense only; what vb_encoder_attention_probs gives),
+ * written per layer from the qkv in the workspace before the next layer overwrites it. */
+int64_t vb_encoder_infer_workspace(int32_t batch, int32_t seq, int32_t hidden, int32_t heads, int32_t inter,
+                                   int32_t attn_dropout_on, int64_t packed_rows);
+int vb_encoder_infer(const vb_layer_desc* descs, int32_t n_layers, const void* x_in, void* workspace, void* y_last, void* y_all,
+                     float* probs, void* stream);
 /* Variable-length ("unpadded") encoder: the same calls over `total` packed rows (see vb_attention_fwd_varlen for cu_seqlens and
  * its caller contract). descs[l].batch is the number of sequences and descs[l].seq the longest length (max_seq); mask_bias is
  * ignored and may be NULL. x_in, dy, dx and every row-sized arena / scratch buffer have `total` rows; lse and scratch.drow are
@@ -266,6 +287,10 @@ int vb_encoder_fwd_varlen(const vb_layer_desc* descs, int32_t n_layers, const in
 int vb_encoder_bwd_varlen(const vb_layer_desc* descs, int32_t n_layers, const int32_t* cu_seqlens, int32_t total, const void* x_in,
                           void* arena, const void* dy, void* dx, const vb_layer_grads* grads, const vb_layer_scratch* scratch,
                           void* stream);
+/* vb_encoder_infer over packed rows: workspace of vb_encoder_infer_workspace with packed_rows = total; y_last bf16 [total, hidden],
+ * y_all NULL or bf16 [n_layers, total, hidden]. There are no attention maps of a variable-length call. */
+int vb_encoder_infer_varlen(const vb_layer_desc* descs, int32_t n_layers, const int32_t* cu_seqlens, int32_t total,
+                            const void* x_in, void* workspace, void* y_last, void* y_all, void* stream);
 
 /* ---- BertEmbeddingsWithVisualEmbedding (M.py:1169-1257) ----------------------------------- */
 typedef struct {

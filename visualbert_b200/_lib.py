@@ -12,6 +12,7 @@ LIB_PATH = os.environ.get("VB_LIB_PATH") or os.path.join(_HERE, "lib", "libvbert
 
 ABI_VERSION = 4  # == VB_ABI_VERSION of include/vbert_b200.h (tests/test_abi.py keeps the two in step)
 VB_EPI_NONE, VB_EPI_GELU, VB_EPI_DGELU = 0, 1, 2
+VB_EPI_GELU_FWD = 4  # 3 is retired
 
 c_void_p, c_int, c_i64, c_f32, c_u64, c_u32 = (
     ctypes.c_void_p, ctypes.c_int32, ctypes.c_int64, ctypes.c_float, ctypes.c_uint64, ctypes.c_uint32)
@@ -80,6 +81,7 @@ EXPORTS = [
     "vb_bert_adam_step", "vb_cast_multi", "vb_encoder_arena_layout", "vb_encoder_fwd", "vb_encoder_bwd",
     "vb_attention_fwd_varlen", "vb_attention_bwd_varlen", "vb_encoder_arena_layout_varlen", "vb_encoder_fwd_varlen",
     "vb_encoder_bwd_varlen", "vb_attention_probs", "vb_encoder_attention_probs",
+    "vb_encoder_infer_workspace", "vb_encoder_infer", "vb_encoder_infer_varlen",
 ]
 VB_ENCODER_ARENA_BUFFERS = 14
 ARENA_NAMES = ("qkv", "ctx", "lse", "pre1", "mean1", "rstd1", "x1", "u", "g", "pre2", "mean2", "rstd2", "keep_mask", "y")
@@ -115,6 +117,10 @@ def lib():
         h.vb_encoder_bwd_varlen.argtypes = [_P, _I, _P, _I, _P, _P, _P, _P, _P, _P, _P]
         h.vb_attention_probs.argtypes = [_P, _P, _P, _I, _I, _I, _I, _P]
         h.vb_encoder_attention_probs.argtypes = [_P, _I, _P, _P, _P]
+        h.vb_encoder_infer_workspace.restype = ctypes.c_int64
+        h.vb_encoder_infer_workspace.argtypes = [_I, _I, _I, _I, _I, _I, c_i64]
+        h.vb_encoder_infer.argtypes = [_P, _I, _P, _P, _P, _P, _P, _P]
+        h.vb_encoder_infer_varlen.argtypes = [_P, _I, _P, _I, _P, _P, _P, _P, _P]
         _lib = h
     return _lib
 

@@ -10,6 +10,7 @@
 //   6 GEMM   pre2 = dropout(g W2^T + b) + x1           (M.py:316-318)
 //   7 LN     out  = LayerNorm(pre2)
 // vb_layer_bwd is the exact adjoint (autograd of the above), weight gradients accumulated in fp32.
+// vb_encoder_infer runs the same sequence for a forward no backward follows: step 5 writes g alone and no statistics are kept.
 #include <string.h>
 
 #include "vb_internal.h"
@@ -70,8 +71,10 @@ static int check_layer(const vb_layer_desc* d, const LayerRows& r) {
     return 0;
 }
 
+// for_bwd = false (vb_encoder_infer): the same launches with the same arguments, but nothing only a backward reads is stored —
+// s->u is not touched (the FFN-up epilogue writes gelu(u) alone) and s->lse, s->mean1/2, s->rstd1/2 may be NULL
 int layer_fwd(const vb_layer_desc* d, const void* x_in, void* x_out, const vb_layer_acts* s, cudaStream_t st,
-              const LayerRows& rows = kDenseRows) {
+              const LayerRows& rows = kDenseRows, bool for_bwd = true) {
     VB_TRY(check_layer(d, rows));
     VB_REQUIRE(x_in && x_out && s, "layer_fwd: null pointer");
     const bool vl = rows.cu_seqlens != nullptr;
@@ -81,7 +84,7 @@ int layer_fwd(const vb_layer_desc* d, const void* x_in, void* x_out, const vb_la
     VB_TRY(gemm(a, st));
     if (vl)
         VB_TRY(attn_fwd_varlen(s->qkv, rows.cu_seqlens, s->ctx, s->lse, s->keep_mask, d->batch, d->seq, rows.total, d->heads, H,
-                               d->attn_dropout, d->seed, drop_stream(d->layer_index, kSiteAttnProbs), st));
+                               d->attn_dropout, d->seed, drop_stream(d->layer_index, kSiteAttnProbs), st, for_bwd));
     else
         VB_TRY(attn_fwd(s->qkv, d->mask_bias, s->ctx, s->lse, s->keep_mask, d->batch, d->seq, d->heads, H, d->attn_dropout, d->seed,
                         drop_stream(d->layer_index, kSiteAttnProbs), st));
@@ -90,9 +93,14 @@ int layer_fwd(const vb_layer_desc* d, const void* x_in, void* x_out, const vb_la
     a.dropout_p = d->hidden_dropout; a.dropout_seed = d->seed; a.dropout_stream = drop_stream(d->layer_index, kSiteAttnOut);
     VB_TRY(gemm(a, st));
     VB_TRY(ln_fwd(s->pre1, H, d->ln1_gamma, d->ln1_beta, s->x1, H, s->mean1, s->rstd1, M, H, kLnEps, st));
-    a = fwd_args(s->x1, d->w_inter, s->u, M, I, H);
-    a.bias = d->b_inter; a.epilogue = VB_EPI_GELU; a.aux_out = s->g; a.ld_aux = I;
-    a.gp_tiled = gemm_gp_tiled_ok(M, I) ? 1 : 0;   // acts.u is private to the library: tile-native whenever the shape allows
+    if (for_bwd) {
+        a = fwd_args(s->x1, d->w_inter, s->u, M, I, H);
+        a.bias = d->b_inter; a.epilogue = VB_EPI_GELU; a.aux_out = s->g; a.ld_aux = I;
+        a.gp_tiled = gemm_gp_tiled_ok(M, I) ? 1 : 0;   // acts.u is private to the library: tile-native whenever the shape allows
+    } else {
+        a = fwd_args(s->x1, d->w_inter, s->g, M, I, H);
+        a.bias = d->b_inter; a.epilogue = VB_EPI_GELU_FWD;
+    }
     VB_TRY(gemm(a, st));
     a = fwd_args(s->g, d->w_out, s->pre2, M, H, I);
     a.bias = d->b_out; a.addend = s->x1; a.ld_add = H;
@@ -220,6 +228,60 @@ int encoder_bwd(const vb_layer_desc* descs, int n, const void* x_in, void* arena
         // the gradient buffer ping-pongs inside `dx` (vb_layer_bwd allows dx to alias dy)
         VB_TRY(layer_bwd(&descs[l], xl, &a, g_in, dx, &grads[l], w, st, rows));
         g_in = dx;
+    }
+    return 0;
+}
+
+// ---- forward-only encoder: every layer through one workspace, nothing kept for a backward ----
+enum { kWsQkv, kWsCtx, kWsPre, kWsX1, kWsG, kWsKeep, kWsY0, kWsY1, kWsBuffers };
+
+// pre1 and pre2 share one buffer (LayerNorm 1 has consumed pre1 before the FFN-down GEMM writes pre2); y0 / y1 are the ping-pong
+// layer outputs of a call without y_all. Everything here is also in an arena slot, which holds u, lse and the statistics besides:
+// the workspace is never larger than the slot.
+long long infer_workspace_layout(int B, int S, int H, int A, int I, int attn_drop, long long packed_rows, long long* off) {
+    const long long M = packed_rows >= 0 ? packed_rows : static_cast<long long>(B) * S;
+    const long long sizes[kWsBuffers] = {M * 3 * H * 2, M * H * 2, M * H * 2, M * H * 2, M * I * 2,
+                                         attn_drop ? attn_keep_bytes(B, S, A) : 0, M * H * 2, M * H * 2};
+    long long o = 0;
+    for (int i = 0; i < kWsBuffers; ++i) {
+        if (off) off[i] = o;
+        o += align256(sizes[i]);
+    }
+    return o;
+}
+
+int encoder_infer(const vb_layer_desc* descs, int n, const void* x_in, void* workspace, void* y_last, void* y_all, float* probs,
+                  cudaStream_t st, const LayerRows& rows = kDenseRows) {
+    VB_REQUIRE(descs && n > 0, "encoder_infer: null descriptors / no layers");
+    VB_REQUIRE(x_in && workspace, "encoder_infer: null x_in / workspace");
+    VB_REQUIRE(y_last || y_all, "encoder_infer: y_last and y_all are both NULL");
+    const vb_layer_desc& d0 = descs[0];
+    for (int l = 0; l < n; ++l) {  // every descriptor is checked before the first launch: a refused call writes nothing
+        VB_TRY(check_layer(&descs[l], rows));
+        VB_REQUIRE(descs[l].batch == d0.batch && descs[l].seq == d0.seq && descs[l].hidden == d0.hidden && descs[l].heads == d0.heads &&
+                   descs[l].inter == d0.inter && (descs[l].attn_dropout > 0.f) == (d0.attn_dropout > 0.f),
+                   "encoder_infer: layers differ in shape");
+    }
+    const bool vl = rows.cu_seqlens != nullptr;
+    const long long M = vl ? rows.total : static_cast<long long>(d0.batch) * d0.seq;
+    const long long y_bytes = M * d0.hidden * 2;
+    char* const ya = static_cast<char*>(y_all);
+    VB_REQUIRE(!ya || !y_last || y_last == ya + (n - 1) * y_bytes, "encoder_infer: with y_all, y_last must be NULL or its last slice");
+    long long off[kWsBuffers];
+    infer_workspace_layout(d0.batch, d0.seq, d0.hidden, d0.heads, d0.inter, d0.attn_dropout > 0.f, vl ? rows.total : -1, off);
+    char* const ws = static_cast<char*>(workspace);
+    vb_layer_acts a;
+    memset(&a, 0, sizeof(a));
+    a.qkv = ws + off[kWsQkv]; a.ctx = ws + off[kWsCtx]; a.pre1 = a.pre2 = ws + off[kWsPre]; a.x1 = ws + off[kWsX1]; a.g = ws + off[kWsG];
+    a.keep_mask = d0.attn_dropout > 0.f ? ws + off[kWsKeep] : nullptr;
+    const long long per_layer = static_cast<long long>(d0.batch) * d0.heads * d0.seq * d0.seq;
+    const void* x = x_in;
+    for (int l = 0; l < n; ++l) {
+        void* y = ya ? ya + l * y_bytes : l == n - 1 ? y_last : ws + off[(l & 1) ? kWsY1 : kWsY0];
+        VB_TRY(layer_fwd(&descs[l], x, y, &a, st, rows, false));
+        if (probs)
+            VB_TRY(attn_probs(a.qkv, descs[l].mask_bias, probs + l * per_layer, d0.batch, d0.seq, d0.heads, d0.hidden, st));
+        x = y;
     }
     return 0;
 }
@@ -358,6 +420,26 @@ int vb_encoder_fwd_varlen(const vb_layer_desc* descs, int32_t n_layers, const in
     if (total <= 0) { vb::set_error("vb_encoder_fwd_varlen: total (%d) must be > 0", total); return 2; }
     const vb::LayerRows rows = {cu_seqlens, total};
     return vb::encoder_fwd(descs, n_layers, x_in, arena, static_cast<cudaStream_t>(stream), rows);
+}
+int64_t vb_encoder_infer_workspace(int32_t batch, int32_t seq, int32_t hidden, int32_t heads, int32_t inter, int32_t attn_dropout_on,
+                                   int64_t packed_rows) {
+    if (batch <= 0 || seq <= 0 || hidden <= 0 || heads <= 0 || inter <= 0 || packed_rows == 0 || packed_rows >= (1LL << 31)) {
+        vb::set_error("vb_encoder_infer_workspace: bad shape (batch %d, seq %d, hidden %d, heads %d, inter %d, packed_rows %lld)", batch,
+                      seq, hidden, heads, inter, static_cast<long long>(packed_rows));
+        return -1;
+    }
+    return vb::infer_workspace_layout(batch, seq, hidden, heads, inter, attn_dropout_on, packed_rows, nullptr);
+}
+int vb_encoder_infer(const vb_layer_desc* descs, int32_t n_layers, const void* x_in, void* workspace, void* y_last, void* y_all,
+                     float* probs, void* stream) {
+    return vb::encoder_infer(descs, n_layers, x_in, workspace, y_last, y_all, probs, static_cast<cudaStream_t>(stream));
+}
+int vb_encoder_infer_varlen(const vb_layer_desc* descs, int32_t n_layers, const int32_t* cu_seqlens, int32_t total, const void* x_in,
+                            void* workspace, void* y_last, void* y_all, void* stream) {
+    if (cu_seqlens == nullptr) { vb::set_error("vb_encoder_infer_varlen: cu_seqlens is NULL"); return 2; }
+    if (total <= 0) { vb::set_error("vb_encoder_infer_varlen: total (%d) must be > 0", total); return 2; }
+    const vb::LayerRows rows = {cu_seqlens, total};
+    return vb::encoder_infer(descs, n_layers, x_in, workspace, y_last, y_all, nullptr, static_cast<cudaStream_t>(stream), rows);
 }
 int vb_encoder_bwd_varlen(const vb_layer_desc* descs, int32_t n_layers, const int32_t* cu_seqlens, int32_t total, const void* x_in,
                           void* arena, const void* dy, void* dx, const vb_layer_grads* grads, const vb_layer_scratch* scratch,

@@ -525,11 +525,11 @@ int attn_fwd(const void* qkv, const float* mask_bias, void* ctx, float* lse, voi
 }
 
 int attn_fwd_varlen(const void* qkv, const int* cu_seqlens, void* ctx, float* lse, void* keep, int B, int max_seq, int total,
-                    int A, int H, float dropout_p, unsigned long long seed, unsigned stream_id, cudaStream_t st) {
+                    int A, int H, float dropout_p, unsigned long long seed, unsigned stream_id, cudaStream_t st, bool need_lse) {
     AttnParams p;
     int rc = fill_params(p, qkv, nullptr, ctx, lse, nullptr, nullptr, nullptr, keep, B, max_seq, A, H, dropout_p, seed, stream_id);
     if (rc) return rc;
-    VB_REQUIRE(lse != nullptr, "attention varlen: lse is NULL");
+    VB_REQUIRE(lse != nullptr || !need_lse, "attention varlen: lse is NULL");
     if ((rc = set_varlen(p, cu_seqlens, total, qkv, ctx))) return rc;
     if (total == 0) return 0;  // no rows: nothing to compute or store
     return attn_fwd_launch(p, st);

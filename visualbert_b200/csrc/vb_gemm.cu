@@ -169,8 +169,10 @@ __device__ __forceinline__ void store16_bf16(bf16* p, const float (&f)[16]) {
 // EPI_DELTA: plain bf16 store plus the attention backward's D[b, head, s] = sum_d dO[row, head, d] * O[row, head, d] (vb_gemm_args.delta_*):
 // the GEMM that PRODUCES dO (input gradient of attention.output.dense) has, in each epilogue thread, 128 consecutive columns of one row —
 // two whole heads — so the row-wise dot product with O needs no exchange; O is read like a residual operand.
+// EPI_GELU_ONLY (VB_EPI_GELU_FWD of the ABI): D = gelu(u) and nothing else — the forward-only FFN-up GEMM. It takes the plain
+// bf16 store path (one coalesced store per element) with the gelu of the two-tensor epilogues.
 enum { EPI_GENERIC = 0, EPI_BIAS = 1, EPI_RESID = 2, EPI_DROP_RESID = 3, EPI_GELU_FWD = 4, EPI_DGELU_BWD = 5, EPI_GELU_FWD_T = 6,
-       EPI_DGELU_BWD_T = 7, EPI_DELTA = 8 };
+       EPI_DGELU_BWD_T = 7, EPI_DELTA = 8, EPI_GELU_ONLY = 9 };
 __host__ __device__ constexpr bool epi_is_gelu(int e) { return e == EPI_GELU_FWD || e == EPI_GELU_FWD_T; }
 __host__ __device__ constexpr bool epi_is_dgelu(int e) { return e == EPI_DGELU_BWD || e == EPI_DGELU_BWD_T; }
 
@@ -211,7 +213,14 @@ __device__ __forceinline__ void epilogue16(const GemmParams& p, int row, int col
             }
         }
         bf16* d = reinterpret_cast<bf16*>(p.D) + static_cast<long long>(row) * p.ldd + col;
-        if (epi_is_gelu(EPI) || (kGeneric && p.epilogue == VB_EPI_GELU)) {
+        if (EPI == EPI_GELU_ONLY) {
+            // D <- gelu(u): the value the GELU epilogue below sends to aux_out, from the same function; its derivative is dropped
+#pragma unroll
+            for (int i = 0; i < 16; ++i) {
+                float gp;
+                gelu_fwd_bwd(x[i], x[i], gp);
+            }
+        } else if (epi_is_gelu(EPI) || (kGeneric && p.epilogue == VB_EPI_GELU)) {
             // aux_out <- gelu(u) (operand of the next GEMM), D <- gelu'(u) (all the backward needs of u)
             float gp[16];
 #pragma unroll
@@ -373,7 +382,7 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
     const long long gp_warp_off =
         ((((static_cast<long long>(tc.m_blk >> 1) * n_blocks + tc.n_blk) * 2 + (tc.m_blk & 1)) * kEpiWarps + ew) * NCH) * 512;
     auto gp_off = [&](int j) { return gp_warp_off + chunk_of(j) * 512 + wrow_of(j) * 16; };
-    constexpr bool kEx = !OUT_F32 && EPI != EPI_BIAS && !epi_is_gelu(EPI);
+    constexpr bool kEx = !OUT_F32 && EPI != EPI_BIAS && !epi_is_gelu(EPI) && EPI != EPI_GELU_ONLY;
     uint32_t ex[kEx ? NCH : 1][8];
     if constexpr (kEx) {
         constexpr bool kWantAdd = EPI == EPI_RESID || EPI == EPI_DROP_RESID || EPI == EPI_DELTA;   // EPI_DELTA: addend = O
@@ -598,12 +607,14 @@ int gemm(const vb_gemm_args& a, cudaStream_t st) {
     VB_REQUIRE((!a.aux_in && !a.aux_out) || a.ld_aux % 16 == 0, "vb_gemm: ld_aux must be a multiple of 16");
     VB_REQUIRE((reinterpret_cast<uintptr_t>(a.aux_in) & 31) == 0 && (reinterpret_cast<uintptr_t>(a.aux_out) & 31) == 0,
                "vb_gemm: aux_in / aux_out must be 32-byte aligned");
-    VB_REQUIRE(a.epilogue == VB_EPI_NONE || a.epilogue == VB_EPI_GELU || a.epilogue == VB_EPI_DGELU,
+    VB_REQUIRE(a.epilogue == VB_EPI_NONE || a.epilogue == VB_EPI_GELU || a.epilogue == VB_EPI_DGELU || a.epilogue == VB_EPI_GELU_FWD,
                "vb_gemm: unknown epilogue %d", a.epilogue);
     VB_REQUIRE(a.epilogue != VB_EPI_GELU || a.aux_out, "vb_gemm: GELU epilogue needs aux_out");
     VB_REQUIRE(a.epilogue != VB_EPI_DGELU || a.aux_in, "vb_gemm: DGELU epilogue needs aux_in");
     VB_REQUIRE(a.epilogue == VB_EPI_NONE || (!a.addend && a.dropout_p == 0.0f),
-               "vb_gemm: the GELU / DGELU epilogues take no dropout and no addend");
+               "vb_gemm: the GELU / DGELU / GELU_FWD epilogues take no dropout and no addend");
+    VB_REQUIRE(a.epilogue != VB_EPI_GELU_FWD || (!a.a_mn_major && !a.b_mn_major && !a.d_fp32 && !a.aux_in && !a.aux_out),
+               "vb_gemm: the GELU_FWD epilogue needs K-major A and B and a bf16 D, and takes no aux_in / aux_out");
     VB_REQUIRE(!a.d_fp32 || (a.epilogue == VB_EPI_NONE && !a.addend && a.dropout_p == 0.0f),
                "vb_gemm: fp32-accumulate output supports bias only");
     VB_REQUIRE(a.dropout_p >= 0.0f && a.dropout_p < 1.0f, "vb_gemm: dropout_p out of range");
@@ -656,6 +667,8 @@ int gemm(const vb_gemm_args& a, cudaStream_t st) {
     else               rc = make_tmap_bf16(&tb, a.B, a.N, a.K, a.ldb, BLOCK_K);
     if (rc) return rc;
 
+    if (a.epilogue == VB_EPI_GELU_FWD)
+        return bn256 ? launch<false, false, 256, false, EPI_GELU_ONLY>(ta, tb, p, st) : launch<false, false, 128, false, EPI_GELU_ONLY>(ta, tb, p, st);
     if (bn256 && !a.d_fp32) {
         // specialised epilogues for the shapes of the layer (forward and input-gradient GEMMs); anything else: generic
         const bool drop = a.dropout_p > 0.0f, add = a.addend != nullptr;

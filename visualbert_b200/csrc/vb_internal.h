@@ -24,9 +24,9 @@ int attn_bwd(const void* qkv, const float* mask_bias, const void* ctx, const flo
              const void* dctx, void* dqkv, float* drow, int B, int S, int A, int H, float dropout_p,
              unsigned long long seed, unsigned stream_id, cudaStream_t st, bool delta_ready = false);
 // variable-length attention: sequence b owns packed rows [cu_seqlens[b], cu_seqlens[b+1]) (device), at most max_seq of them;
-// lse / drow are [A, total]
+// lse / drow are [A, total]; need_lse = false (a forward no backward follows) lets lse be NULL, as the dense call always does
 int attn_fwd_varlen(const void* qkv, const int* cu_seqlens, void* ctx, float* lse, void* keep, int B, int max_seq, int total,
-                    int A, int H, float dropout_p, unsigned long long seed, unsigned stream_id, cudaStream_t st);
+                    int A, int H, float dropout_p, unsigned long long seed, unsigned stream_id, cudaStream_t st, bool need_lse = true);
 int attn_bwd_varlen(const void* qkv, const int* cu_seqlens, const void* ctx, const float* lse, const void* keep,
                     const void* dctx, void* dqkv, float* drow, int B, int max_seq, int total, int A, int H, float dropout_p,
                     unsigned long long seed, unsigned stream_id, cudaStream_t st, bool delta_ready = false);

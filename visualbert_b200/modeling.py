@@ -222,21 +222,19 @@ class BertEncoder(nn.Module):
                                  "padded per-layer path")
             if len(self.layer) == 0:
                 return [hidden_states]
-            meta = _encoder_meta(self, self.layer, seed, varlen=varlen)
-            ys = ops.bert_encoder(hidden_states.to(torch.bfloat16), None, meta, self._fused_params())
-            return list(ys) if output_all_encoded_layers else [ys[-1]]
+            meta = _encoder_meta(self, self.layer, seed, varlen=varlen, all_layers=bool(output_all_encoded_layers))
+            return list(ops.bert_encoder(hidden_states.to(torch.bfloat16), None, meta, self._fused_params()))
         if attention_mask.dim() == 4:
             attention_mask = attention_mask[:, 0, 0, :]
         fused = (hidden_states.is_cuda and len(self.layer) > 0
                  and not (output_all_encoded_layers and torch.is_grad_enabled() and self.training))
         if fused:
-            # one C call for the whole stack (vb_encoder_fwd / vb_encoder_bwd, one activation arena), and with maps one
-            # vb_encoder_attention_probs call over the same arena
-            meta = _encoder_meta(self, self.layer, seed, attn_maps=want_maps)
+            # one C call for the whole stack: vb_encoder_fwd / vb_encoder_bwd over one activation arena (with maps, one
+            # vb_encoder_attention_probs call over the same arena), or vb_encoder_infer when no graph can be recorded
+            meta = _encoder_meta(self, self.layer, seed, attn_maps=want_maps, all_layers=bool(output_all_encoded_layers))
             ys = ops.bert_encoder(hidden_states.to(torch.bfloat16), attention_mask.float().contiguous(), meta, self._fused_params())
-            L = len(self.layer)
-            outs = list(ys[:L]) if output_all_encoded_layers else [ys[L - 1]]
-            return (outs, list(ys[L:])) if want_maps else outs
+            n = len(self.layer) if output_all_encoded_layers else 1
+            return (list(ys[:n]), list(ys[n:])) if want_maps else list(ys)
         outs, attn = [], []
         for layer in self.layer:
             if want_maps:

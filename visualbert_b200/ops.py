@@ -399,13 +399,57 @@ class _EncoderFn(torch.autograd.Function):
         return (dx, None, None) + _autograd_grads(flat, L, H, I)
 
 
+def _encoder_infer(x, mbias, meta, params):
+    """The forward of bert_encoder when no graph can be recorded (the reference evaluates under torch.no_grad(),
+    train.py:292-325): vb_encoder_infer / vb_encoder_infer_varlen run every layer through one workspace that does not grow with
+    the depth and store nothing a backward would read. The workspace lives for the call only — kept, it would sit in the
+    allocator through the next training epoch — and the outputs are freshly allocated: one tensor when only the last layer is
+    wanted, one [L, ...] tensor unbound into L views otherwise. Bit for bit the arena path's outputs, dropout included (same
+    seed and layer indices in the descriptors)."""
+    _require_cuda(x, "bert_encoder")
+    B, S, H, M, oshape = _EncoderFn._shape(x, meta)
+    vl = meta.get("varlen")
+    L = len(params) // 16
+    I = params[10].shape[0]
+    A = meta["heads"]
+    x = x.detach().contiguous()
+    if meta.get("attn_maps") and vl is not None:
+        raise ValueError("bert_encoder: attention maps need a dense (padded) call")
+    with torch.cuda.device(x.device):
+        descs = meta["plan"].prepare(meta["caches"], params, B, S, H, A, I, mbias, meta, x.device, vl)[0]
+        nbytes = int(_lib.lib().vb_encoder_infer_workspace(B, S, H, A, I, 1 if meta["attn_dropout"] > 0 else 0, -1 if vl is None else M))
+        if nbytes < 0:
+            _lib.check(1, "vb_encoder_infer_workspace")
+        ws = torch.empty(nbytes, device=x.device, dtype=torch.uint8)
+        if meta.get("all_layers", True):
+            y_all = torch.empty((L,) + tuple(oshape), device=x.device, dtype=_BF16)
+            y_last, outs = None, tuple(y_all.unbind(0))
+        else:
+            y_last = torch.empty(oshape, device=x.device, dtype=_BF16)
+            y_all, outs = None, (y_last,)
+        probs = torch.empty(L, B, A, S, S, device=x.device, dtype=torch.float32) if meta.get("attn_maps") else None
+        if vl is None:
+            _lib.check(_lib.lib().vb_encoder_infer(descs, L, x.data_ptr(), ws.data_ptr(), _ptr(y_last), _ptr(y_all), _ptr(probs),
+                                                   _stream()), "vb_encoder_infer")
+        else:
+            _lib.check(_lib.lib().vb_encoder_infer_varlen(descs, L, vl["cu_seqlens"].data_ptr(), M, x.data_ptr(), ws.data_ptr(),
+                                                          _ptr(y_last), _ptr(y_all), _stream()), "vb_encoder_infer_varlen")
+    return outs + (() if probs is None else tuple(probs.unbind(0)))
+
+
 def bert_encoder(x, mbias, meta, params):
     """All layers at once. meta: dict(heads, layer_index0, hidden_dropout, attn_dropout, seed, train, caches=[LayerWeights],
-    plan=EncoderPlan, optional varlen=unpad_plan(...), optional attn_maps=True); params: 16 tensors per layer in bert_layer
-    order. Returns the tuple of all layer outputs (only the last one is differentiable: a caller that needs gradients through
-    intermediate outputs calls bert_layer once per layer), followed, with attn_maps, by the L detached fp32 [B, A, S, S]
-    attention maps."""
-    return _EncoderFn.apply(x, mbias, meta, *params)
+    plan=EncoderPlan, optional varlen=unpad_plan(...), optional attn_maps=True, optional all_layers=False); params: 16 tensors
+    per layer in bert_layer order. Returns the tuple of all layer outputs (only the last one is differentiable: a caller that
+    needs gradients through intermediate outputs calls bert_layer once per layer) — with all_layers=False only the last
+    layer's — followed, with attn_maps, by the L detached fp32 [B, A, S, S] attention maps.
+
+    When no graph can be recorded (grad mode off, or neither x nor any parameter requires grad) the call takes the
+    forward-only route (_encoder_infer); every other call keeps its activations in the arena of _EncoderFn."""
+    if not (torch.is_grad_enabled() and (x.requires_grad or any(p.requires_grad for p in params))):
+        return _encoder_infer(x, mbias, meta, params)
+    outs = _EncoderFn.apply(x, mbias, meta, *params)
+    return outs if meta.get("all_layers", True) else outs[len(params) // 16 - 1:]
 
 
 def unpad_plan(valid):
@@ -429,7 +473,7 @@ def bert_layer(x, mbias, meta, params):
     BertLayer in reference order (q.w, q.b, k.w, k.b, v.w, v.b, attention.output dense.w/.b, LayerNorm.w/.b,
     intermediate.dense.w/.b, output.dense.w/.b, LayerNorm.w/.b). With meta["attn_maps"] returns (output, detached fp32
     [B, A, S, S] attention maps)."""
-    outs = _EncoderFn.apply(x, mbias, meta, *params)
+    outs = bert_encoder(x, mbias, meta, params)
     return outs if meta.get("attn_maps") else outs[0]
 
 
