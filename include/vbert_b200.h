@@ -40,6 +40,19 @@ int64_t vb_launch_count(void);
 void vb_profile_enable(int on);
 int vb_profile_read(double* ms, double* work, int64_t* launches);
 
+/* Deterministic reductions (torch.use_deterministic_algorithms). While a workspace is set ON THE CALLING THREAD, every entry
+ * point that reduces across CTAs does so in a fixed order: split-K weight gradients, LayerNorm dgamma/dbeta/dbias, column sums,
+ * embedding-table gradients, the BertAdam gradient norms. Results are then bitwise reproducible for the same inputs, shapes,
+ * build and GPU model. workspace = NULL turns it off (the default: today's kernels, unchanged). The library allocates nothing;
+ * a call that needs more scratch than `bytes` fails with vb_last_error() naming the bytes it needs, BEFORE launching anything
+ * (a split-K GEMM whose slabs do not fit lowers its split factor instead). The workspace must be 256-byte aligned.
+ * The workspace is used in stream order: do not share one workspace between streams that run concurrently. */
+int vb_set_deterministic(void* workspace, int64_t bytes);
+/* bytes of workspace that every call of an encoder / embedding / MLM-decoder / BertAdam of this shape needs
+ * (rows = the largest M of any call; adam_chunks = n_chunks of the largest vb_bert_adam_step). Arguments that do not apply may
+ * be 0 (e.g. inter and vocab for a BertAdam-only workspace); for the embedding pass inter = visual_dim. -1 on a bad shape. */
+int64_t vb_deterministic_workspace_bytes(int64_t rows, int32_t hidden, int32_t inter, int32_t vocab, int32_t adam_chunks);
+
 /* ---- GEMM core (wgmma + TMA + mbarrier) --------------------------------------------------- */
 /* epilogue selectors */
 #define VB_EPI_NONE 0

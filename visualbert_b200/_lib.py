@@ -82,6 +82,7 @@ EXPORTS = [
     "vb_attention_fwd_varlen", "vb_attention_bwd_varlen", "vb_encoder_arena_layout_varlen", "vb_encoder_fwd_varlen",
     "vb_encoder_bwd_varlen", "vb_attention_probs", "vb_encoder_attention_probs",
     "vb_encoder_infer_workspace", "vb_encoder_infer", "vb_encoder_infer_varlen",
+    "vb_set_deterministic", "vb_deterministic_workspace_bytes",
 ]
 VB_ENCODER_ARENA_BUFFERS = 14
 ARENA_NAMES = ("qkv", "ctx", "lse", "pre1", "mean1", "rstd1", "x1", "u", "g", "pre2", "mean2", "rstd2", "keep_mask", "y")
@@ -121,6 +122,9 @@ def lib():
         h.vb_encoder_infer_workspace.argtypes = [_I, _I, _I, _I, _I, _I, c_i64]
         h.vb_encoder_infer.argtypes = [_P, _I, _P, _P, _P, _P, _P, _P]
         h.vb_encoder_infer_varlen.argtypes = [_P, _I, _P, _I, _P, _P, _P, _P, _P]
+        h.vb_set_deterministic.argtypes = [_P, c_i64]
+        h.vb_deterministic_workspace_bytes.restype = ctypes.c_int64
+        h.vb_deterministic_workspace_bytes.argtypes = [c_i64, _I, _I, _I, _I]
         _lib = h
     return _lib
 

@@ -110,12 +110,20 @@ int layer_fwd(const vb_layer_desc* d, const void* x_in, void* x_out, const vb_la
     return 0;
 }
 
+// deterministic mode: the workspace one layer backward needs (its LayerNorm and column-sum partials; a weight-gradient GEMM
+// whose slabs do not fit lowers its split factor instead). Checked before the first launch, so a refused call launches nothing.
+static long long layer_bwd_det_bytes(int M, int H, int I) {
+    const long long c = colsum_det_bytes(M, I) > colsum_det_bytes(M, 3 * H) ? colsum_det_bytes(M, I) : colsum_det_bytes(M, 3 * H);
+    return ln_bwd_det_bytes(M, H) > c ? ln_bwd_det_bytes(M, H) : c;
+}
+
 int layer_bwd(const vb_layer_desc* d, const void* x_in, const vb_layer_acts* s, const void* dy, void* dx,
               const vb_layer_grads* g, const vb_layer_scratch* w, cudaStream_t st, const LayerRows& rows = kDenseRows) {
     VB_TRY(check_layer(d, rows));
     VB_REQUIRE(x_in && s && dy && dx && g && w, "layer_bwd: null pointer");
     const bool vl = rows.cu_seqlens != nullptr;
     const int M = vl ? rows.total : d->batch * d->seq, H = d->hidden, I = d->inter;
+    VB_TRY(det_require(layer_bwd_det_bytes(M, H, I), "layer backward"));
     const bool hd = d->hidden_dropout > 0.f;
     VB_REQUIRE(!hd || w->d_pre_drop, "layer_bwd: d_pre_drop scratch required when hidden_dropout > 0");
     void* dpm = hd ? w->d_pre_drop : w->d_pre;  // gradient entering the Linear in front of each LayerNorm
@@ -355,6 +363,14 @@ int embed_bwd_api(const vb_embed_desc* d, const vb_embed_acts* s, const void* dy
     VB_TRY(check_embed(d));
     VB_REQUIRE(s && dy && g && g->d_pre, "embed_bwd: null pointer");
     const int M = d->batch * (d->text_len + d->num_regions), H = d->hidden, BV = d->batch * d->num_regions;
+    if (det_ws().ptr != nullptr) {   // every launch of the call fits the workspace, or nothing is launched
+        const long long temp = embed_sort_temp_bytes(d->batch, d->text_len, d->num_regions);
+        VB_REQUIRE(temp >= 0, "embed_bwd: radix sort size query failed");
+        long long need = embed_bwd_det_bytes(d->batch, d->text_len, d->num_regions, H, temp);
+        if (ln_bwd_det_bytes(M, H) > need) need = ln_bwd_det_bytes(M, H);
+        if (BV > 0 && colsum_det_bytes(BV, H) > need) need = colsum_det_bytes(BV, H);
+        VB_TRY(det_require(need, "embed_bwd"));
+    }
     VB_TRY(ln_bwd(dy, s->pre, s->mean, s->rstd, d->gamma, g->d_pre, nullptr, g->dgamma, g->dbeta, nullptr, M, H, 0.f,
                   d->seed, 0, d->dropout, kEmbedDropStream, st));
     EmbedBwdParams p;
@@ -376,9 +392,54 @@ int embed_bwd_api(const vb_embed_desc* d, const vb_embed_acts* s, const void* dy
     return 0;
 }
 
+// vb_deterministic_workspace_bytes: the largest workspace any deterministic call of these shapes takes, as a function that grows
+// with every argument. A weight-gradient GEMM's slabs are sized for the split factor of every K up to `rows` (so that none of these
+// GEMMs lowers its split factor, and the bits do not depend on which calls sized the workspace first); the split factor falls as
+// the tile count grows, so the MLM decoder's [vocab, H] term is the largest over every smaller padded vocabulary. Column sums are
+// bounded by 4 * max(N, 6 * SMs * 256) bytes (colsum_gy partial rows of N columns).
+static int max_splits(long long tiles, int rows) {
+    int splits = 1;
+    for (int kb = 1; kb <= gemm_k_blocks(rows); ++kb) { const int s = wgrad_splits(tiles, kb); if (s > splits) splits = s; }
+    return splits;
+}
+long long deterministic_workspace_bytes(long long rows, int H, int I, int vocab, int adam_chunks) {
+    long long need = 4LL * adam_chunks;
+    auto up = [&](long long b) { if (b > need) need = b; };
+    if (rows > 0 && H > 0) {
+        const int R = rows < (1LL << 30) ? static_cast<int>(rows) : (1 << 30);
+        auto colsum_bound = [&](long long N) { return 4 * (N > 6LL * 256 * num_sms() ? N : 6LL * 256 * num_sms()); };
+        const int shapes[4][2] = {{3 * H, H}, {H, H}, {I, H}, {H, I}};
+        for (const auto& sh : shapes) {
+            if (sh[0] <= 0 || sh[1] <= 0) continue;
+            const int splits = max_splits(gemm_tiles(sh[0], sh[1]), R);
+            if (splits > 1) up(static_cast<long long>(splits) * sh[0] * sh[1] * 4);
+        }
+        long long last_tiles = -1;
+        int splits = 1;
+        for (int v = 16; v <= (vocab + 15) / 16 * 16; v += 16) {
+            const long long t = gemm_tiles(v, H);
+            if (t != last_tiles) { splits = max_splits(t, R); last_tiles = t; }
+            if (splits > 1) up(static_cast<long long>(splits) * v * H * 4);
+        }
+        up(colsum_bound((vocab + 15) / 16 * 16));
+        up(colsum_bound(I > 3 * H ? I : 3 * H));
+        up(ln_bwd_det_bytes(R, H));
+        up(embed_bwd_det_bytes(1, R, 0, H, -1));   // 3 items per row: at least as many as any split of `rows` into text and regions
+    }
+    return align256(need);
+}
+
 }  // namespace vb
 
 extern "C" {
+int64_t vb_deterministic_workspace_bytes(int64_t rows, int32_t hidden, int32_t inter, int32_t vocab, int32_t adam_chunks) {
+    if (rows < 0 || hidden < 0 || inter < 0 || vocab < 0 || adam_chunks < 0 || (rows > 0 && hidden % 8 != 0)) {
+        vb::set_error("vb_deterministic_workspace_bytes: bad shape (rows %lld, hidden %d, inter %d, vocab %d, adam_chunks %d)",
+                      static_cast<long long>(rows), hidden, inter, vocab, adam_chunks);
+        return -1;
+    }
+    return vb::deterministic_workspace_bytes(rows, hidden, inter, vocab, adam_chunks);
+}
 int vb_layer_fwd(const vb_layer_desc* d, const void* x_in, void* x_out, const vb_layer_acts* acts, void* stream) {
     return vb::layer_fwd(d, x_in, x_out, acts, static_cast<cudaStream_t>(stream));
 }

@@ -21,6 +21,11 @@ extern std::atomic<long long> g_launches;  // kernel launches issued by this lib
 int num_sms();      // SM count of the CALLER'S CURRENT device (cached per device)
 constexpr int kMaxDevices = 64;
 int current_device();  // cudaGetDevice, clamped to [0, kMaxDevices)
+// Deterministic reductions (vb_set_deterministic): the calling thread's workspace, ptr == nullptr when the mode is off.
+struct DetWs { void* ptr; long long bytes; };
+DetWs det_ws();
+// 0 when the mode is off or `need` bytes fit the workspace; else sets the error (naming the bytes) and returns 2
+int det_require(long long need, const char* what);
 // cudaFuncAttributeMaxDynamicSharedMemorySize is a per-device property of a kernel: `cache` is the caller's static
 // per-device record of the size already configured (DataParallel threads / several devices in one process).
 template <typename K>
@@ -85,6 +90,12 @@ void set_error(const char* fmt, ...);
             vb::set_error(__VA_ARGS__);                                                       \
             return 2;                                                                         \
         }                                                                                     \
+    } while (0)
+
+#define VB_TRY_RC(expr)      \
+    do {                     \
+        int _rc = (expr);    \
+        if (_rc) return _rc; \
     } while (0)
 
 // ---------------------------------------------------------------------------------------------

@@ -11,6 +11,8 @@
 //              projection's weight-gradient GEMM.
 //  mask_bias   (1 - cat(input_mask, image_mask)) * -10000                    (modeling.py:1417, 1286-1294)
 //  cast / colsum / fill helpers.
+#include <cub/device/device_radix_sort.cuh>
+
 #include "vb_internal.h"
 
 namespace vb {
@@ -232,8 +234,10 @@ __global__ void cast_bf16_f32_kernel(const bf16* __restrict__ src, float* __rest
 // iteration so every thread keeps 4 x 16 B loads in flight (the kernel is pure HBM streaming). The rows are swept from the
 // LAST to the first: the tensor was just written by the previous kernel, whose tiles run in increasing row order, so its tail
 // is what the L2 still holds.
-__global__ void __launch_bounds__(256)
-colsum_kernel(const bf16* __restrict__ x, long long ld, float* __restrict__ out, int M, int N) {
+// PART = true (deterministic mode): out is the workspace and block row y STORES its sums to out[y * N + col]; partials_reduce
+// adds them in blockIdx.y order.
+template <bool PART>
+__device__ __forceinline__ void colsum_body(const bf16* __restrict__ x, long long ld, float* __restrict__ out, int M, int N) {
     __shared__ float red[8][32][9];
     const int ch = blockIdx.x * 32 + threadIdx.x;
     pdl_trigger();
@@ -267,9 +271,184 @@ colsum_kernel(const bf16* __restrict__ x, long long ld, float* __restrict__ out,
             float s = 0.f;
 #pragma unroll
             for (int y = 0; y < 8; ++y) s += red[y][threadIdx.x][i];
-            atomicAdd(out + ch * 8 + i, s);
+            if constexpr (PART) out[static_cast<long long>(blockIdx.y) * N + ch * 8 + i] = s;
+            else atomicAdd(out + ch * 8 + i, s);
         }
     }
+}
+__global__ void __launch_bounds__(256)
+colsum_kernel(const bf16* __restrict__ x, long long ld, float* __restrict__ out, int M, int N) { colsum_body<false>(x, ld, out, M, N); }
+__global__ void __launch_bounds__(256)
+colsum_part_kernel(const bf16* __restrict__ x, long long ld, float* __restrict__ out, int M, int N) { colsum_body<true>(x, ld, out, M, N); }
+
+// ---- embedding backward in deterministic mode --------------------------------------------------------------------------------
+// Every table row the backward adds into is a KEY in one key space: word rows [0, vocab), position rows [vocab, + max_pos), text
+// types [.., + n_types), visual position 0 (one key), visual types [.., + n_types). Each text row contributes three (key, row)
+// items (word, position, type), each visual row two (visual position 0, visual type), listed in row order. A stable radix sort
+// by key makes every key's items one run, in row order. The run sums are then formed in a fixed association: the sorted items
+// are cut into windows of kSegWin; embed_seg_kernel sums each run's items inside a window in order and adds a run that lies
+// inside one window straight into its table row (no other writer has that key), or stores the partial of a run that crosses a
+// window edge (its head part in a window it did not start in, its tail part in the window it started in); embed_seg_join_kernel
+// adds those partials in window order for the window a crossing run started in, and adds the sum into the table row once.
+constexpr int kSegWin = 64;
+
+__device__ __forceinline__ float* embed_key_row(const EmbedBwdParams& p, unsigned k) {
+    const long long H = p.H;
+    if (k < static_cast<unsigned>(p.vocab)) return p.dword + k * H;
+    k -= p.vocab;
+    if (k < static_cast<unsigned>(p.max_pos)) return p.dpos + k * H;
+    k -= p.max_pos;
+    if (k < static_cast<unsigned>(p.n_types)) return p.dtype + k * H;
+    k -= p.n_types;
+    if (k == 0) return p.dpos_vis;
+    return p.dtype_vis + (k - 1) * H;
+}
+
+// one thread per row of de: its (key, row) items; the visual rows are also copied to dvis (the projection's weight-gradient input)
+__global__ void __launch_bounds__(256) embed_keys_kernel(const EmbedBwdParams p, unsigned* __restrict__ keys, int* __restrict__ vals) {
+    const int S = p.T + p.V;
+    const long long row = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
+    if (row >= static_cast<long long>(p.B) * S) return;
+    const int b = static_cast<int>(row / S), s = static_cast<int>(row % S);
+    const unsigned kpos = p.vocab, ktype = kpos + p.max_pos, kvpos = ktype + p.n_types;
+    if (s < p.T) {
+        const long long i = (static_cast<long long>(b) * p.T + s) * 3, t = static_cast<long long>(b) * p.T + s;
+        keys[i] = clampi(p.ids[t], p.vocab);
+        keys[i + 1] = kpos + (s < p.max_pos ? s : p.max_pos - 1);
+        keys[i + 2] = ktype + clampi(p.tt[t], p.n_types);
+        vals[i] = vals[i + 1] = vals[i + 2] = static_cast<int>(row);
+    } else {
+        const long long t = static_cast<long long>(b) * p.V + (s - p.T), i = 3LL * p.B * p.T + 2 * t;
+        keys[i] = kvpos;
+        keys[i + 1] = kvpos + 1 + clampi(p.vt[t], p.n_types);
+        vals[i] = vals[i + 1] = static_cast<int>(row);
+    }
+}
+
+__global__ void __launch_bounds__(256) embed_vis_copy_kernel(const EmbedBwdParams p) {
+    const int S = p.T + p.V, c8 = p.H / 8;
+    const long long n = static_cast<long long>(p.B) * p.V * c8;
+    for (long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x; i < n; i += static_cast<long long>(gridDim.x) * blockDim.x) {
+        const long long r = i / c8, c = i - r * c8;
+        const long long b = r / p.V, v = r - b * p.V;
+        stg_v4(p.dvis + r * p.H + c * 8, ldg_v4(p.de + (b * S + p.T + v) * p.H + c * 8));
+    }
+}
+
+template <int NC>
+__device__ __forceinline__ void seg_add_row(const EmbedBwdParams& p, int row, int lane, float (&acc)[NC][8]) {
+#pragma unroll
+    for (int c = 0; c < NC; ++c) {
+        const int ch = lane + c * 32;
+        if (ch < p.H / 8) {
+            const uint4 u = ldg_v4(p.de + static_cast<long long>(row) * p.H + ch * 8);
+            const float2 x0 = unpack_bf16x2(u.x), x1 = unpack_bf16x2(u.y), x2 = unpack_bf16x2(u.z), x3 = unpack_bf16x2(u.w);
+            acc[c][0] += x0.x; acc[c][1] += x0.y; acc[c][2] += x1.x; acc[c][3] += x1.y;
+            acc[c][4] += x2.x; acc[c][5] += x2.y; acc[c][6] += x3.x; acc[c][7] += x3.y;
+        }
+    }
+}
+template <int NC>
+__device__ __forceinline__ void seg_flush(float* dst, bool add, int H, int lane, float (&acc)[NC][8]) {
+#pragma unroll
+    for (int c = 0; c < NC; ++c) {
+        const int ch = lane + c * 32;
+        if (ch < H / 8) {
+            float4* d = reinterpret_cast<float4*>(dst + ch * 8);
+            float4 a0 = make_float4(acc[c][0], acc[c][1], acc[c][2], acc[c][3]), a1 = make_float4(acc[c][4], acc[c][5], acc[c][6], acc[c][7]);
+            if (add) {
+                const float4 o0 = d[0], o1 = d[1];
+                a0.x += o0.x; a0.y += o0.y; a0.z += o0.z; a0.w += o0.w;
+                a1.x += o1.x; a1.y += o1.y; a1.z += o1.z; a1.w += o1.w;
+            }
+            d[0] = a0; d[1] = a1;
+        }
+#pragma unroll
+        for (int i = 0; i < 8; ++i) acc[c][i] = 0.f;
+    }
+}
+
+// one warp per window; slots: [2][windows][H] fp32 (0: head partials, 1: tail partials)
+template <int NC>
+__global__ void __launch_bounds__(kEmbWarps * 32)
+embed_seg_kernel(const EmbedBwdParams p, const unsigned* __restrict__ keys, const int* __restrict__ vals, int n, float* __restrict__ slots) {
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const int w = blockIdx.x * kEmbWarps + warp, windows = (n + kSegWin - 1) / kSegWin;
+    if (w >= windows) return;
+    const int beg = w * kSegWin, end = min(beg + kSegWin, n);
+    const bool from_before = beg > 0 && keys[beg - 1] == keys[beg];
+    float acc[NC][8];
+#pragma unroll
+    for (int c = 0; c < NC; ++c)
+#pragma unroll
+        for (int i = 0; i < 8; ++i) acc[c][i] = 0.f;
+    int run_beg = beg;
+    for (int i = beg; i < end; ++i) {
+        const unsigned k = keys[i];
+        seg_add_row<NC>(p, vals[i], lane, acc);
+        const bool run_end = i + 1 == n || keys[i + 1] != k;
+        if (run_end || i + 1 == end) {
+            const bool head = run_beg == beg && from_before;
+            if (head) seg_flush<NC>(slots + static_cast<long long>(w) * p.H, false, p.H, lane, acc);
+            else if (!run_end) seg_flush<NC>(slots + (static_cast<long long>(windows) + w) * p.H, false, p.H, lane, acc);
+            else seg_flush<NC>(embed_key_row(p, k), true, p.H, lane, acc);
+            run_beg = i + 1;
+        }
+    }
+}
+
+// one warp per window: the window a crossing run started in adds its tail partial and the head partials of the following windows
+template <int NC>
+__global__ void __launch_bounds__(kEmbWarps * 32)
+embed_seg_join_kernel(const EmbedBwdParams p, const unsigned* __restrict__ keys, int n, const float* __restrict__ slots) {
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const int w = blockIdx.x * kEmbWarps + warp, windows = (n + kSegWin - 1) / kSegWin;
+    if (w >= windows) return;
+    const int beg = w * kSegWin, end = min(beg + kSegWin, n);
+    const unsigned k = keys[end - 1];
+    const bool starts_here = !(beg > 0 && keys[beg - 1] == k && keys[beg] == k);
+    if (!starts_here || end == n || keys[end] != k) return;
+    float acc[NC][8];
+#pragma unroll
+    for (int c = 0; c < NC; ++c)
+#pragma unroll
+        for (int i = 0; i < 8; ++i) acc[c][i] = 0.f;
+    auto add_slot = [&](const float* src) {
+#pragma unroll
+        for (int c = 0; c < NC; ++c) {
+            const int ch = lane + c * 32;
+            if (ch < p.H / 8) {
+                const float4 a = *reinterpret_cast<const float4*>(src + ch * 8), b = *reinterpret_cast<const float4*>(src + ch * 8 + 4);
+                acc[c][0] += a.x; acc[c][1] += a.y; acc[c][2] += a.z; acc[c][3] += a.w;
+                acc[c][4] += b.x; acc[c][5] += b.y; acc[c][6] += b.z; acc[c][7] += b.w;
+            }
+        }
+    };
+    add_slot(slots + (static_cast<long long>(windows) + w) * p.H);
+    for (int w2 = w + 1; w2 < windows; ++w2) {
+        add_slot(slots + static_cast<long long>(w2) * p.H);
+        const int e2 = min((w2 + 1) * kSegWin, n);
+        if (e2 == n || keys[e2] != k) break;
+    }
+    seg_flush<NC>(embed_key_row(p, k), true, p.H, lane, acc);
+}
+
+static long long embed_items(int B, int T, int V) { return 3LL * B * T + 2LL * B * V; }
+static long long al256(long long x) { return (x + 255) / 256 * 256; }
+long long embed_sort_temp_bytes(int B, int T, int V) {
+    size_t bytes = 0;
+    cub::DoubleBuffer<unsigned> k(nullptr, nullptr);
+    cub::DoubleBuffer<int> v(nullptr, nullptr);
+    if (cub::DeviceRadixSort::SortPairs(nullptr, bytes, k, v, static_cast<int>(embed_items(B, T, V)), 0, 32) != cudaSuccess) return -1;
+    return static_cast<long long>(bytes);
+}
+// workspace layout: keys[2][n] (u32), vals[2][n] (i32), slots [2][windows][H] fp32, sort temp. sort_temp < 0: a bound on the sort's
+// temporary storage (32 bytes per item + 1 MB, several times what the radix sort takes) for vb_deterministic_workspace_bytes,
+// which must work without a device
+long long embed_bwd_det_bytes(int B, int T, int V, int H, long long sort_temp) {
+    const long long n = embed_items(B, T, V), windows = (n + kSegWin - 1) / kSegWin;
+    if (sort_temp < 0) sort_temp = 32 * n + (1 << 20);
+    return 4 * al256(4 * n) + al256(2 * windows * H * 4) + al256(sort_temp);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -293,10 +472,63 @@ int embed_fwd(const EmbedParams& p, cudaStream_t st) {
     return 0;
 }
 
+static int embed_bwd_det(const EmbedBwdParams& p, const DetWs& det, cudaStream_t st) {
+    VB_REQUIRE(((reinterpret_cast<uintptr_t>(p.dtype) | reinterpret_cast<uintptr_t>(p.dpos_vis) | reinterpret_cast<uintptr_t>(p.dtype_vis)) & 15) == 0,
+               "embed backward: gradient tables must be 16-byte aligned");
+    const long long n = embed_items(p.B, p.T, p.V), windows = (n + kSegWin - 1) / kSegWin;
+    VB_REQUIRE(n < (1LL << 31) && static_cast<long long>(p.vocab) + p.max_pos + 2LL * p.n_types + 1 < (1LL << 32),
+               "embed backward: too many rows / table rows for deterministic mode");
+    const long long temp = embed_sort_temp_bytes(p.B, p.T, p.V);
+    VB_REQUIRE(temp >= 0, "embed backward: radix sort size query failed");
+    VB_TRY_RC(det_require(embed_bwd_det_bytes(p.B, p.T, p.V, p.H, temp), "embed backward"));
+    char* ws = static_cast<char*>(det.ptr);
+    unsigned* k0 = reinterpret_cast<unsigned*>(ws);
+    unsigned* k1 = reinterpret_cast<unsigned*>(ws + al256(4 * n));
+    int* v0 = reinterpret_cast<int*>(ws + 2 * al256(4 * n));
+    int* v1 = reinterpret_cast<int*>(ws + 3 * al256(4 * n));
+    float* slots = reinterpret_cast<float*>(ws + 4 * al256(4 * n));
+    void* sort_temp = ws + 4 * al256(4 * n) + al256(2 * windows * p.H * 4);
+    const long long rows = static_cast<long long>(p.B) * (p.T + p.V);
+    const unsigned max_key = static_cast<unsigned>(p.vocab + p.max_pos + 2 * p.n_types);
+    int end_bit = 1;
+    while (end_bit < 32 && (max_key >> end_bit) != 0) ++end_bit;
+    const int nc = (p.H / 8 + 31) / 32;
+    const int seg_grid = static_cast<int>((windows + kEmbWarps - 1) / kEmbWarps);
+    ProfScope ps(st, PROF_EMBED, 6.0 * rows * p.H, 5);
+    embed_keys_kernel<<<static_cast<int>((rows + 255) / 256), 256, 0, st>>>(p, k0, v0);
+    VB_CHECK_CUDA(cudaGetLastError());
+    if (p.V > 0) {
+        long long blocks = (static_cast<long long>(p.B) * p.V * (p.H / 8) + 255) / 256;
+        if (blocks > num_sms() * 8) blocks = num_sms() * 8;
+        embed_vis_copy_kernel<<<static_cast<int>(blocks), 256, 0, st>>>(p);
+        VB_CHECK_CUDA(cudaGetLastError());
+    }
+    cub::DoubleBuffer<unsigned> kb(k0, k1);
+    cub::DoubleBuffer<int> vb(v0, v1);
+    size_t tb = static_cast<size_t>(temp);
+    VB_CHECK_CUDA(cub::DeviceRadixSort::SortPairs(sort_temp, tb, kb, vb, static_cast<int>(n), 0, end_bit, st));
+    const unsigned* keys = kb.Current();
+    const int* vals = vb.Current();
+#define VB_SEG(NC)                                                                                                        \
+    embed_seg_kernel<NC><<<seg_grid, kEmbWarps * 32, 0, st>>>(p, keys, vals, static_cast<int>(n), slots);                \
+    embed_seg_join_kernel<NC><<<seg_grid, kEmbWarps * 32, 0, st>>>(p, keys, static_cast<int>(n), slots)
+    switch (nc) {
+        case 1: VB_SEG(1); break;
+        case 2: VB_SEG(2); break;
+        case 3: VB_SEG(3); break;
+        default: VB_SEG(4); break;
+    }
+#undef VB_SEG
+    VB_CHECK_CUDA(cudaGetLastError());
+    return 0;
+}
+
 int embed_bwd(const EmbedBwdParams& p, cudaStream_t st) {
     VB_REQUIRE(p.H % 8 == 0 && p.H <= 1024, "embed backward: H=%d must be a multiple of 8 and <= 1024", p.H);
     VB_REQUIRE((reinterpret_cast<uintptr_t>(p.dword) & 15) == 0 && (reinterpret_cast<uintptr_t>(p.dpos) & 15) == 0,
                "embed backward: gradient tables must be 16-byte aligned");
+    const DetWs det = det_ws();
+    if (det.ptr != nullptr) return embed_bwd_det(p, det, st);
     const long long rows = static_cast<long long>(p.B) * (p.T + p.V);
     const int cb = p.B < 32 ? p.B : 32, nb = (p.B + cb - 1) / cb;   // a warp task: one sequence position, up to 32 examples
     const long long tasks = static_cast<long long>(p.T + p.V) * nb;
@@ -357,12 +589,30 @@ int cast_bf16_f32(const void* src, float* dst, long long n, cudaStream_t st) {
     return 0;
 }
 
-int colsum(const void* x, long long ld, float* out, int M, int N, cudaStream_t st) {
-    VB_REQUIRE(N % 8 == 0 && M > 0, "colsum: bad shape");
+static int colsum_gy(int M, int N) {
     const int gx = (N / 8 + 31) / 32;
     int gy = (num_sms() * 6) / gx;
     if (gy < 1) gy = 1;
     if (gy > (M + 7) / 8) gy = (M + 7) / 8;
+    return gy;
+}
+long long colsum_det_bytes(int M, int N) { return static_cast<long long>(colsum_gy(M, N)) * N * 4; }
+
+int colsum(const void* x, long long ld, float* out, int M, int N, cudaStream_t st) {
+    VB_REQUIRE(N % 8 == 0 && M > 0, "colsum: bad shape");
+    const int gx = (N / 8 + 31) / 32;
+    const int gy = colsum_gy(M, N);
+    const DetWs det = det_ws();
+    if (det.ptr != nullptr) {
+        VB_TRY_RC(det_require(colsum_det_bytes(M, N), "colsum"));
+        {
+            ProfScope ps(st, PROF_COLSUM, 2.0 * M * N, 1);
+            VB_CHECK_CUDA(launch_pdl(colsum_part_kernel, dim3(gx, gy), dim3(32, 8), 0, st, static_cast<const bf16*>(x), ld,
+                                     static_cast<float*>(det.ptr), M, N));
+        }
+        VB_CHECK_CUDA(cudaGetLastError());
+        return partials_reduce(static_cast<const float*>(det.ptr), gy, N, N, out, nullptr, nullptr, st);
+    }
     {
         ProfScope ps(st, PROF_COLSUM, 2.0 * M * N, 1);
         VB_CHECK_CUDA(launch_pdl(colsum_kernel, dim3(gx, gy), dim3(32, 8), 0, st, static_cast<const bf16*>(x), ld, out, M, N));

@@ -41,6 +41,17 @@ void set_error(const char* fmt, ...) {
 }
 const char* get_error() { return g_err; }
 
+// ---- deterministic reductions: thread-local like the error message (the autograd engine runs backward on its own thread) ----
+static thread_local void* g_det_ptr = nullptr;
+static thread_local long long g_det_bytes = 0;
+DetWs det_ws() { return DetWs{g_det_ptr, g_det_bytes}; }
+int det_require(long long need, const char* what) {
+    VB_REQUIRE(g_det_ptr == nullptr || need <= g_det_bytes,
+               "%s: deterministic mode needs %lld bytes of workspace, %lld are set (vb_deterministic_workspace_bytes)", what, need,
+               g_det_bytes);
+    return 0;
+}
+
 // ---- live profiling -------------------------------------------------------------------------
 struct ProfRec { cudaEvent_t e0, e1; int cat; double work; int launches; };
 static bool g_prof_on = false;
@@ -171,8 +182,10 @@ __device__ __forceinline__ void store16_bf16(bf16* p, const float (&f)[16]) {
 // two whole heads — so the row-wise dot product with O needs no exchange; O is read like a residual operand.
 // EPI_GELU_ONLY (VB_EPI_GELU_FWD of the ABI): D = gelu(u) and nothing else — the forward-only FFN-up GEMM. It takes the plain
 // bf16 store path (one coalesced store per element) with the gelu of the two-tensor epilogues.
+// EPI_SLAB (fp32 output, deterministic mode): split s STORES its partial tile to slab s of the workspace, D = slab base with
+// ldd = N, slab s at D + s * M * N, no bias; splitk_reduce_kernel then adds bias + the slabs in split order into the real D.
 enum { EPI_GENERIC = 0, EPI_BIAS = 1, EPI_RESID = 2, EPI_DROP_RESID = 3, EPI_GELU_FWD = 4, EPI_DGELU_BWD = 5, EPI_GELU_FWD_T = 6,
-       EPI_DGELU_BWD_T = 7, EPI_DELTA = 8, EPI_GELU_ONLY = 9 };
+       EPI_DGELU_BWD_T = 7, EPI_DELTA = 8, EPI_GELU_ONLY = 9, EPI_SLAB = 10 };
 __host__ __device__ constexpr bool epi_is_gelu(int e) { return e == EPI_GELU_FWD || e == EPI_GELU_FWD_T; }
 __host__ __device__ constexpr bool epi_is_dgelu(int e) { return e == EPI_DGELU_BWD || e == EPI_DGELU_BWD_T; }
 
@@ -441,6 +454,10 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
                 epilogue16<OUT_F32, EPI, true>(p, row, col, sb, e, x, o0, o1);
                 stg_v8(reinterpret_cast<bf16*>(p.D) + gp_off(k), o0);
                 stg_v8(p.aux_out + static_cast<long long>(row) * p.ld_aux + col, o1);
+            } else if constexpr (EPI == EPI_SLAB) {
+                float* d = reinterpret_cast<float*>(p.D) + (static_cast<long long>(blockIdx.x / (m_blocks * n_blocks)) * p.M + row) * p.ldd + col;
+#pragma unroll
+                for (int i = 0; i < 4; ++i) *reinterpret_cast<float4*>(d + 4 * i) = make_float4(x[4 * i], x[4 * i + 1], x[4 * i + 2], x[4 * i + 3]);
             } else if constexpr (EPI == EPI_DELTA) {
                 uint32_t o0[8];
                 epilogue16<OUT_F32, EPI, true>(p, row, col, sb, e, x, o0);
@@ -578,7 +595,7 @@ static int launch(const CUtensorMap& ta, const CUtensorMap& tb, const GemmParams
 // tiles * splits CTAs fill whole waves of one CTA per SM. It minimises the time of the busiest SM in k-blocks, waves * (k-blocks
 // per split + kCtaCost), where kCtaCost stands for what every CTA pays besides its main loop (launch, first TMA round trip,
 // red.add of its partial tile); the smallest such factor wins.
-static int wgrad_splits(long long tiles, int k_blocks) {
+int wgrad_splits(long long tiles, int k_blocks) {
     constexpr int kCtaCost = 4;
     const long long sms = num_sms();
     int best = 1;
@@ -589,6 +606,35 @@ static int wgrad_splits(long long tiles, int k_blocks) {
     }
     return best;
 }
+
+// D[M, N] += bias + sum_s slab[s] (fp32, slab s at slab + s * M * N), four columns per thread, the splits added in order
+__global__ void __launch_bounds__(256)
+splitk_reduce_kernel(const float* __restrict__ slab, int splits, int M, int N, const float* __restrict__ bias, float* __restrict__ D,
+                     long long ldd) {
+    const long long n4 = static_cast<long long>(M) * N / 4, plane = static_cast<long long>(M) * N;
+    for (long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x; i < n4; i += static_cast<long long>(gridDim.x) * blockDim.x) {
+        const long long e = 4 * i;
+        const int row = static_cast<int>(e / N), col = static_cast<int>(e - static_cast<long long>(row) * N);
+        float4 a = *reinterpret_cast<const float4*>(slab + e);
+        if (bias != nullptr) { a.x += bias[col]; a.y += bias[col + 1]; a.z += bias[col + 2]; a.w += bias[col + 3]; }
+        for (int s = 1; s < splits; ++s) {
+            const float4 b = *reinterpret_cast<const float4*>(slab + s * plane + e);
+            a.x += b.x; a.y += b.y; a.z += b.z; a.w += b.w;
+        }
+        float4* d = reinterpret_cast<float4*>(D + static_cast<long long>(row) * ldd + col);
+        float4 o = *d;
+        o.x += a.x; o.y += a.y; o.z += a.z; o.w += a.w;
+        *d = o;
+    }
+}
+
+// BLOCK_N of a call: 256 unless N is small or padding N up to a multiple of 256 wastes more than 1/8 of the columns
+static bool use_bn256(int N) { return N >= 256 && ((N + 255) / 256 * 256 - N) * 8 <= N; }
+long long gemm_tiles(int M, int N) {
+    const bool bn256 = use_bn256(N);
+    return static_cast<long long>((M + BLOCK_M - 1) / BLOCK_M) * ((N + (bn256 ? 255 : 127)) / (bn256 ? 256 : 128));
+}
+int gemm_k_blocks(int K) { return (K + BLOCK_K - 1) / BLOCK_K; }
 
 bool gemm_delta_ok(int M, int N) {
     const int n_pad256 = (N + 255) / 256 * 256;
@@ -651,12 +697,19 @@ int gemm(const vb_gemm_args& a, cudaStream_t st) {
         p.drop_stream = a.dropout_stream;
     }
 
-    // BLOCK_N: 256 unless N is small or padding N up to a multiple of 256 wastes more than 1/8 of the columns
-    const int n_pad256 = (a.N + 255) / 256 * 256;
-    const bool bn256 = (a.N >= 256) && ((n_pad256 - a.N) * 8 <= a.N);
+    const bool bn256 = use_bn256(a.N);
     VB_REQUIRE(!a.delta_out || bn256, "vb_gemm: delta_out needs 256-wide tiles");
-    const long long tiles = static_cast<long long>((a.M + BLOCK_M - 1) / BLOCK_M) * ((a.N + (bn256 ? 255 : 127)) / (bn256 ? 256 : 128));
-    p.splits = a.d_fp32 ? wgrad_splits(tiles, (a.K + BLOCK_K - 1) / BLOCK_K) : 1;
+    p.splits = a.d_fp32 ? wgrad_splits(gemm_tiles(a.M, a.N), gemm_k_blocks(a.K)) : 1;
+    // Deterministic mode: the splits of an fp32 output store to their own slabs instead of red.add-ing one tile (one split is
+    // already one writer per element). Slab kernels exist for the weight-gradient layout (A and B MN-major); other layouts,
+    // and shapes whose slabs do not fit the workspace, lower the split factor to what fits, down to 1.
+    const DetWs det = det_ws();
+    if (a.d_fp32 && p.splits > 1 && det.ptr != nullptr) {
+        const long long plane = static_cast<long long>(a.M) * a.N * 4;
+        if (!(a.a_mn_major && a.b_mn_major)) p.splits = 1;
+        while (p.splits > 1 && p.splits * plane > det.bytes) --p.splits;
+    }
+    const bool slab = a.d_fp32 && p.splits > 1 && det.ptr != nullptr;
 
     CUtensorMap ta, tb;
     int rc;
@@ -667,6 +720,22 @@ int gemm(const vb_gemm_args& a, cudaStream_t st) {
     else               rc = make_tmap_bf16(&tb, a.B, a.N, a.K, a.ldb, BLOCK_K);
     if (rc) return rc;
 
+    if (slab) {
+        GemmParams q = p;
+        q.D = det.ptr; q.ldd = a.N; q.bias = nullptr;
+        const int rc2 = bn256 ? launch<true, true, 256, true, EPI_SLAB>(ta, tb, q, st) : launch<true, true, 128, true, EPI_SLAB>(ta, tb, q, st);
+        if (rc2) return rc2;
+        const long long n4 = static_cast<long long>(a.M) * a.N / 4;
+        long long blocks = (n4 + 255) / 256;
+        if (blocks > num_sms() * 8) blocks = num_sms() * 8;
+        {
+            ProfScope ps(st, PROF_GEMM_WGRAD, 0.0, 1);
+            splitk_reduce_kernel<<<static_cast<int>(blocks), 256, 0, st>>>(static_cast<const float*>(det.ptr), p.splits, a.M, a.N, a.bias,
+                                                                           static_cast<float*>(a.D), a.ldd);
+        }
+        VB_CHECK_CUDA(cudaGetLastError());
+        return 0;
+    }
     if (a.epilogue == VB_EPI_GELU_FWD)
         return bn256 ? launch<false, false, 256, false, EPI_GELU_ONLY>(ta, tb, p, st) : launch<false, false, 128, false, EPI_GELU_ONLY>(ta, tb, p, st);
     if (bn256 && !a.d_fp32) {
@@ -736,6 +805,16 @@ int vb_profile_read(double* ms, double* work, int64_t* launches) {
         vb::g_prof_pool.push_back(r);
     }
     vb::g_prof.clear();
+    return 0;
+}
+int vb_set_deterministic(void* workspace, int64_t bytes) {
+    if (workspace != nullptr && (bytes <= 0 || (reinterpret_cast<uintptr_t>(workspace) & 255) != 0)) {
+        vb::set_error("vb_set_deterministic: the workspace must be 256-byte aligned and bytes > 0 (got %p, %lld)", workspace,
+                      static_cast<long long>(bytes));
+        return 2;
+    }
+    vb::g_det_ptr = workspace;
+    vb::g_det_bytes = workspace != nullptr ? bytes : 0;
     return 0;
 }
 int vb_gemm_delta_ok(int32_t M, int32_t N) { return vb::gemm_delta_ok(M, N) ? 1 : 0; }

@@ -33,6 +33,15 @@ int attn_bwd_varlen(const void* qkv, const int* cu_seqlens, const void* ctx, con
 long long attn_keep_bytes(int B, int S, int A);
 // the pre-dropout attention maps softmax(QK^T / 8 + mask_bias) of a dense call, fp32 [B, A, S, S] (vb_attention_probs.cu)
 int attn_probs(const void* qkv, const float* mask_bias, float* probs, int B, int S, int A, int H, cudaStream_t st);
+// deterministic mode (vb_set_deterministic; see vb_common.cuh det_ws)
+int wgrad_splits(long long tiles, int k_blocks);   // split-K factor of an fp32 output (vb_gemm.cu)
+long long gemm_tiles(int M, int N);
+int gemm_k_blocks(int K);
+long long ln_bwd_det_bytes(int rows, int H);       // workspace of one ln_bwd call in deterministic mode
+long long colsum_det_bytes(int M, int N);          // ... of one colsum call
+long long embed_bwd_det_bytes(int B, int T, int V, int H, long long sort_temp);   // ... of embed_bwd (sort_temp < 0: a bound)
+long long embed_sort_temp_bytes(int B, int T, int V);
+int partials_reduce(const float* part, int parts, int width, int seg, float* o0, float* o1, float* o2, cudaStream_t st);
 int colsum(const void* x, long long ld, float* out, int M, int N, cudaStream_t st);
 int cast_f32_bf16(const float* src, void* dst, long long n, cudaStream_t st);
 int cast_bf16_f32(const void* src, float* dst, long long n, cudaStream_t st);

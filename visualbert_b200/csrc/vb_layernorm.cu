@@ -100,14 +100,16 @@ __device__ __forceinline__ uint4 pack8(const float (&f)[8]) {
 // float4 slot of (array a, chunk ch, half h) inside a slab of `chunks` chunks: lanes -> consecutive 16 B
 __device__ __forceinline__ int slot(int a, int h, int ch, int chunks) { return (a * 2 + h) * chunks + ch; }
 
-template <int NC>
-__global__ void __launch_bounds__(kLnWarps * 32, 2)
-ln_bwd_kernel(const bf16* __restrict__ dy, const bf16* __restrict__ x, const float* __restrict__ mean,
-              const float* __restrict__ rstd, const float* __restrict__ gamma, bf16* __restrict__ dx,
-              bf16* __restrict__ dx_drop, float* __restrict__ dgamma, float* __restrict__ dbeta,
-              float* __restrict__ dbias, int rows, int H, float drop_scale, unsigned drop_thresh16,
-              unsigned long long drop_seed, unsigned drop_stream, float in_scale, unsigned in_thresh16,
-              unsigned in_stream) {
+// PART = false: the block's column sums go to dgamma / dbeta / dbias by atomicAdd. PART = true (deterministic mode): dgamma is
+// the workspace and block b STORES its sums to dgamma[(b * 3 + array) * H + col]; partials_reduce adds them in block order.
+template <int NC, bool PART>
+__device__ __forceinline__ void
+ln_bwd_body(const bf16* __restrict__ dy, const bf16* __restrict__ x, const float* __restrict__ mean,
+            const float* __restrict__ rstd, const float* __restrict__ gamma, bf16* __restrict__ dx,
+            bf16* __restrict__ dx_drop, float* __restrict__ dgamma, float* __restrict__ dbeta,
+            float* __restrict__ dbias, int rows, int H, float drop_scale, unsigned drop_thresh16,
+            unsigned long long drop_seed, unsigned drop_stream, float in_scale, unsigned in_thresh16,
+            unsigned in_stream) {
     extern __shared__ float4 sm4[];  // [gamma: 2*chunks] [warp][3 arrays][2 halves][chunks]
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int chunks = H >> 3;
@@ -221,10 +223,59 @@ ln_bwd_kernel(const bf16* __restrict__ dy, const bf16* __restrict__ x, const flo
         float s = 0.f;
 #pragma unroll
         for (int w = 0; w < kLnWarps; ++w) s += accf[(w * 6 * chunks + slot(a, h, ch, chunks)) * 4 + e];
-        float* dst = a == 0 ? dgamma : (a == 1 ? dbeta : dbias);
-        if (dst != nullptr) atomicAdd(dst + col, s);
+        if constexpr (PART) {
+            dgamma[static_cast<long long>(blockIdx.x) * 3 * H + i] = s;
+        } else {
+            float* dst = a == 0 ? dgamma : (a == 1 ? dbeta : dbias);
+            if (dst != nullptr) atomicAdd(dst + col, s);
+        }
     }
 }
+
+#define VB_LN_BWD_PARAMS                                                                                                       \
+    const bf16 *__restrict__ dy, const bf16 *__restrict__ x, const float *__restrict__ mean, const float *__restrict__ rstd,   \
+        const float *__restrict__ gamma, bf16 *__restrict__ dx, bf16 *__restrict__ dx_drop, float *__restrict__ dgamma,        \
+        float *__restrict__ dbeta, float *__restrict__ dbias, int rows, int H, float drop_scale, unsigned drop_thresh16,      \
+        unsigned long long drop_seed, unsigned drop_stream, float in_scale, unsigned in_thresh16, unsigned in_stream
+#define VB_LN_BWD_ARGS \
+    dy, x, mean, rstd, gamma, dx, dx_drop, dgamma, dbeta, dbias, rows, H, drop_scale, drop_thresh16, drop_seed, drop_stream, in_scale, in_thresh16, in_stream
+template <int NC>
+__global__ void __launch_bounds__(kLnWarps * 32, 2) ln_bwd_kernel(VB_LN_BWD_PARAMS) { ln_bwd_body<NC, false>(VB_LN_BWD_ARGS); }
+template <int NC>
+__global__ void __launch_bounds__(kLnWarps * 32, 2) ln_bwd_part_kernel(VB_LN_BWD_PARAMS) { ln_bwd_body<NC, true>(VB_LN_BWD_ARGS); }
+#undef VB_LN_BWD_PARAMS
+#undef VB_LN_BWD_ARGS
+
+// out_j[i % seg] += sum_p part[p * width + i] for i in [0, width), j = i / seg (null outputs are skipped): the block partials of a
+// deterministic-mode column reduction, added in partial order. One thread per column; consecutive threads read consecutive columns.
+__global__ void __launch_bounds__(256)
+partials_reduce_kernel(const float* __restrict__ part, int parts, int width, int seg, float* o0, float* o1, float* o2) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= width) return;
+    float s = 0.f;
+    for (int p = 0; p < parts; ++p) s += part[static_cast<long long>(p) * width + i];
+    const int j = i / seg;
+    float* o = j == 0 ? o0 : (j == 1 ? o1 : o2);
+    if (o != nullptr) o[i - j * seg] += s;
+}
+
+int partials_reduce(const float* part, int parts, int width, int seg, float* o0, float* o1, float* o2, cudaStream_t st) {
+    {
+        ProfScope ps(st, PROF_COLSUM, 4.0 * parts * width, 1);
+        partials_reduce_kernel<<<(width + 255) / 256, 256, 0, st>>>(part, parts, width, seg, o0, o1, o2);
+    }
+    VB_CHECK_CUDA(cudaGetLastError());
+    return 0;
+}
+
+// grid of ln_bwd: 2 resident blocks per SM (123 registers: the row is cached in fp32; an 80-register / 3-block build spills and
+// measured 30 % slower), fewer when there are fewer row groups
+static int ln_bwd_grid(int rows) {
+    int grid = num_sms() * 2;
+    const int need = (rows + kLnWarps - 1) / kLnWarps;
+    return grid > need ? need : grid;
+}
+long long ln_bwd_det_bytes(int rows, int H) { return static_cast<long long>(ln_bwd_grid(rows)) * 3 * H * 4; }
 
 int ln_fwd(const void* x, long long ldx, const float* gamma, const float* beta, void* y, long long ldy,
            float* mean, float* rstd, int rows, int H, float eps, cudaStream_t st) {
@@ -256,11 +307,9 @@ int ln_bwd(const void* dy, const void* x, const float* mean, const float* rstd, 
     VB_REQUIRE(rows > 0, "layernorm backward: no rows");
     VB_REQUIRE((dropout_p > 0.f) == (dx_drop != nullptr), "layernorm backward: dx_drop iff dropout_p > 0");
     const int nc = (H / 8 + 31) / 32;
-    // 2 resident blocks per SM (123 registers: the row is cached in fp32; an 80-register / 3-block build spills and
-    // measured 30 % slower)
-    int grid = num_sms() * 2;
-    const int need = (rows + kLnWarps - 1) / kLnWarps;
-    if (grid > need) grid = need;
+    const int grid = ln_bwd_grid(rows);
+    const DetWs det = det_ws();
+    if (det.ptr != nullptr) VB_TRY_RC(det_require(ln_bwd_det_bytes(rows, H), "layernorm backward"));
     const DropQ dq = dropout_quantise(dropout_p), iq = dropout_quantise(in_dropout_p);
     const float scale = dq.scale, in_scale = iq.scale;
     const unsigned th = dq.thr8, in_th = iq.thr8;
@@ -270,20 +319,40 @@ int ln_bwd(const void* dy, const void* x, const float* mean, const float* rstd, 
     VB_CHECK_CUDA(ensure_dyn_smem(ln_bwd_kernel<2>, 100 * 1024, cfg2));
     VB_CHECK_CUDA(ensure_dyn_smem(ln_bwd_kernel<3>, 100 * 1024, cfg3));
     VB_CHECK_CUDA(ensure_dyn_smem(ln_bwd_kernel<4>, 100 * 1024, cfg4));
-    ProfScope ps(st, PROF_LN_BWD, (dx_drop ? 8.0 : 6.0) * rows * H, 1);
-#define VB_LN_BWD(NC)                                                                                        \
-    VB_CHECK_CUDA(launch_pdl(ln_bwd_kernel<NC>, dim3(grid), dim3(kLnWarps * 32), smem, st,                  \
-        static_cast<const bf16*>(dy), static_cast<const bf16*>(x), mean, rstd, gamma, static_cast<bf16*>(dx), \
-        static_cast<bf16*>(dx_drop), dgamma, dbeta, dbias, rows, H, scale, th, seed, stream_id, in_scale,    \
-        in_th, in_stream_id))
-    switch (nc) {
-        case 1: VB_LN_BWD(1); break;
-        case 2: VB_LN_BWD(2); break;
-        case 3: VB_LN_BWD(3); break;
-        default: VB_LN_BWD(4); break;
+    if (det.ptr != nullptr) {
+        static int dcfg1[kMaxDevices] = {0}, dcfg2[kMaxDevices] = {0}, dcfg3[kMaxDevices] = {0}, dcfg4[kMaxDevices] = {0};
+        VB_CHECK_CUDA(ensure_dyn_smem(ln_bwd_part_kernel<1>, 100 * 1024, dcfg1));
+        VB_CHECK_CUDA(ensure_dyn_smem(ln_bwd_part_kernel<2>, 100 * 1024, dcfg2));
+        VB_CHECK_CUDA(ensure_dyn_smem(ln_bwd_part_kernel<3>, 100 * 1024, dcfg3));
+        VB_CHECK_CUDA(ensure_dyn_smem(ln_bwd_part_kernel<4>, 100 * 1024, dcfg4));
     }
+    {
+        ProfScope ps(st, PROF_LN_BWD, (dx_drop ? 8.0 : 6.0) * rows * H, 1);
+#define VB_LN_BWD(K, NC, DG)                                                                                 \
+    VB_CHECK_CUDA(launch_pdl(K<NC>, dim3(grid), dim3(kLnWarps * 32), smem, st,                              \
+        static_cast<const bf16*>(dy), static_cast<const bf16*>(x), mean, rstd, gamma, static_cast<bf16*>(dx), \
+        static_cast<bf16*>(dx_drop), DG, dbeta, dbias, rows, H, scale, th, seed, stream_id, in_scale,        \
+        in_th, in_stream_id))
+        if (det.ptr != nullptr) {
+            float* part = static_cast<float*>(det.ptr);
+            switch (nc) {
+                case 1: VB_LN_BWD(ln_bwd_part_kernel, 1, part); break;
+                case 2: VB_LN_BWD(ln_bwd_part_kernel, 2, part); break;
+                case 3: VB_LN_BWD(ln_bwd_part_kernel, 3, part); break;
+                default: VB_LN_BWD(ln_bwd_part_kernel, 4, part); break;
+            }
+        } else {
+            switch (nc) {
+                case 1: VB_LN_BWD(ln_bwd_kernel, 1, dgamma); break;
+                case 2: VB_LN_BWD(ln_bwd_kernel, 2, dgamma); break;
+                case 3: VB_LN_BWD(ln_bwd_kernel, 3, dgamma); break;
+                default: VB_LN_BWD(ln_bwd_kernel, 4, dgamma); break;
+            }
+        }
 #undef VB_LN_BWD
+    }
     VB_CHECK_CUDA(cudaGetLastError());
+    if (det.ptr != nullptr) return partials_reduce(static_cast<const float*>(det.ptr), grid, 3 * H, H, dgamma, dbeta, dbias, st);
     return 0;
 }
 

@@ -23,8 +23,10 @@ __device__ __forceinline__ int find_tensor(const vb_adam_tensor* __restrict__ ta
     return lo;
 }
 
-__global__ void __launch_bounds__(kAdamThreads)
-adam_sumsq_kernel(const vb_adam_tensor* __restrict__ tab, int n_tensors, float* __restrict__ sumsq) {
+// PART = false: the chunk's sum of squares is atomically added to sumsq[tensor]. PART = true (deterministic mode): it is stored
+// to sumsq[chunk] (the workspace), and adam_update_ordered_kernel adds a tensor's chunk sums in chunk order.
+template <bool PART>
+__device__ __forceinline__ void adam_sumsq_body(const vb_adam_tensor* __restrict__ tab, int n_tensors, float* __restrict__ sumsq) {
     __shared__ float sh[kAdamThreads / 32];
     const int t = find_tensor(tab, n_tensors, blockIdx.x);
     const vb_adam_tensor e = tab[t];
@@ -49,9 +51,14 @@ adam_sumsq_kernel(const vb_adam_tensor* __restrict__ tab, int n_tensors, float* 
         float r = 0.f;
 #pragma unroll
         for (int i = 0; i < kAdamThreads / 32; ++i) r += sh[i];
-        atomicAdd(sumsq + t, r);
+        if constexpr (PART) sumsq[blockIdx.x] = r;
+        else atomicAdd(sumsq + t, r);
     }
 }
+__global__ void __launch_bounds__(kAdamThreads)
+adam_sumsq_kernel(const vb_adam_tensor* __restrict__ tab, int n_tensors, float* __restrict__ sumsq) { adam_sumsq_body<false>(tab, n_tensors, sumsq); }
+__global__ void __launch_bounds__(kAdamThreads)
+adam_sumsq_part_kernel(const vb_adam_tensor* __restrict__ tab, int n_tensors, float* __restrict__ part) { adam_sumsq_body<true>(tab, n_tensors, part); }
 
 struct AdamHyper { float b1, one_minus_b1, b2, one_minus_b2, eps, max_grad_norm; };
 
@@ -65,16 +72,33 @@ __device__ __forceinline__ void adam_elem(float& p, float g, float& m, float& v,
     p -= lr * upd;
 }
 
-__global__ void __launch_bounds__(kAdamThreads)
-adam_update_kernel(const vb_adam_tensor* __restrict__ tab, int n_tensors, const float* __restrict__ sumsq,
-                   const AdamHyper h) {
+// ORDERED = false: sumsq[t] is the tensor's sum of squares. ORDERED = true: sumsq holds one partial per chunk, and every CTA of
+// the tensor sums them in the same fixed order (thread i takes chunks i, i + 256, ... in order, then a fixed reduction tree).
+template <bool ORDERED>
+__device__ __forceinline__ void adam_update_body(const vb_adam_tensor* __restrict__ tab, int n_tensors, const float* __restrict__ sumsq,
+                                                 const AdamHyper& h) {
     const int t = find_tensor(tab, n_tensors, blockIdx.x);
     const vb_adam_tensor e = tab[t];
     const long long begin = static_cast<long long>(blockIdx.x - e.first_chunk) * kAdamChunk;
     const long long end = min(begin + kAdamChunk, static_cast<long long>(e.numel));
     float coef = 1.f;
     if (h.max_grad_norm > 0.f) {  // torch.nn.utils.clip_grad_norm_: coef = max_norm / (total_norm + 1e-6), applied if < 1
-        const float c = h.max_grad_norm / (sqrtf(sumsq[t]) + 1e-6f);
+        float ss;
+        if constexpr (ORDERED) {
+            __shared__ float sh[kAdamThreads / 32];
+            const int nch = static_cast<int>((e.numel + kAdamChunk - 1) / kAdamChunk);
+            float s = 0.f;
+            for (int i = threadIdx.x; i < nch; i += kAdamThreads) s += sumsq[e.first_chunk + i];
+            s = warp_sum(s);
+            if ((threadIdx.x & 31) == 0) sh[threadIdx.x >> 5] = s;
+            __syncthreads();
+            ss = 0.f;
+#pragma unroll
+            for (int i = 0; i < kAdamThreads / 32; ++i) ss += sh[i];
+        } else {
+            ss = sumsq[t];
+        }
+        const float c = h.max_grad_norm / (sqrtf(ss) + 1e-6f);
         coef = c < 1.f ? c : 1.f;
     }
     float* p = static_cast<float*>(e.p);
@@ -108,6 +132,14 @@ adam_update_kernel(const vb_adam_tensor* __restrict__ tab, int n_tensors, const 
         p[i] = pp; m[i] = mm; v[i] = vv;
     }
 }
+__global__ void __launch_bounds__(kAdamThreads)
+adam_update_kernel(const vb_adam_tensor* __restrict__ tab, int n_tensors, const float* __restrict__ sumsq, const AdamHyper h) {
+    adam_update_body<false>(tab, n_tensors, sumsq, h);
+}
+__global__ void __launch_bounds__(kAdamThreads)
+adam_update_ordered_kernel(const vb_adam_tensor* __restrict__ tab, int n_tensors, const float* __restrict__ part, const AdamHyper h) {
+    adam_update_body<true>(tab, n_tensors, part, h);
+}
 
 int bert_adam_step(const vb_adam_tensor* table, int n_tensors, int n_chunks, float* sumsq, double b1, double b2, double eps,
                    double max_grad_norm, cudaStream_t st) {
@@ -117,6 +149,21 @@ int bert_adam_step(const vb_adam_tensor* table, int n_tensors, int n_chunks, flo
     // the reference holds b1 / b2 as Python doubles and forms (1 - b) in double before it meets the fp32 tensors
     const AdamHyper h{static_cast<float>(b1), static_cast<float>(1.0 - b1), static_cast<float>(b2), static_cast<float>(1.0 - b2),
                       static_cast<float>(eps), static_cast<float>(max_grad_norm)};
+    const DetWs det = det_ws();
+    if (det.ptr != nullptr) {
+        VB_TRY_RC(det_require(4LL * n_chunks, "vb_bert_adam_step"));
+        float* part = static_cast<float*>(det.ptr);
+        if (max_grad_norm > 0.0) {
+            ProfScope ps(st, PROF_OTHER, 0.0, 1);
+            adam_sumsq_part_kernel<<<n_chunks, kAdamThreads, 0, st>>>(table, n_tensors, part);
+        }
+        {
+            ProfScope ps(st, PROF_OTHER, 0.0, 1);
+            adam_update_ordered_kernel<<<n_chunks, kAdamThreads, 0, st>>>(table, n_tensors, part, h);
+        }
+        VB_CHECK_CUDA(cudaGetLastError());
+        return 0;
+    }
     if (max_grad_norm > 0.0) {
         VB_CHECK_CUDA(cudaMemsetAsync(sumsq, 0, sizeof(float) * n_tensors, st));
         ProfScope ps(st, PROF_OTHER, 0.0, 1);

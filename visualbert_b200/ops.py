@@ -7,7 +7,10 @@ without a CUDA device these ops raise.
 Activations are bf16; parameters are the model's fp32 master weights, cast to bf16 "compute weights"
 in a WeightBank by one vb_cast_multi launch per refresh. Parameter gradients come back in fp32.
 """
+import contextlib
 import ctypes
+import functools
+import threading
 
 import torch
 
@@ -58,6 +61,74 @@ def _bwd_scratch(dev, M, H, I, A, need_drop):
     w = {k: (c[k][:M] if c[k] is not None else None) for k in ("d_pre", "d_pre_drop", "d_big", "d_x1", "d_ctx")}
     w["drow"] = c["drow"][:A * M]   # [B, A, S] dense, [heads, total] unpadded
     return w
+
+
+_det_ws_cache = {}
+_det_current = threading.local()   # the (pointer, bytes) this thread last handed to vb_set_deterministic
+
+
+@functools.lru_cache(maxsize=256)
+def _det_workspace_bytes(sms, rows, H, I, vocab, adam_chunks):
+    """vb_deterministic_workspace_bytes on the current device; the split factors it sizes come from the SM count, which is part
+    of the cache key so that devices with different SM counts in one process each get their own size."""
+    need = int(_lib.lib().vb_deterministic_workspace_bytes(rows, H, I, vocab, adam_chunks))
+    if need < 0:
+        _lib.check(1, "vb_deterministic_workspace_bytes")
+    return need
+
+
+def _det_workspace(dev, rows=0, H=0, I=0, vocab=0, adam_chunks=0):
+    """The deterministic-mode workspace of a device (vb_deterministic_workspace_bytes): one buffer per device that only grows,
+    like _bwd_scratch. Every library call uses it from its start, in stream order."""
+    with torch.cuda.device(dev):
+        need = _det_workspace_bytes(torch.cuda.get_device_properties(dev).multi_processor_count, rows, H, I, vocab, adam_chunks)
+    ws = _det_ws_cache.get(dev)
+    if ws is None or ws.numel() < need:
+        _det_ws_cache.pop(dev, None)   # free the smaller buffer before allocating
+        with _unfilled():
+            ws = torch.empty(max(need, 256), device=dev, dtype=torch.uint8)
+        _det_ws_cache[dev] = ws
+    return ws
+
+
+@contextlib.contextmanager
+def _unfilled():
+    """Allocations inside skip torch's fill of uninitialized memory, which torch.use_deterministic_algorithms turns on by default
+    (torch.utils.deterministic.fill_uninitialized_memory): used only around buffers the library writes completely before anything
+    reads them (the activation arena, backward scratch, embedding and decoder outputs), where the fill is pure HBM traffic — over
+    12 GB per training step at the benchmark shape. Nothing is changed when torch's deterministic mode is off."""
+    if not torch.are_deterministic_algorithms_enabled():
+        yield
+        return
+    du = torch.utils.deterministic
+    old = du.fill_uninitialized_memory
+    du.fill_uninitialized_memory = False
+    try:
+        yield
+    finally:
+        du.fill_uninitialized_memory = old
+
+
+@contextlib.contextmanager
+def deterministic(dev, rows=0, H=0, I=0, vocab=0, adam_chunks=0):
+    """Run the library calls inside in deterministic mode (vb_set_deterministic) when torch.use_deterministic_algorithms is on
+    (warn_only included): every gradient reduction then adds in a fixed order, so the same inputs give the same bits. The mode is
+    a thread-local flag of the library and the autograd engine runs backward on its own thread, so it is set around each call,
+    not once per step; on exit the thread's previous setting comes back, so scopes may nest. Buffers allocated inside are
+    _unfilled. With torch's flag off nothing is called and the default kernels run."""
+    if not torch.are_deterministic_algorithms_enabled():
+        yield
+        return
+    ws = _det_workspace(dev, rows, H, I, vocab, adam_chunks)
+    prev = getattr(_det_current, "ws", (None, 0))
+    _lib.check(_lib.lib().vb_set_deterministic(ws.data_ptr(), ws.numel()), "vb_set_deterministic")
+    _det_current.ws = (ws.data_ptr(), ws.numel())
+    try:
+        with _unfilled():
+            yield
+    finally:
+        _lib.lib().vb_set_deterministic(prev[0], prev[1])
+        _det_current.ws = prev
 
 
 def cast_to_bf16(src, out=None):
@@ -343,7 +414,7 @@ class _EncoderFn(torch.autograd.Function):
         I = params[10].shape[0]
         A = meta["heads"]
         x = x.contiguous()
-        with torch.cuda.device(x.device):
+        with torch.cuda.device(x.device), deterministic(x.device, M, H, I):
             descs, weights, stride, off = meta["plan"].prepare(meta["caches"], params, B, S, H, A, I, mbias, meta, x.device, vl)
             arena = torch.empty(L * stride, device=x.device, dtype=torch.uint8)
             if vl is None:
@@ -380,7 +451,7 @@ class _EncoderFn(torch.autograd.Function):
             return (None,) * (3 + 16 * L)
         dy = douts[L - 1].to(_BF16).contiguous()
         grads, flat = _layer_grads(ctx.params, L, H, I, dev)
-        with torch.cuda.device(dev):
+        with torch.cuda.device(dev), deterministic(dev, M, H, I):
             w = _bwd_scratch(dev, M, H, I, A, meta["hidden_dropout"] > 0)
             sc = _lib.LayerScratch(**{k: _ptr(t) for k, t in w.items()})
             dx = torch.empty(oshape, device=dev, dtype=_BF16)
@@ -497,14 +568,16 @@ class _EmbedFn(torch.autograd.Function):
             f = feats.reshape(B * V, Dv)
             fb = cast_to_bf16(f) if f.dtype == torch.float32 else f.to(_BF16).contiguous()
             wp = meta["cache"].get(pw, train=meta.get("train", False))
-            vis_proj = torch.empty(B * V, H, device=dev, dtype=_BF16)
+            with _unfilled():
+                vis_proj = torch.empty(B * V, H, device=dev, dtype=_BF16)
             xb = None if vis_extra is None else vis_extra.detach().reshape(B * V, H).to(_BF16).contiguous()
         else:
             Dv, vt, fb, wp, vis_proj, xb = 0, None, None, None, None, None
-        pre = torch.empty(M, H, device=dev, dtype=_BF16)
-        mean = torch.empty(M, device=dev, dtype=torch.float32)
-        rstd = torch.empty(M, device=dev, dtype=torch.float32)
-        y = torch.empty(B, T + V, H, device=dev, dtype=_BF16)
+        with _unfilled():
+            pre = torch.empty(M, H, device=dev, dtype=_BF16)
+            mean = torch.empty(M, device=dev, dtype=torch.float32)
+            rstd = torch.empty(M, device=dev, dtype=torch.float32)
+            y = torch.empty(B, T + V, H, device=dev, dtype=_BF16)
         d = _lib.EmbedDesc(
             batch=B, text_len=T, num_regions=V, hidden=H, visual_dim=Dv, vocab=word.shape[0], max_pos=pos.shape[0],
             n_types=typ.shape[0], eps=1e-12, dropout=meta["dropout"], seed=meta["seed"],
@@ -547,18 +620,19 @@ class _EmbedFn(torch.autograd.Function):
             dbeta = torch.zeros_like(beta, dtype=f32)
             dpw = torch.zeros(H, Dv, device=dev, dtype=f32) if V > 0 else None
             dpb = torch.zeros(H, device=dev, dtype=f32) if V > 0 else None
-        d_pre = torch.empty(M, H, device=dev, dtype=_BF16)
-        if V > 0:
-            d_vis = torch.empty(B * V, H, device=dev, dtype=_BF16)
-            d_feats = torch.empty(B * V, Dv, device=dev, dtype=_BF16) if ctx.feats_need_grad else None
-        else:
-            d_vis = d_feats = None
+        with _unfilled():
+            d_pre = torch.empty(M, H, device=dev, dtype=_BF16)
+            if V > 0:
+                d_vis = torch.empty(B * V, H, device=dev, dtype=_BF16)
+                d_feats = torch.empty(B * V, Dv, device=dev, dtype=_BF16) if ctx.feats_need_grad else None
+            else:
+                d_vis = d_feats = None
         a = _lib.EmbedActs(vis_proj=0, pre=pre.data_ptr(), mean=mean.data_ptr(), rstd=rstd.data_ptr())
         g = _lib.EmbedGrads(
             dword=dword.data_ptr(), dpos=dpos.data_ptr(), dtype=dtyp.data_ptr(), dpos_vis=dpos_vis.data_ptr(),
             dtype_vis=dtyp_vis.data_ptr(), dw_proj=_ptr(dpw), db_proj=_ptr(dpb), dgamma=dgamma.data_ptr(),
             dbeta=dbeta.data_ptr(), d_pre=d_pre.data_ptr(), d_vis=_ptr(d_vis), d_feats=_ptr(d_feats))
-        with torch.cuda.device(dev):
+        with torch.cuda.device(dev), deterministic(dev, M, H, Dv):
             _lib.check(_lib.lib().vb_embed_bwd(ctypes.byref(ctx.desc), ctypes.byref(a), ctypes.c_void_p(dy.data_ptr()),
                                                ctypes.byref(g), _stream()), "vb_embed_bwd")
         dfe = None
@@ -602,7 +676,8 @@ class _MlmDecoderFn(torch.autograd.Function):
         table, bias_p = cache.get(E, bias, train=train)
         Vp = table.shape[0]
         t = t.to(_BF16).contiguous()
-        logits = torch.empty(n, Vp, device=t.device, dtype=_BF16)
+        with _unfilled():
+            logits = torch.empty(n, Vp, device=t.device, dtype=_BF16)
         _gemm(t.device, A=t.data_ptr(), lda=H, B=table.data_ptr(), ldb=H, M=n, N=Vp, K=H, D=logits.data_ptr(), ldd=Vp,
               bias=bias_p.data_ptr())
         ctx.save_for_backward(t, table)
@@ -616,7 +691,8 @@ class _MlmDecoderFn(torch.autograd.Function):
         n, H = t.shape
         Vp = dlogits.shape[1]
         dlogits = dlogits.contiguous()
-        dt = torch.empty(n, H, device=t.device, dtype=_BF16)
+        with _unfilled():
+            dt = torch.empty(n, H, device=t.device, dtype=_BF16)
         _gemm(t.device, A=dlogits.data_ptr(), lda=Vp, B=table.data_ptr(), ldb=H, b_mn_major=1, M=n, N=H, K=Vp, D=dt.data_ptr(), ldd=H)
         direct = _grad_targets((E, bias))
         if direct is not None:
@@ -625,11 +701,12 @@ class _MlmDecoderFn(torch.autograd.Function):
         else:
             dE = torch.zeros(V, H, device=t.device, dtype=torch.float32)
             db_pad = torch.zeros(Vp, device=t.device, dtype=torch.float32)
-        _gemm(t.device, A=dlogits.data_ptr(), lda=Vp, a_mn_major=1, B=t.data_ptr(), ldb=H, b_mn_major=1, M=V, N=H, K=n,
-              D=dE.data_ptr(), ldd=H, d_fp32=1, splits=1)
-        with torch.cuda.device(t.device):
-            _lib.check(_lib.lib().vb_colsum_bf16(ctypes.c_void_p(dlogits.data_ptr()), ctypes.c_int64(Vp), ctypes.c_void_p(db_pad.data_ptr()),
-                                                 n, Vp, _stream()), "vb_colsum_bf16")
+        with deterministic(t.device, n, H, 0, V):
+            _gemm(t.device, A=dlogits.data_ptr(), lda=Vp, a_mn_major=1, B=t.data_ptr(), ldb=H, b_mn_major=1, M=V, N=H, K=n,
+                  D=dE.data_ptr(), ldd=H, d_fp32=1, splits=1)
+            with torch.cuda.device(t.device):
+                _lib.check(_lib.lib().vb_colsum_bf16(ctypes.c_void_p(dlogits.data_ptr()), ctypes.c_int64(Vp),
+                                                     ctypes.c_void_p(db_pad.data_ptr()), n, Vp, _stream()), "vb_colsum_bf16")
         if direct is not None:
             db.add_(db_pad[:V])
             return dt, None, None, None, None

@@ -17,6 +17,7 @@ from torch.optim import Optimizer
 from torch.optim.optimizer import required
 
 from . import _lib
+from .ops import deterministic
 
 
 class _LRSchedule:
@@ -174,7 +175,7 @@ class BertAdam(Optimizer):
         plan["dev_tab"].copy_(host, non_blocking=True)
         b1, b2, e, max_norm = key
         st = torch.cuda.current_stream(dev).cuda_stream
-        with torch.cuda.device(dev):
+        with torch.cuda.device(dev), deterministic(dev, adam_chunks=plan["n_chunks"]):
             _lib.check(_lib.lib().vb_bert_adam_step(
                 ctypes.c_void_p(plan["dev_tab"].data_ptr()), len(items), plan["n_chunks"], ctypes.c_void_p(plan["sumsq"].data_ptr()),
                 ctypes.c_double(b1), ctypes.c_double(b2), ctypes.c_double(e), ctypes.c_double(max_norm), ctypes.c_void_p(st)),
