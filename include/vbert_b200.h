@@ -53,6 +53,15 @@ int vb_set_deterministic(void* workspace, int64_t bytes);
  * be 0 (e.g. inter and vocab for a BertAdam-only workspace); for the embedding pass inter = visual_dim. -1 on a bad shape. */
 int64_t vb_deterministic_workspace_bytes(int64_t rows, int32_t hidden, int32_t inter, int32_t vocab, int32_t adam_chunks);
 
+/* Dropout seed offset in device memory (CUDA graphs). While `offset` is set ON THE CALLING THREAD, every dropout a call draws or
+ * regenerates — GEMM epilogues, LayerNorm backward (hidden dropout and in_dropout), embeddings, attention keep bits — uses the seed
+ * (seed argument or descriptor seed) + *offset (mod 2^64): the bits equal those of the same call with that sum passed by value.
+ * offset points at one uint64 in DEVICE memory (8-byte aligned); the kernels read it when they run, the host never does, so a
+ * captured graph that is replayed after the value changed draws fresh bits. Calls without dropout are unaffected. offset = NULL
+ * turns it off (the default: the same kernels, grids and bits as without this call). Launches issued while their stream is
+ * capturing skip the vb_profile_enable event pairs; nothing else in the library synchronises with the host or allocates. */
+int vb_set_dropout_offset(const uint64_t* offset);
+
 /* ---- GEMM core (wgmma + TMA + mbarrier) --------------------------------------------------- */
 /* epilogue selectors */
 #define VB_EPI_NONE 0

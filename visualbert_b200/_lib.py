@@ -82,7 +82,7 @@ EXPORTS = [
     "vb_attention_fwd_varlen", "vb_attention_bwd_varlen", "vb_encoder_arena_layout_varlen", "vb_encoder_fwd_varlen",
     "vb_encoder_bwd_varlen", "vb_attention_probs", "vb_encoder_attention_probs",
     "vb_encoder_infer_workspace", "vb_encoder_infer", "vb_encoder_infer_varlen",
-    "vb_set_deterministic", "vb_deterministic_workspace_bytes",
+    "vb_set_deterministic", "vb_deterministic_workspace_bytes", "vb_set_dropout_offset",
 ]
 VB_ENCODER_ARENA_BUFFERS = 14
 ARENA_NAMES = ("qkv", "ctx", "lse", "pre1", "mean1", "rstd1", "x1", "u", "g", "pre2", "mean2", "rstd2", "keep_mask", "y")
@@ -125,6 +125,7 @@ def lib():
         h.vb_set_deterministic.argtypes = [_P, c_i64]
         h.vb_deterministic_workspace_bytes.restype = ctypes.c_int64
         h.vb_deterministic_workspace_bytes.argtypes = [c_i64, _I, _I, _I, _I]
+        h.vb_set_dropout_offset.argtypes = [_P]
         _lib = h
     return _lib
 

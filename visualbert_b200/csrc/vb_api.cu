@@ -354,6 +354,7 @@ int embed_fwd_api(const vb_embed_desc* d, void* y, const vb_embed_acts* s, cudaS
         p.drop_thresh16 = q.thr8;
         p.drop_seed = d->seed;
         p.drop_stream = kEmbedDropStream;
+        p.drop_offset = drop_offset();
     }
     return embed_fwd(p, st);
 }

@@ -30,9 +30,10 @@ namespace vb {
 
 // MT = m16 tiles per warp: 1 -> 4 warps x 16 rows, 2 -> 2 warps x 32 rows (FA2-style: each ldmatrix'd K/V
 // fragment feeds twice as many MMAs and the warp carries twice as many independent accumulators).
-template <int MT, int MINB, bool VL = false>
-__global__ void __launch_bounds__(128 / MT, MINB)
-attn_fwd_kernel(const AttnParams p, const int nsub) {
+// OFF: the keep bits use the seed folded from p.drop_seed64 + *p.drop_offset (vb_set_dropout_offset)
+template <int MT, bool VL, bool OFF>
+__device__ __forceinline__ void attn_fwd_body(const AttnParams& p, const int nsub, const unsigned long long* drop_offset = nullptr,
+                                              unsigned long long seed64 = 0, unsigned stream_id = 0) {
     constexpr int NT = 128 / MT;
     extern __shared__ __align__(128) uint8_t dsmem[];
     __shared__ float sbias[kMaxSub * kBlk];
@@ -133,8 +134,9 @@ attn_fwd_kernel(const AttnParams p, const int nsub) {
                 }
                 if (p.drop_scale != 0.f) {
                     const int qa = qrow0 + mt * 16 + g, qc = qa + 8;
-                    const uint32_t ka_bits = attn_keep16(p.drop_seed, bh, qa, kb, t, nkb, p.drop_thresh16);
-                    const uint32_t kc_bits = attn_keep16(p.drop_seed, bh, qc, kb, t, nkb, p.drop_thresh16);
+                    const unsigned sd = OFF ? attn_seed_fold(seed64 + *drop_offset, stream_id) : p.drop_seed;
+                    const uint32_t ka_bits = attn_keep16(sd, bh, qa, kb, t, nkb, p.drop_thresh16);
+                    const uint32_t kc_bits = attn_keep16(sd, bh, qc, kb, t, nkb, p.drop_thresh16);
 #pragma unroll
                     for (int nt = 0; nt < 8; ++nt) {
                         s[mt][nt][0] = ((ka_bits >> (2 * nt)) & 1u) ? s[mt][nt][0] * p.drop_scale : 0.f;
@@ -166,6 +168,14 @@ attn_fwd_kernel(const AttnParams p, const int nsub) {
             if (r0 + g + 8 < S) lse[r0 + g + 8] = (m[mt][1] + log2f(l[mt][1])) * 0.6931471805599453f;
         }
     }
+}
+
+template <int MT, int MINB, bool VL = false>
+__global__ void __launch_bounds__(128 / MT, MINB) attn_fwd_kernel(const AttnParams p, const int nsub) { attn_fwd_body<MT, VL, false>(p, nsub); }
+template <int MT, int MINB, bool VL = false>
+__global__ void __launch_bounds__(128 / MT, MINB)
+attn_fwd_off_kernel(const AttnParams p, const int nsub, const unsigned long long* drop_offset, unsigned long long seed64, unsigned stream_id) {
+    attn_fwd_body<MT, VL, true>(p, nsub, drop_offset, seed64, stream_id);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -441,7 +451,7 @@ static bool aligned16(const void* ptr) { return (reinterpret_cast<uintptr_t>(ptr
 
 static int fill_params(AttnParams& p, const void* qkv, const float* mask_bias, void* ctx, float* lse,
                        const void* dctx, void* dqkv, float* drow, void* keep, int B, int S, int A, int H,
-                       float dropout_p, unsigned long long seed, unsigned stream_id) {
+                       float dropout_p, unsigned long long seed, unsigned stream_id, AttnDropOffset* off = nullptr) {
     VB_REQUIRE(B > 0 && S > 0 && A > 0, "attention: empty problem");
     VB_REQUIRE(H == A * kHd, "attention: head_dim must be 64 (hidden=%d heads=%d)", H, A);
     VB_REQUIRE(A <= 65535 && B <= 65535, "attention: grid too large");
@@ -466,11 +476,9 @@ static int fill_params(AttnParams& p, const void* qkv, const float* mask_bias, v
     const unsigned th8 = static_cast<unsigned>(dropout_p * 256.f + 0.5f);
     p.drop_thresh16 = th8;
     p.drop_scale = dropout_p > 0.f ? 256.f / (256.f - static_cast<float>(th8 > 255 ? 255 : th8)) : 0.f;
-    // fold the per-layer stream id into the 32-bit seed of the element hash
-    unsigned long long z = seed + 0x9E3779B97F4A7C15ull * (stream_id + 1ull);
-    z = (z ^ (z >> 30)) * 0xBF58476D1CE4E5B9ull;
-    z = (z ^ (z >> 27)) * 0x94D049BB133111EBull;
-    p.drop_seed = static_cast<unsigned>(z ^ (z >> 31));
+    // fold the per-layer stream id into the 32-bit seed of the element hash (on the device when the offset is there)
+    p.drop_seed = attn_seed_fold(seed, stream_id);
+    if (off != nullptr) *off = AttnDropOffset{dropout_p > 0.f ? drop_offset() : nullptr, seed, stream_id};
     return 0;
 }
 
@@ -490,21 +498,28 @@ static int set_varlen(AttnParams& p, const int* cu_seqlens, int total, const voi
     return 0;
 }
 
-static int attn_fwd_launch(const AttnParams& p, cudaStream_t st) {
+static int attn_fwd_launch(const AttnParams& p, const AttnDropOffset& off, cudaStream_t st) {
     const int B = p.B, S = p.S, A = p.A;
     dim3 grid((S + kBlk - 1) / kBlk, A, B);
     const AttnRoute route = attn_route(S);
-    if (route == AttnRoute::Wgmma) return attn_fwd_wgmma(p, st);
-    if (route == AttnRoute::Head) return attn_fwd_head(p, static_cast<int>(grid.x), st);
+    if (route == AttnRoute::Wgmma) return attn_fwd_wgmma(p, off, st);
+    if (route == AttnRoute::Head) return attn_fwd_head(p, off, static_cast<int>(grid.x), st);
     const long long nkb = grid.x;
     VB_REQUIRE(p.drop_scale == 0.f || static_cast<long long>(B) * A * (nkb * kBlk) * nkb * 16 < (1LL << 32),
                "attention dropout: mask counter space exceeded (B*A*S too large)");
     const int nsub = static_cast<int>(grid.x) < kMaxSub ? static_cast<int>(grid.x) : kMaxSub;
     const int smem = (1 + 2 * nsub) * kTileBytes;
     static int configured[kMaxDevices] = {0}, configured_vl[kMaxDevices] = {0};
+    static int configured_off[kMaxDevices] = {0}, configured_vl_off[kMaxDevices] = {0};
     {
         ProfScope ps(st, PROF_ATTN_FWD, 4.0 * B * A * S * S * kHd, 1);
-        if (p.cu_seqlens == nullptr) {
+        if (off.offset != nullptr && p.cu_seqlens == nullptr) {
+            VB_CHECK_CUDA(ensure_dyn_smem(attn_fwd_off_kernel<1, 3>, (1 + 2 * kMaxSub) * kTileBytes, configured_off));
+            attn_fwd_off_kernel<1, 3><<<grid, 128, smem, st>>>(p, nsub, off.offset, off.seed, off.stream_id);
+        } else if (off.offset != nullptr) {
+            VB_CHECK_CUDA(ensure_dyn_smem(attn_fwd_off_kernel<1, 3, true>, (1 + 2 * kMaxSub) * kTileBytes, configured_vl_off));
+            attn_fwd_off_kernel<1, 3, true><<<grid, 128, smem, st>>>(p, nsub, off.offset, off.seed, off.stream_id);
+        } else if (p.cu_seqlens == nullptr) {
             VB_CHECK_CUDA(ensure_dyn_smem(attn_fwd_kernel<1, 3>, (1 + 2 * kMaxSub) * kTileBytes, configured));
             attn_fwd_kernel<1, 3><<<grid, 128, smem, st>>>(p, nsub);
         } else {
@@ -519,20 +534,22 @@ static int attn_fwd_launch(const AttnParams& p, cudaStream_t st) {
 int attn_fwd(const void* qkv, const float* mask_bias, void* ctx, float* lse, void* keep, int B, int S, int A, int H,
              float dropout_p, unsigned long long seed, unsigned stream_id, cudaStream_t st) {
     AttnParams p;
-    int rc = fill_params(p, qkv, mask_bias, ctx, lse, nullptr, nullptr, nullptr, keep, B, S, A, H, dropout_p, seed, stream_id);
+    AttnDropOffset off;
+    int rc = fill_params(p, qkv, mask_bias, ctx, lse, nullptr, nullptr, nullptr, keep, B, S, A, H, dropout_p, seed, stream_id, &off);
     if (rc) return rc;
-    return attn_fwd_launch(p, st);
+    return attn_fwd_launch(p, off, st);
 }
 
 int attn_fwd_varlen(const void* qkv, const int* cu_seqlens, void* ctx, float* lse, void* keep, int B, int max_seq, int total,
                     int A, int H, float dropout_p, unsigned long long seed, unsigned stream_id, cudaStream_t st, bool need_lse) {
     AttnParams p;
-    int rc = fill_params(p, qkv, nullptr, ctx, lse, nullptr, nullptr, nullptr, keep, B, max_seq, A, H, dropout_p, seed, stream_id);
+    AttnDropOffset off;
+    int rc = fill_params(p, qkv, nullptr, ctx, lse, nullptr, nullptr, nullptr, keep, B, max_seq, A, H, dropout_p, seed, stream_id, &off);
     if (rc) return rc;
     VB_REQUIRE(lse != nullptr || !need_lse, "attention varlen: lse is NULL");
     if ((rc = set_varlen(p, cu_seqlens, total, qkv, ctx))) return rc;
     if (total == 0) return 0;  // no rows: nothing to compute or store
-    return attn_fwd_launch(p, st);
+    return attn_fwd_launch(p, off, st);
 }
 
 static int attn_bwd_launch(const AttnParams& p, cudaStream_t st, bool delta_ready) {

@@ -27,7 +27,7 @@ struct AttnParams {
     float scale;       // 1/sqrt(head_dim)
     float drop_scale;  // 1/(1-p) or 0
     unsigned drop_thresh16;  // attention: 8-bit threshold, round(p * 256)
-    unsigned drop_seed;
+    unsigned drop_seed;     // attn_seed_fold(seed, stream id) of the call
     // variable-length ("unpadded") calls: sequence b owns the packed rows [cu_seqlens[b], cu_seqlens[b+1]) of `total`; S is then
     // the longest sequence (it sizes the grid and the keep-mask layout), lse / drow are [A, total], and mask_bias is unused
     const int* cu_seqlens;  // device [B + 1]; nullptr for dense calls
@@ -64,6 +64,22 @@ template <bool VL>
 __device__ __forceinline__ float key_bias2(const AttnParams& p, int b, int key, int len) {
     if constexpr (VL) return key < len ? 0.f : -INFINITY;
     else return key < p.S ? p.mask_bias[static_cast<long long>(b) * p.S + key] * kLog2e : -INFINITY;
+}
+
+// vb_set_dropout_offset: a forward call whose offset is set draws its keep bits with attn_seed_fold(seed + *offset, stream_id)
+// instead of p.drop_seed, in the *_off kernels (the backward kernels read the bits the forward stored and need no seed)
+struct AttnDropOffset {
+    const unsigned long long* offset;   // nullptr: unset, or no dropout
+    unsigned long long seed;
+    unsigned stream_id;
+};
+// The 32-bit seed of the attention keep-bit hash: the per-layer stream id folded into the 64-bit seed (splitmix64 finaliser).
+// On the host for a call with its seed by value, on the device when the seed offset lives in device memory.
+__host__ __device__ __forceinline__ unsigned attn_seed_fold(unsigned long long seed, unsigned stream_id) {
+    unsigned long long z = seed + 0x9E3779B97F4A7C15ull * (stream_id + 1ull);
+    z = (z ^ (z >> 30)) * 0xBF58476D1CE4E5B9ull;
+    z = (z ^ (z >> 27)) * 0x94D049BB133111EBull;
+    return static_cast<unsigned>(z ^ (z >> 31));
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -307,12 +323,12 @@ constexpr int kMaxSub = 4;  // 64-row tiles per resident stage
 // Every launcher serves dense calls and, when p.cu_seqlens != nullptr, variable-length ones (a separate instantiation of each
 // kernel, so the dense code is unchanged).
 // whole-head persistent kernels (vb_attention_head.cu), 192 < seq <= 256; nkb = ceil(S / 64)
-int attn_fwd_head(const AttnParams& p, int nkb, cudaStream_t st);
+int attn_fwd_head(const AttnParams& p, const AttnDropOffset& off, int nkb, cudaStream_t st);
 int attn_bwd_head(const AttnParams& p, int nkb, cudaStream_t st, bool delta_ready);
-int attn_keep_mask(const AttnParams& p, int nkb, cudaStream_t st);
+int attn_keep_mask(const AttnParams& p, const AttnDropOffset& off, int nkb, cudaStream_t st);
 int attn_delta(const AttnParams& p, cudaStream_t st);
 // wgmma / TMA / mbarrier kernels (vb_attention_wgmma.cu), seq <= 192
-int attn_fwd_wgmma(const AttnParams& p, cudaStream_t st);
+int attn_fwd_wgmma(const AttnParams& p, const AttnDropOffset& off, cudaStream_t st);
 int attn_bwd_wgmma(const AttnParams& p, cudaStream_t st, bool delta_ready);
 int make_tmap_bf16(CUtensorMap* m, const void* ptr, uint64_t inner, uint64_t outer, uint64_t ld_elems, uint32_t box_outer);
 

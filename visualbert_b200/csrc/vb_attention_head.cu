@@ -36,11 +36,9 @@ __device__ __forceinline__ void load_rows(uint32_t tiles, const bf16* base, long
 // backward) and the transpose keepT[(bh * np64 + key) * nkb + qb] (bit = query % 64; rows = keys: for a backward
 // that walks keys). A block is one 64 x 64 bit tile; the transpose is 64 warp ballots per 32 rows.
 // ------------------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(64)
-attn_keep_mask_kernel(unsigned long long* __restrict__ keep, unsigned long long* __restrict__ keepT, int nkb, int np64, int S,
-                      unsigned seed, unsigned thresh8) {
-    pdl_trigger();
-    pdl_wait();
+__device__ __forceinline__ void
+attn_keep_mask_body(unsigned long long* __restrict__ keep, unsigned long long* __restrict__ keepT, int nkb, int np64, int S,
+                    unsigned seed, unsigned thresh8) {
     const int kb = blockIdx.x % nkb, qb = (blockIdx.x / nkb) % nkb;
     const long long bh = blockIdx.x / (nkb * nkb);
     const int row = qb * 64 + threadIdx.x;
@@ -85,6 +83,21 @@ attn_keep_mask_kernel(unsigned long long* __restrict__ keep, unsigned long long*
     uint32_t* kt32 = reinterpret_cast<uint32_t*>(keepT);
     kt32[((bh * np64 + kb * 64 + lane) * nkb + qb) * 2 + wi] = t_lo;
     kt32[((bh * np64 + kb * 64 + 32 + lane) * nkb + qb) * 2 + wi] = t_hi;
+}
+__global__ void __launch_bounds__(64)
+attn_keep_mask_kernel(unsigned long long* __restrict__ keep, unsigned long long* __restrict__ keepT, int nkb, int np64, int S,
+                      unsigned seed, unsigned thresh8) {
+    pdl_trigger();
+    pdl_wait();
+    attn_keep_mask_body(keep, keepT, nkb, np64, S, seed, thresh8);
+}
+// vb_set_dropout_offset: the seed is folded from seed64 + *offset, read once the previous kernel's writes are visible
+__global__ void __launch_bounds__(64)
+attn_keep_mask_off_kernel(unsigned long long* __restrict__ keep, unsigned long long* __restrict__ keepT, int nkb, int np64, int S,
+                          unsigned long long seed64, unsigned stream_id, const unsigned long long* __restrict__ offset, unsigned thresh8) {
+    pdl_trigger();
+    pdl_wait();
+    attn_keep_mask_body(keep, keepT, nkb, np64, S, attn_seed_fold(seed64 + *offset, stream_id), thresh8);
 }
 
 // one 64-key block of the forward pass for a 16-row warp tile (same math as the staged kernel)
@@ -495,19 +508,23 @@ static int launch_fwd(const AttnParams& p, int nkb, cudaStream_t st) {
 }
 
 // draws the attention-dropout keep bits of the whole layer call (no-op without dropout)
-int attn_keep_mask(const AttnParams& p, int nkb, cudaStream_t st) {
+int attn_keep_mask(const AttnParams& p, const AttnDropOffset& off, int nkb, cudaStream_t st) {
     if (p.drop_scale == 0.f) return 0;
     const int np64 = nkb * kBlk;
     const long long nwords = static_cast<long long>(p.B) * p.A * np64 * nkb;
     VB_REQUIRE(nwords * 16 < (1LL << 32), "attention dropout: mask counter space exceeded (B*A*S too large)");
     ProfScope ps(st, PROF_ATTN_FWD, 0.0, 1);
-    VB_CHECK_CUDA(launch_pdl(attn_keep_mask_kernel, dim3(static_cast<unsigned>(nwords / 64)), dim3(64), 0, st, p.keep, p.keep + nwords,
-                             nkb, np64, p.S, p.drop_seed, p.drop_thresh16));
+    if (off.offset != nullptr)
+        VB_CHECK_CUDA(launch_pdl(attn_keep_mask_off_kernel, dim3(static_cast<unsigned>(nwords / 64)), dim3(64), 0, st, p.keep,
+                                 p.keep + nwords, nkb, np64, p.S, off.seed, off.stream_id, off.offset, p.drop_thresh16));
+    else
+        VB_CHECK_CUDA(launch_pdl(attn_keep_mask_kernel, dim3(static_cast<unsigned>(nwords / 64)), dim3(64), 0, st, p.keep, p.keep + nwords,
+                                 nkb, np64, p.S, p.drop_seed, p.drop_thresh16));
     return 0;
 }
 
-int attn_fwd_head(const AttnParams& p, int nkb, cudaStream_t st) {
-    int rc = attn_keep_mask(p, nkb, st);
+int attn_fwd_head(const AttnParams& p, const AttnDropOffset& off, int nkb, cudaStream_t st) {
+    int rc = attn_keep_mask(p, off, nkb, st);
     if (rc) return rc;
     rc = p.cu_seqlens ? launch_fwd<true>(p, nkb, st) : launch_fwd<false>(p, nkb, st);
     if (rc) return rc;

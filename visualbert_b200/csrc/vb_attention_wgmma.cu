@@ -378,9 +378,9 @@ static int launch_bwd_wgmma(const AttnParams& p, const CUtensorMap& tq, const CU
     return 0;
 }
 
-int attn_fwd_wgmma(const AttnParams& p, cudaStream_t st) {
+int attn_fwd_wgmma(const AttnParams& p, const AttnDropOffset& off, cudaStream_t st) {
     const int nkb = (p.S + kBlk - 1) / kBlk;
-    int rc = attn_keep_mask(p, nkb, st);
+    int rc = attn_keep_mask(p, off, nkb, st);
     if (rc) return rc;
     CUtensorMap tq;
     const bool vl = p.cu_seqlens != nullptr;

@@ -26,6 +26,9 @@ struct DetWs { void* ptr; long long bytes; };
 DetWs det_ws();
 // 0 when the mode is off or `need` bytes fit the workspace; else sets the error (naming the bytes) and returns 2
 int det_require(long long need, const char* what);
+// Device-side dropout seed offset (vb_set_dropout_offset): the calling thread's uint64 device pointer, nullptr when unset. While
+// it is set, every launch that draws dropout bits runs the kernel instantiation that adds *offset to its seed when it runs.
+const unsigned long long* drop_offset();
 // cudaFuncAttributeMaxDynamicSharedMemorySize is a per-device property of a kernel: `cache` is the caller's static
 // per-device record of the size already configured (DataParallel threads / several devices in one process).
 template <typename K>
@@ -202,15 +205,18 @@ inline DropQ dropout_quantise(float p) {
     return q;
 }
 // Keep-mask bits for the 8 consecutive elements starting at flat element index `elem8 * 8`.
-// Each element consumes 8 random bits; kept iff bits >= thr8.
-__device__ __forceinline__ uint32_t dropout_keep8(uint64_t seed, uint32_t stream, uint64_t elem8, uint32_t thr8) {
-    const uint32_t key = dropout_key(seed, stream) ^ (static_cast<uint32_t>(elem8 >> 31) * 0x27d4eb2fu);
+// Each element consumes 8 random bits; kept iff bits >= thr8. dropout_keep8_key takes key0 = dropout_key(seed, stream).
+__device__ __forceinline__ uint32_t dropout_keep8_key(uint32_t key0, uint64_t elem8, uint32_t thr8) {
+    const uint32_t key = key0 ^ (static_cast<uint32_t>(elem8 >> 31) * 0x27d4eb2fu);
     const uint32_t base = static_cast<uint32_t>(elem8) << 1;
     const uint32_t t4 = thr8 * 0x01010101u;
     // __vcmpgeu4: per-byte (a >= b) ? 0xff : 0x00; the multiply gathers the 4 byte LSBs into one nibble
     const uint32_t m0 = __vcmpgeu4(mix32(base ^ key), t4) & 0x01010101u;
     const uint32_t m1 = __vcmpgeu4(mix32((base + 1u) ^ key), t4) & 0x01010101u;
     return ((m0 * 0x01020408u) >> 24) | (((m1 * 0x01020408u) >> 24) << 4);
+}
+__device__ __forceinline__ uint32_t dropout_keep8(uint64_t seed, uint32_t stream, uint64_t elem8, uint32_t thr8) {
+    return dropout_keep8_key(dropout_key(seed, stream), elem8, thr8);
 }
 
 // ---------------------------------------------------------------------------------------------

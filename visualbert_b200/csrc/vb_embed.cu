@@ -21,9 +21,9 @@ constexpr int kEmbWarps = 8;
 
 __device__ __forceinline__ int clampi(long long v, int hi) { return v < 0 ? 0 : (v >= hi ? hi - 1 : static_cast<int>(v)); }
 
-template <int NC>
-__global__ void __launch_bounds__(kEmbWarps * 32)
-embed_fwd_kernel(const EmbedParams p) {
+// OFF: the dropout seed is p.drop_seed + *p.drop_offset (vb_set_dropout_offset)
+template <int NC, bool OFF>
+__device__ __forceinline__ void embed_fwd_body(const EmbedParams& p) {
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int S = p.T + p.V;
     const long long row = static_cast<long long>(blockIdx.x) * kEmbWarps + warp;
@@ -100,7 +100,7 @@ embed_fwd_kernel(const EmbedParams p) {
                 o[i] = __ldg(p.gamma + ch * 8 + i) * ((v[c][i] - mean) * rstd) + __ldg(p.beta + ch * 8 + i);
             if (p.drop_scale != 0.f) {
                 const unsigned long long e8 = (static_cast<unsigned long long>(row) * static_cast<unsigned>(H) + ch * 8) >> 3;
-                const uint32_t keep = dropout_keep8(p.drop_seed, p.drop_stream, e8, p.drop_thresh16);
+                const uint32_t keep = dropout_keep8(OFF ? p.drop_seed + *p.drop_offset : p.drop_seed, p.drop_stream, e8, p.drop_thresh16);
 #pragma unroll
                 for (int i = 0; i < 8; ++i) o[i] = ((keep >> i) & 1u) ? o[i] * p.drop_scale : 0.f;
             }
@@ -111,6 +111,11 @@ embed_fwd_kernel(const EmbedParams p) {
         }
     }
 }
+
+template <int NC>
+__global__ void __launch_bounds__(kEmbWarps * 32) embed_fwd_kernel(const EmbedParams p) { embed_fwd_body<NC, false>(p); }
+template <int NC>
+__global__ void __launch_bounds__(kEmbWarps * 32) embed_fwd_off_kernel(const EmbedParams p) { embed_fwd_body<NC, true>(p); }
 
 // Adjoint of the gather / concat: word rows are scattered with vector reductions; the position, token-type and visual
 // position / type gradients — a few rows that EVERY example adds into — are first summed in registers over a chunk of
@@ -462,11 +467,20 @@ int embed_fwd(const EmbedParams& p, cudaStream_t st) {
     const int grid = static_cast<int>((rows + kEmbWarps - 1) / kEmbWarps);
     const int nc = (p.H / 8 + 31) / 32;
     ProfScope ps(st, PROF_EMBED, 8.0 * rows * p.H, 1);
-    switch (nc) {
-        case 1: embed_fwd_kernel<1><<<grid, kEmbWarps * 32, 0, st>>>(p); break;
-        case 2: embed_fwd_kernel<2><<<grid, kEmbWarps * 32, 0, st>>>(p); break;
-        case 3: embed_fwd_kernel<3><<<grid, kEmbWarps * 32, 0, st>>>(p); break;
-        default: embed_fwd_kernel<4><<<grid, kEmbWarps * 32, 0, st>>>(p); break;
+    if (p.drop_offset != nullptr) {   // dropout seed + *offset, read by the kernel (vb_set_dropout_offset)
+        switch (nc) {
+            case 1: embed_fwd_off_kernel<1><<<grid, kEmbWarps * 32, 0, st>>>(p); break;
+            case 2: embed_fwd_off_kernel<2><<<grid, kEmbWarps * 32, 0, st>>>(p); break;
+            case 3: embed_fwd_off_kernel<3><<<grid, kEmbWarps * 32, 0, st>>>(p); break;
+            default: embed_fwd_off_kernel<4><<<grid, kEmbWarps * 32, 0, st>>>(p); break;
+        }
+    } else {
+        switch (nc) {
+            case 1: embed_fwd_kernel<1><<<grid, kEmbWarps * 32, 0, st>>>(p); break;
+            case 2: embed_fwd_kernel<2><<<grid, kEmbWarps * 32, 0, st>>>(p); break;
+            case 3: embed_fwd_kernel<3><<<grid, kEmbWarps * 32, 0, st>>>(p); break;
+            default: embed_fwd_kernel<4><<<grid, kEmbWarps * 32, 0, st>>>(p); break;
+        }
     }
     VB_CHECK_CUDA(cudaGetLastError());
     return 0;

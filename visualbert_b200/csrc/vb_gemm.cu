@@ -51,6 +51,9 @@ int det_require(long long need, const char* what) {
                g_det_bytes);
     return 0;
 }
+// ---- dropout seed offset in device memory: thread-local for the same reason ----
+static thread_local const unsigned long long* g_drop_offset = nullptr;
+const unsigned long long* drop_offset() { return g_drop_offset; }
 
 // ---- live profiling -------------------------------------------------------------------------
 struct ProfRec { cudaEvent_t e0, e1; int cat; double work; int launches; };
@@ -62,6 +65,9 @@ static std::mutex g_prof_mu;
 ProfScope::ProfScope(cudaStream_t s, int cat, double work, int launches) : slot(-1), st(s) {
     g_launches.fetch_add(launches);
     if (!g_prof_on) return;
+    // an event recorded into a capturing stream becomes a graph node, not a timestamp this process can read back
+    cudaStreamCaptureStatus cs = cudaStreamCaptureStatusNone;
+    if (cudaStreamIsCapturing(s, &cs) != cudaSuccess || cs != cudaStreamCaptureStatusNone) return;
     std::lock_guard<std::mutex> lk(g_prof_mu);
     ProfRec r;
     if (!g_prof_pool.empty()) { r = g_prof_pool.back(); g_prof_pool.pop_back(); }
@@ -118,7 +124,10 @@ struct GemmParams {
     unsigned long long drop_seed;
     unsigned drop_stream;
     int m_fast;              // tile order: m-blocks run faster than n-blocks (see decode_tile)
-    float* delta_out;        // EPI_DELTA: fp32 [rows / delta_seq][N / 64][delta_seq]
+    union {
+        float* delta_out;        // EPI_DELTA: fp32 [rows / delta_seq][N / 64][delta_seq]
+        const unsigned long long* drop_offset;   // EPI_GENERIC_OFF: device offset added to drop_seed (a dropout GEMM has no delta)
+    };
     int delta_seq;
 };
 bool gemm_gp_tiled_ok(int M, int N);
@@ -185,7 +194,10 @@ __device__ __forceinline__ void store16_bf16(bf16* p, const float (&f)[16]) {
 // EPI_SLAB (fp32 output, deterministic mode): split s STORES its partial tile to slab s of the workspace, D = slab base with
 // ldd = N, slab s at D + s * M * N, no bias; splitk_reduce_kernel then adds bias + the slabs in split order into the real D.
 enum { EPI_GENERIC = 0, EPI_BIAS = 1, EPI_RESID = 2, EPI_DROP_RESID = 3, EPI_GELU_FWD = 4, EPI_DGELU_BWD = 5, EPI_GELU_FWD_T = 6,
-       EPI_DGELU_BWD_T = 7, EPI_DELTA = 8, EPI_GELU_ONLY = 9, EPI_SLAB = 10 };
+       EPI_DGELU_BWD_T = 7, EPI_DELTA = 8, EPI_GELU_ONLY = 9, EPI_SLAB = 10, EPI_GENERIC_OFF = 11 };
+// EPI_GENERIC_OFF: the generic epilogue with the dropout seed p.drop_seed + *p.drop_offset, read from device memory when the
+// epilogue runs (vb_set_dropout_offset); a call with dropout takes it whenever an offset is set, so no other kernel reads it.
+__host__ __device__ constexpr bool epi_is_generic(int e) { return e == EPI_GENERIC || e == EPI_GENERIC_OFF; }
 __host__ __device__ constexpr bool epi_is_gelu(int e) { return e == EPI_GELU_FWD || e == EPI_GELU_FWD_T; }
 __host__ __device__ constexpr bool epi_is_dgelu(int e) { return e == EPI_DGELU_BWD || e == EPI_DGELU_BWD_T; }
 
@@ -206,13 +218,14 @@ __device__ __forceinline__ void epilogue16(const GemmParams& p, int row, int col
 #pragma unroll
         for (int i = 0; i < 4; ++i) red_add_v4_f32(d + 4 * i, x[4 * i], x[4 * i + 1], x[4 * i + 2], x[4 * i + 3]);
     } else {
-        constexpr bool kGeneric = EPI == EPI_GENERIC;
+        constexpr bool kGeneric = epi_is_generic(EPI);
         if (EPI == EPI_DROP_RESID || (kGeneric && p.drop_scale != 0.0f)) {
             const unsigned long long e8 =
                 (static_cast<unsigned long long>(row) * static_cast<unsigned>(p.N) + col) >> 3;
 #pragma unroll
             for (int h = 0; h < 2; ++h) {
-                const uint32_t keep = dropout_keep8(p.drop_seed, p.drop_stream, e8 + h, p.drop_thresh16);
+                const uint32_t keep = dropout_keep8(EPI == EPI_GENERIC_OFF ? p.drop_seed + *p.drop_offset : p.drop_seed, p.drop_stream, e8 + h,
+                                                    p.drop_thresh16);
 #pragma unroll
                 for (int i = 0; i < 8; ++i) x[8 * h + i] = ((keep >> i) & 1u) ? x[8 * h + i] * p.drop_scale : 0.0f;
             }
@@ -402,10 +415,10 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
         const int row0 = tc.m_blk * BLOCK_M + q * 32 + wrow_of(0), c0 = col0 + chunk_of(0) * 16;   // step j: row0 + (row step) j
         const bf16* exb = nullptr;
         long long ex_step = 0;
-        if (kWantAdd || (EPI == EPI_GENERIC && p.addend != nullptr)) {
+        if (kWantAdd || (epi_is_generic(EPI) && p.addend != nullptr)) {
             exb = p.addend + static_cast<long long>(row0) * p.ld_add + c0;
             ex_step = kRowPerLane ? 16 : RPI * p.ld_add;
-        } else if (EPI == EPI_DGELU_BWD || (EPI == EPI_GENERIC && p.epilogue == VB_EPI_DGELU)) {
+        } else if (EPI == EPI_DGELU_BWD || (epi_is_generic(EPI) && p.epilogue == VB_EPI_DGELU)) {
             exb = p.aux_in + static_cast<long long>(row0) * p.ld_aux + c0;
             ex_step = kRowPerLane ? 16 : RPI * p.ld_aux;
         } else if (EPI == EPI_DGELU_BWD_T) {
@@ -689,12 +702,15 @@ int gemm(const vb_gemm_args& a, cudaStream_t st) {
         p.delta_out = a.delta_out; p.delta_seq = a.delta_seq;
     }
     p.m_fast = (a.M + BLOCK_M - 1) / BLOCK_M < (a.N + 255) / 256 ? 1 : 0;
+    // the device seed offset of a dropout call (p.drop_offset shares its storage with delta_out: dispatch on this, not on p)
+    const unsigned long long* const off = a.dropout_p > 0.0f ? drop_offset() : nullptr;
     if (a.dropout_p > 0.0f) {
         const DropQ q = dropout_quantise(a.dropout_p);
         p.drop_scale = q.scale;
         p.drop_thresh16 = q.thr8;
         p.drop_seed = a.dropout_seed;
         p.drop_stream = a.dropout_stream;
+        if (off != nullptr) p.drop_offset = off;
     }
 
     const bool bn256 = use_bn256(a.N);
@@ -735,6 +751,17 @@ int gemm(const vb_gemm_args& a, cudaStream_t st) {
         }
         VB_CHECK_CUDA(cudaGetLastError());
         return 0;
+    }
+    if (off != nullptr) {
+        // dropout with the seed offset in device memory: the generic epilogue (it applies bias, dropout and addend in the order of
+        // the specialised ones, so the bits equal a call with seed + *offset by value)
+#define VB_DISPATCH_OFF(AM, BM) \
+    (bn256 ? launch<AM, BM, 256, false, EPI_GENERIC_OFF>(ta, tb, p, st) : launch<AM, BM, 128, false, EPI_GENERIC_OFF>(ta, tb, p, st))
+        if (!a.a_mn_major && !a.b_mn_major) return VB_DISPATCH_OFF(false, false);
+        if (!a.a_mn_major && a.b_mn_major) return VB_DISPATCH_OFF(false, true);
+        if (a.a_mn_major && a.b_mn_major) return VB_DISPATCH_OFF(true, true);
+        return VB_DISPATCH_OFF(true, false);
+#undef VB_DISPATCH_OFF
     }
     if (a.epilogue == VB_EPI_GELU_FWD)
         return bn256 ? launch<false, false, 256, false, EPI_GELU_ONLY>(ta, tb, p, st) : launch<false, false, 128, false, EPI_GELU_ONLY>(ta, tb, p, st);
@@ -815,6 +842,14 @@ int vb_set_deterministic(void* workspace, int64_t bytes) {
     }
     vb::g_det_ptr = workspace;
     vb::g_det_bytes = workspace != nullptr ? bytes : 0;
+    return 0;
+}
+int vb_set_dropout_offset(const uint64_t* offset) {
+    if ((reinterpret_cast<uintptr_t>(offset) & 7) != 0) {
+        vb::set_error("vb_set_dropout_offset: the offset must be 8-byte aligned (got %p)", static_cast<const void*>(offset));
+        return 2;
+    }
+    vb::g_drop_offset = reinterpret_cast<const unsigned long long*>(offset);
     return 0;
 }
 int vb_gemm_delta_ok(int32_t M, int32_t N) { return vb::gemm_delta_ok(M, N) ? 1 : 0; }

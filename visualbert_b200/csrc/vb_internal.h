@@ -56,6 +56,7 @@ struct EmbedParams {
     int B, T, V, H, vocab, max_pos, n_types;
     float eps;
     float drop_scale; unsigned drop_thresh16; unsigned long long drop_seed; unsigned drop_stream;
+    const unsigned long long* drop_offset;   // non-null: the dropout seed is drop_seed + *drop_offset (vb_set_dropout_offset)
 };
 struct EmbedBwdParams {
     const bf16* de;

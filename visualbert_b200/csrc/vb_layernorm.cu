@@ -102,14 +102,15 @@ __device__ __forceinline__ int slot(int a, int h, int ch, int chunks) { return (
 
 // PART = false: the block's column sums go to dgamma / dbeta / dbias by atomicAdd. PART = true (deterministic mode): dgamma is
 // the workspace and block b STORES its sums to dgamma[(b * 3 + array) * H + col]; partials_reduce adds them in block order.
-template <int NC, bool PART>
+// OFF = true (vb_set_dropout_offset): the dropout seed is drop_seed + *drop_offset, read once global memory may be touched.
+template <int NC, bool PART, bool OFF = false>
 __device__ __forceinline__ void
 ln_bwd_body(const bf16* __restrict__ dy, const bf16* __restrict__ x, const float* __restrict__ mean,
             const float* __restrict__ rstd, const float* __restrict__ gamma, bf16* __restrict__ dx,
             bf16* __restrict__ dx_drop, float* __restrict__ dgamma, float* __restrict__ dbeta,
             float* __restrict__ dbias, int rows, int H, float drop_scale, unsigned drop_thresh16,
             unsigned long long drop_seed, unsigned drop_stream, float in_scale, unsigned in_thresh16,
-            unsigned in_stream) {
+            unsigned in_stream, const unsigned long long* __restrict__ drop_offset = nullptr) {
     extern __shared__ float4 sm4[];  // [gamma: 2*chunks] [warp][3 arrays][2 halves][chunks]
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int chunks = H >> 3;
@@ -118,6 +119,15 @@ ln_bwd_body(const bf16* __restrict__ dy, const bf16* __restrict__ x, const float
     pdl_trigger();
     for (int i = threadIdx.x; i < kLnWarps * 6 * chunks; i += blockDim.x) sm4[2 * chunks + i] = make_float4(0.f, 0.f, 0.f, 0.f);
     pdl_wait();  // the accumulators are cleared while the previous kernel drains; global memory is touched from here on
+    // OFF: the hash keys of the summed seed wait in shared memory (the 64-bit sum held in registers spills the NC = 4 build)
+    __shared__ uint32_t s_key[2];   // [0]: hidden dropout (drop_stream), [1]: in_dropout (in_stream)
+    if constexpr (OFF) {
+        if (threadIdx.x == 0) {
+            const unsigned long long sd = drop_seed + *drop_offset;
+            s_key[0] = dropout_key(sd, drop_stream);
+            s_key[1] = dropout_key(sd, in_stream);
+        }
+    }
     for (int i = threadIdx.x; i < 2 * chunks; i += blockDim.x) {
         const int h = i / chunks, ch = i % chunks;
         sgam[i] = __ldg(reinterpret_cast<const float4*>(gamma + ch * 8 + h * 4));
@@ -168,7 +178,8 @@ ln_bwd_body(const bf16* __restrict__ dy, const bf16* __restrict__ x, const float
             const int ch = lane + c * 32;
             if (ch < chunks) {
                 if (in_scale != 0.f) {  // dy is the gradient of dropout(LN(x)): re-apply the keep mask
-                    const uint32_t keep = dropout_keep8(drop_seed, in_stream, e8row + ch, in_thresh16);
+                    const uint32_t keep = OFF ? dropout_keep8_key(s_key[1], e8row + ch, in_thresh16)
+                                              : dropout_keep8(drop_seed, in_stream, e8row + ch, in_thresh16);
 #pragma unroll
                     for (int i = 0; i < 8; ++i) dv[c][i] = ((keep >> i) & 1u) ? dv[c][i] * in_scale : 0.f;
                 }
@@ -197,7 +208,8 @@ ln_bwd_body(const bf16* __restrict__ dy, const bf16* __restrict__ x, const float
                     o[i] = fmaf(-xh[c][i], rc2, fmaf(dv[c][i] * gm[i], rs_cur, -rc1));
                 stg_v4(dx + rbase + ch * 8, pack8(o));
                 if (dx_drop != nullptr) {
-                    const uint32_t keep = dropout_keep8(drop_seed, drop_stream, e8row + ch, drop_thresh16);
+                    const uint32_t keep = OFF ? dropout_keep8_key(s_key[0], e8row + ch, drop_thresh16)
+                                              : dropout_keep8(drop_seed, drop_stream, e8row + ch, drop_thresh16);
 #pragma unroll
                     for (int i = 0; i < 8; ++i) o[i] = ((keep >> i) & 1u) ? o[i] * drop_scale : 0.f;
                     stg_v4(dx_drop + rbase + ch * 8, pack8(o));
@@ -243,6 +255,16 @@ template <int NC>
 __global__ void __launch_bounds__(kLnWarps * 32, 2) ln_bwd_kernel(VB_LN_BWD_PARAMS) { ln_bwd_body<NC, false>(VB_LN_BWD_ARGS); }
 template <int NC>
 __global__ void __launch_bounds__(kLnWarps * 32, 2) ln_bwd_part_kernel(VB_LN_BWD_PARAMS) { ln_bwd_body<NC, true>(VB_LN_BWD_ARGS); }
+template <int NC>
+__global__ void __launch_bounds__(kLnWarps * 32, 2)
+ln_bwd_off_kernel(VB_LN_BWD_PARAMS, const unsigned long long* __restrict__ drop_offset) {
+    ln_bwd_body<NC, false, true>(VB_LN_BWD_ARGS, drop_offset);
+}
+template <int NC>
+__global__ void __launch_bounds__(kLnWarps * 32, 2)
+ln_bwd_part_off_kernel(VB_LN_BWD_PARAMS, const unsigned long long* __restrict__ drop_offset) {
+    ln_bwd_body<NC, true, true>(VB_LN_BWD_ARGS, drop_offset);
+}
 #undef VB_LN_BWD_PARAMS
 #undef VB_LN_BWD_ARGS
 
@@ -310,6 +332,8 @@ int ln_bwd(const void* dy, const void* x, const float* mean, const float* rstd, 
     const int grid = ln_bwd_grid(rows);
     const DetWs det = det_ws();
     if (det.ptr != nullptr) VB_TRY_RC(det_require(ln_bwd_det_bytes(rows, H), "layernorm backward"));
+    // the offset kernels only when this call draws dropout bits (hidden dropout or the embeddings' in_dropout)
+    const unsigned long long* off = (dropout_p > 0.f || in_dropout_p > 0.f) ? drop_offset() : nullptr;
     const DropQ dq = dropout_quantise(dropout_p), iq = dropout_quantise(in_dropout_p);
     const float scale = dq.scale, in_scale = iq.scale;
     const unsigned th = dq.thr8, in_th = iq.thr8;
@@ -319,6 +343,17 @@ int ln_bwd(const void* dy, const void* x, const float* mean, const float* rstd, 
     VB_CHECK_CUDA(ensure_dyn_smem(ln_bwd_kernel<2>, 100 * 1024, cfg2));
     VB_CHECK_CUDA(ensure_dyn_smem(ln_bwd_kernel<3>, 100 * 1024, cfg3));
     VB_CHECK_CUDA(ensure_dyn_smem(ln_bwd_kernel<4>, 100 * 1024, cfg4));
+    if (off != nullptr) {
+        static int ocfg[2][4][kMaxDevices] = {};
+        VB_CHECK_CUDA(ensure_dyn_smem(ln_bwd_off_kernel<1>, 100 * 1024, ocfg[0][0]));
+        VB_CHECK_CUDA(ensure_dyn_smem(ln_bwd_off_kernel<2>, 100 * 1024, ocfg[0][1]));
+        VB_CHECK_CUDA(ensure_dyn_smem(ln_bwd_off_kernel<3>, 100 * 1024, ocfg[0][2]));
+        VB_CHECK_CUDA(ensure_dyn_smem(ln_bwd_off_kernel<4>, 100 * 1024, ocfg[0][3]));
+        VB_CHECK_CUDA(ensure_dyn_smem(ln_bwd_part_off_kernel<1>, 100 * 1024, ocfg[1][0]));
+        VB_CHECK_CUDA(ensure_dyn_smem(ln_bwd_part_off_kernel<2>, 100 * 1024, ocfg[1][1]));
+        VB_CHECK_CUDA(ensure_dyn_smem(ln_bwd_part_off_kernel<3>, 100 * 1024, ocfg[1][2]));
+        VB_CHECK_CUDA(ensure_dyn_smem(ln_bwd_part_off_kernel<4>, 100 * 1024, ocfg[1][3]));
+    }
     if (det.ptr != nullptr) {
         static int dcfg1[kMaxDevices] = {0}, dcfg2[kMaxDevices] = {0}, dcfg3[kMaxDevices] = {0}, dcfg4[kMaxDevices] = {0};
         VB_CHECK_CUDA(ensure_dyn_smem(ln_bwd_part_kernel<1>, 100 * 1024, dcfg1));
@@ -333,7 +368,29 @@ int ln_bwd(const void* dy, const void* x, const float* mean, const float* rstd, 
         static_cast<const bf16*>(dy), static_cast<const bf16*>(x), mean, rstd, gamma, static_cast<bf16*>(dx), \
         static_cast<bf16*>(dx_drop), DG, dbeta, dbias, rows, H, scale, th, seed, stream_id, in_scale,        \
         in_th, in_stream_id))
-        if (det.ptr != nullptr) {
+#define VB_LN_BWD_OFF(K, NC, DG)                                                                             \
+    VB_CHECK_CUDA(launch_pdl(K<NC>, dim3(grid), dim3(kLnWarps * 32), smem, st,                              \
+        static_cast<const bf16*>(dy), static_cast<const bf16*>(x), mean, rstd, gamma, static_cast<bf16*>(dx), \
+        static_cast<bf16*>(dx_drop), DG, dbeta, dbias, rows, H, scale, th, seed, stream_id, in_scale,        \
+        in_th, in_stream_id, off))
+        if (off != nullptr) {
+            float* part = static_cast<float*>(det.ptr);
+            if (det.ptr != nullptr) {
+                switch (nc) {
+                    case 1: VB_LN_BWD_OFF(ln_bwd_part_off_kernel, 1, part); break;
+                    case 2: VB_LN_BWD_OFF(ln_bwd_part_off_kernel, 2, part); break;
+                    case 3: VB_LN_BWD_OFF(ln_bwd_part_off_kernel, 3, part); break;
+                    default: VB_LN_BWD_OFF(ln_bwd_part_off_kernel, 4, part); break;
+                }
+            } else {
+                switch (nc) {
+                    case 1: VB_LN_BWD_OFF(ln_bwd_off_kernel, 1, dgamma); break;
+                    case 2: VB_LN_BWD_OFF(ln_bwd_off_kernel, 2, dgamma); break;
+                    case 3: VB_LN_BWD_OFF(ln_bwd_off_kernel, 3, dgamma); break;
+                    default: VB_LN_BWD_OFF(ln_bwd_off_kernel, 4, dgamma); break;
+                }
+            }
+        } else if (det.ptr != nullptr) {
             float* part = static_cast<float*>(det.ptr);
             switch (nc) {
                 case 1: VB_LN_BWD(ln_bwd_part_kernel, 1, part); break;
@@ -350,6 +407,7 @@ int ln_bwd(const void* dy, const void* x, const float* mean, const float* rstd, 
             }
         }
 #undef VB_LN_BWD
+#undef VB_LN_BWD_OFF
     }
     VB_CHECK_CUDA(cudaGetLastError());
     if (det.ptr != nullptr) return partials_reduce(static_cast<const float*>(det.ptr), grid, 3 * H, H, dgamma, dbeta, dbias, st);

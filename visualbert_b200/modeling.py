@@ -157,7 +157,7 @@ def _encoder_meta(owner, layers, seed, **more):
     return dict(heads=l0.attention.self.num_attention_heads, layer_index0=l0.layer_index,
                 hidden_dropout=l0.hidden_dropout_prob if train else 0.0,
                 attn_dropout=l0.attention_probs_dropout_prob if train else 0.0, seed=int(seed), train=train,
-                caches=[l._weights for l in layers], plan=plan, **more)
+                caches=[l._weights for l in layers], plan=plan, seed_offset=ops.current_seed_offset() if train else None, **more)
 
 
 class BertLayer(nn.Module):
@@ -306,7 +306,7 @@ class BertEmbeddingsWithVisualEmbedding(nn.Module):
         if visual_embeddings is not None and visual_embeddings_type is None:
             visual_embeddings_type = torch.zeros(visual_embeddings.shape[:-1], dtype=torch.long, device=input_ids.device)
         meta = dict(dropout=self.hidden_dropout_prob if self.training else 0.0, seed=int(seed), cache=self._weights,
-                    train=self.training)
+                    train=self.training, seed_offset=ops.current_seed_offset() if self.training else None)
         return ops.bert_embeddings(
             meta, input_ids, token_type_ids, visual_embeddings_type, visual_embeddings,
             self.word_embeddings.weight, self.position_embeddings.weight, self.token_type_embeddings.weight,
@@ -474,6 +474,8 @@ class BertVisualModel(PreTrainedBertModel):
         self.apply(self.init_bert_weights)
         self._unpadded = False
         self._step = 0
+        self._capturable = False
+        self._seed_offset = None   # capturable mode: the step snapshot of the latest training forward (int64 [1])
         # base of the counter-hash dropout streams: follows torch.manual_seed (so runs are reproducible the torch way);
         # the data-parallel rank is mixed in per forward (next_seed) so replicas draw different masks
         self.dropout_seed = (0x5EED ^ torch.initial_seed()) & 0xFFFFFFFF
@@ -504,7 +506,32 @@ class BertVisualModel(PreTrainedBertModel):
                 items += holder.items(*masters)
                 holder.owner = bank
             bank.bind(items)
-        bank.refresh(force=self.training)
+        bank.refresh(force=self.training or self._capturable)
+
+    def set_graph_capturable(self, flag=True):
+        """Opt-in CUDA-graph-capturable mode, off by default.
+
+        When on, the dropout step counter is an int64 tensor on the model's device (a non-persistent buffer: it moves with
+        .to() and stays out of state_dict). Each training forward increments it and snapshots it into a tensor of its own; the
+        descriptors carry the base seed K = (dropout_seed + c * rank) * golden and the kernels add the snapshot, read from device
+        memory when they run (vb_set_dropout_offset). Every forward therefore draws exactly the seed next_seed() gives in the
+        default mode, a backward uses its own forward's snapshot (gradient accumulation stays correct), and a captured graph
+        draws fresh masks at every replay. The compute-weight cast is enqueued on every forward, eval mode included, so
+        replays see parameter changes made between them. dropout_state() reads the counter back (one host synchronisation);
+        set_dropout_state() writes it in place (a captured graph sees the new value). States carry over between the modes.
+        Not available with the unpadded path (set_unpadded), which synchronises with the host."""
+        flag = bool(flag)
+        if flag and self._unpadded:
+            raise ValueError("set_graph_capturable: not supported with set_unpadded (its row plan synchronises with the host)")
+        if flag and not self._capturable:
+            dev = next(self.parameters()).device
+            self.register_buffer("_vb_step", torch.tensor([self._step], dtype=torch.int64, device=dev), persistent=False)
+        elif not flag and self._capturable:
+            self._step = int(self._vb_step.item())
+            del self._vb_step
+            self._seed_offset = None
+        self._capturable = flag
+        return self
 
     def set_unpadded(self, flag=True):
         """Opt-in unpadded ("variable-length") encoder execution, off by default.
@@ -523,6 +550,8 @@ class BertVisualModel(PreTrainedBertModel):
         bypass_transformer or output_attention_weights, nor, in training mode under grad, with output_all_encoded_layers=True
         (gradients through intermediate layers): those raise instead of running padded."""
         flag = bool(flag)
+        if flag and self._capturable:
+            raise ValueError("set_unpadded: not supported in graph-capturable mode (set_graph_capturable)")
         if flag and self.bypass_transformer:
             raise ValueError("set_unpadded: not supported with bypass_transformer")
         if flag and self.output_attention_weights:
@@ -546,21 +575,32 @@ class BertVisualModel(PreTrainedBertModel):
         return [zero.index_copy(0, idx, y.to(torch.bfloat16)).view(B, S, H) for y in ys]
 
     def next_seed(self):
-        """Per-forward dropout seed: forward and backward of one step share it; steps differ."""
-        self._step += 1
+        """Per-forward dropout seed: forward and backward of one step share it; steps differ. In graph-capturable mode the
+        step lives on the device: this returns the base K, and the seed the kernels use is K + the snapshot left in
+        self._seed_offset (what the default mode returns, mod 2^64)."""
         rank = 0
         if torch.distributed.is_available() and torch.distributed.is_initialized():
             rank = torch.distributed.get_rank()
-        return ((self.dropout_seed + 0x632BE59B * rank) * 0x9E3779B97F4A7C15 + self._step) & 0xFFFFFFFFFFFFFFFF
+        base = ((self.dropout_seed + 0x632BE59B * rank) * 0x9E3779B97F4A7C15) & 0xFFFFFFFFFFFFFFFF
+        if self._capturable:
+            self._vb_step.add_(1)
+            self._seed_offset = self._vb_step.clone()
+            return base
+        self._step += 1
+        return (base + self._step) & 0xFFFFFFFFFFFFFFFF
 
     def dropout_state(self):
         """(base seed, forwards so far): save next to a checkpoint and hand back to set_dropout_state() to resume the
-        exact dropout sequence (kept out of state_dict so reference checkpoints still load with strict=True)."""
-        return {"seed": int(self.dropout_seed), "step": int(self._step)}
+        exact dropout sequence (kept out of state_dict so reference checkpoints still load with strict=True). In
+        graph-capturable mode this reads the device counter: one host synchronisation."""
+        step = int(self._vb_step.item()) if self._capturable else int(self._step)
+        return {"seed": int(self.dropout_seed), "step": step}
 
     def set_dropout_state(self, state):
         self.dropout_seed = int(state["seed"])
         self._step = int(state["step"])
+        if self._capturable:
+            self._vb_step.fill_(self._step)
 
     def forward(self, input_ids, token_type_ids, attention_mask, visual_embeddings, position_embeddings_visual,
                 visual_embeddings_type, image_text_alignment, confidence, output_all_encoded_layers=True):
@@ -570,7 +610,17 @@ class BertVisualModel(PreTrainedBertModel):
             attention_mask = torch.ones(input_ids.size(0), T + V, dtype=torch.long, device=input_ids.device)
         if token_type_ids is None:
             token_type_ids = torch.zeros_like(input_ids)
+        capturing = input_ids.is_cuda and torch.cuda.is_current_stream_capturing()
+        if capturing and not self._capturable:
+            raise ValueError("CUDA graph capture of a forward needs graph-capturable mode: call set_graph_capturable() first "
+                             "(otherwise every replay would reuse the captured step's dropout masks)")
         seed = self.next_seed() if self.training else 0
+        with ops.forward_seed_offset(self._seed_offset if (self._capturable and self.training) else None):
+            return self._forward(input_ids, token_type_ids, attention_mask, visual_embeddings, position_embeddings_visual,
+                                 visual_embeddings_type, image_text_alignment, confidence, output_all_encoded_layers, seed)
+
+    def _forward(self, input_ids, token_type_ids, attention_mask, visual_embeddings, position_embeddings_visual,
+                 visual_embeddings_type, image_text_alignment, confidence, output_all_encoded_layers, seed):
         self.refresh_compute_weights()
         bias = None if self._unpadded else ops.mask_bias(attention_mask, None)
         x = self.embeddings(input_ids, token_type_ids, visual_embeddings=visual_embeddings,
@@ -728,6 +778,9 @@ class TrainVisualBERTObjective(PreTrainedBertModel):
         """Indices of the rows that carry an MLM target. `nonzero` synchronises with the device, so forward() calls this
         BEFORE the encoder is enqueued (the stream is empty then) instead of draining ~12 ms of queued work later.
         Labels outside [0, vocab) are treated like the reference's ignore index -1 (CrossEntropyLoss(ignore_index=-1))."""
+        if flat_labels.is_cuda and torch.cuda.is_current_stream_capturing():
+            raise ValueError("CUDA graph capture: finding the MLM target rows needs a host synchronisation (nonzero); pass "
+                             "masked_lm_rows (parallel.BatchPrefetcher computes them on the host)")
         flat = flat_labels.contiguous().view(-1)
         keep = flat >= 0 if vocab is None else (flat >= 0) & (flat < vocab)
         return torch.nonzero(keep).squeeze(1)
@@ -752,8 +805,19 @@ class TrainVisualBERTObjective(PreTrainedBertModel):
         labels = flat_labels.contiguous().view(-1)
         if rows is None:
             rows = self._labelled_rows(flat_labels, self.cls.predictions.decoder.weight.size(0))
-        hidden = sequence_output.reshape(-1, sequence_output.size(-1)).index_select(0, rows)
         head = self.cls.predictions
+        if self.bert._capturable and sequence_output.is_cuda:
+            # fixed-capacity rows (parallel.BatchPrefetcher(mlm_rows_capacity=N)): -1 entries are "no target". They read row 0
+            # with label -1 (no loss, no gradient in the cross-entropy kernels); the loss is the sum over the valid rows divided by
+            # their count, counted on the device, so neither the shapes nor the host depend on how many targets a batch has.
+            valid = rows >= 0
+            safe = rows.clamp(min=0)
+            hidden = sequence_output.reshape(-1, sequence_output.size(-1)).index_select(0, safe)
+            lab = torch.where(valid, labels.index_select(0, safe), torch.full_like(safe, -1))
+            count = valid.sum(dtype=torch.float32).clamp(min=1.0).reshape(())
+            scores = ops.mlm_decoder(head.transform(hidden), head.decoder.weight, head.bias, self._decoder_cache(), self.training)
+            return ops.cross_entropy_rows(scores, lab, head.decoder.weight.size(0), count)
+        hidden = sequence_output.reshape(-1, sequence_output.size(-1)).index_select(0, rows)
         if rows.numel() == 0 or not hidden.is_cuda:
             return F.cross_entropy(head(hidden).float(), labels.index_select(0, rows))
         # decoder + loss on the library's kernels: wgmma GEMMs (fwd / dgrad / wgrad into the tied word-embedding
@@ -770,6 +834,8 @@ class TrainVisualBERTObjective(PreTrainedBertModel):
         (b * (T + V) + t, int64, on the device) of the positions whose `masked_lm_labels` is not -1. When given (e.g. by
         `parallel.BatchPrefetcher`, which computes them on the host from the host copy of the labels) the forward pass
         contains no host synchronisation at all; when omitted they are found with one `nonzero` before the encoder."""
+        if self.training_head_type == "vqa_advanced" and input_ids.is_cuda and torch.cuda.is_current_stream_capturing():
+            raise ValueError("CUDA graph capture: the vqa_advanced head reads its accuracy with .item(); run it eagerly")
         if "_bank_extra" not in self.bert.__dict__:
             self._register_decoder_in_bank()
         flat_input_ids = transform_to_batch_sequence(input_ids)

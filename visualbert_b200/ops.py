@@ -46,6 +46,9 @@ def _bwd_scratch(dev, M, H, I, A, need_drop):
     backward."""
     key = (dev, H, I, A)
     c = _bwd_scratch_cache.get(key)
+    if _capturing() and (c is None or c["rows"] < M or (need_drop and c["d_pre_drop"] is None)):
+        raise ValueError("CUDA graph capture: the encoder backward scratch would grow inside the graph's private pool; warm up at "
+                         "this shape first (run the step eagerly once)")
     if c is None or c["rows"] < M:
         rows = M if c is None else max(M, c["rows"] + c["rows"] // 4)
         rows = (rows + 255) // 256 * 256
@@ -83,6 +86,9 @@ def _det_workspace(dev, rows=0, H=0, I=0, vocab=0, adam_chunks=0):
     with torch.cuda.device(dev):
         need = _det_workspace_bytes(torch.cuda.get_device_properties(dev).multi_processor_count, rows, H, I, vocab, adam_chunks)
     ws = _det_ws_cache.get(dev)
+    if _capturing() and (ws is None or ws.numel() < need):
+        raise ValueError("CUDA graph capture: the deterministic-mode workspace would grow inside the graph's private pool; warm up "
+                         "at this shape first (run the step eagerly once)")
     if ws is None or ws.numel() < need:
         _det_ws_cache.pop(dev, None)   # free the smaller buffer before allocating
         with _unfilled():
@@ -129,6 +135,48 @@ def deterministic(dev, rows=0, H=0, I=0, vocab=0, adam_chunks=0):
     finally:
         _lib.lib().vb_set_deterministic(prev[0], prev[1])
         _det_current.ws = prev
+
+
+_offset_current = threading.local()   # .lib: the pointer this thread last handed to vb_set_dropout_offset; .fwd: see below
+
+
+@contextlib.contextmanager
+def dropout_offset(offset):
+    """Library calls inside draw every dropout with seed + *offset (vb_set_dropout_offset), offset being a one-element int64
+    device tensor that the kernels read when they run — a CUDA graph captured inside draws fresh bits at each replay once the
+    tensor has changed. Thread-local like `deterministic` (the autograd engine runs backward on its own thread), so it is set
+    around each call and the previous setting comes back on exit. offset None: nothing is called."""
+    if offset is None:
+        yield
+        return
+    prev = getattr(_offset_current, "lib", None)
+    _lib.check(_lib.lib().vb_set_dropout_offset(ctypes.c_void_p(offset.data_ptr())), "vb_set_dropout_offset")
+    _offset_current.lib = offset.data_ptr()
+    try:
+        yield
+    finally:
+        _lib.lib().vb_set_dropout_offset(ctypes.c_void_p(prev))
+        _offset_current.lib = prev
+
+
+@contextlib.contextmanager
+def forward_seed_offset(offset):
+    """The seed offset the encoder and embedding calls of one model forward record in their meta (and so their backward):
+    BertVisualModel.forward sets it in graph-capturable mode; None elsewhere."""
+    prev = getattr(_offset_current, "fwd", None)
+    _offset_current.fwd = offset
+    try:
+        yield
+    finally:
+        _offset_current.fwd = prev
+
+
+def current_seed_offset():
+    return getattr(_offset_current, "fwd", None)
+
+
+def _capturing():
+    return torch.cuda.is_available() and torch.cuda.is_current_stream_capturing()
 
 
 def cast_to_bf16(src, out=None):
@@ -414,7 +462,7 @@ class _EncoderFn(torch.autograd.Function):
         I = params[10].shape[0]
         A = meta["heads"]
         x = x.contiguous()
-        with torch.cuda.device(x.device), deterministic(x.device, M, H, I):
+        with torch.cuda.device(x.device), deterministic(x.device, M, H, I), dropout_offset(meta.get("seed_offset")):
             descs, weights, stride, off = meta["plan"].prepare(meta["caches"], params, B, S, H, A, I, mbias, meta, x.device, vl)
             arena = torch.empty(L * stride, device=x.device, dtype=torch.uint8)
             if vl is None:
@@ -451,7 +499,7 @@ class _EncoderFn(torch.autograd.Function):
             return (None,) * (3 + 16 * L)
         dy = douts[L - 1].to(_BF16).contiguous()
         grads, flat = _layer_grads(ctx.params, L, H, I, dev)
-        with torch.cuda.device(dev), deterministic(dev, M, H, I):
+        with torch.cuda.device(dev), deterministic(dev, M, H, I), dropout_offset(meta.get("seed_offset")):
             w = _bwd_scratch(dev, M, H, I, A, meta["hidden_dropout"] > 0)
             sc = _lib.LayerScratch(**{k: _ptr(t) for k, t in w.items()})
             dx = torch.empty(oshape, device=dev, dtype=_BF16)
@@ -486,7 +534,7 @@ def _encoder_infer(x, mbias, meta, params):
     x = x.detach().contiguous()
     if meta.get("attn_maps") and vl is not None:
         raise ValueError("bert_encoder: attention maps need a dense (padded) call")
-    with torch.cuda.device(x.device):
+    with torch.cuda.device(x.device), dropout_offset(meta.get("seed_offset")):
         descs = meta["plan"].prepare(meta["caches"], params, B, S, H, A, I, mbias, meta, x.device, vl)[0]
         nbytes = int(_lib.lib().vb_encoder_infer_workspace(B, S, H, A, I, 1 if meta["attn_dropout"] > 0 else 0, -1 if vl is None else M))
         if nbytes < 0:
@@ -586,10 +634,11 @@ class _EmbedFn(torch.autograd.Function):
             pos_vis=pos_vis.data_ptr(), type_vis=typ_vis.data_ptr(), gamma=gamma.data_ptr(), beta=beta.data_ptr(),
             visual_addend=_ptr(xb))
         a = _lib.EmbedActs(vis_proj=_ptr(vis_proj), pre=pre.data_ptr(), mean=mean.data_ptr(), rstd=rstd.data_ptr())
-        with torch.cuda.device(dev):
+        with torch.cuda.device(dev), dropout_offset(meta.get("seed_offset")):
             _lib.check(_lib.lib().vb_embed_fwd(ctypes.byref(d), ctypes.c_void_p(y.data_ptr()), ctypes.byref(a), _stream()),
                        "vb_embed_fwd")
         ctx.desc = d   # the backward's too: it does not read visual_addend
+        ctx.seed_offset = meta.get("seed_offset")
         ctx.shape = (B, T, V, H, Dv)
         ctx.feats_need_grad = feats is not None and feats.requires_grad
         ctx.feats_dtype = None if feats is None else feats.dtype
@@ -632,7 +681,7 @@ class _EmbedFn(torch.autograd.Function):
             dword=dword.data_ptr(), dpos=dpos.data_ptr(), dtype=dtyp.data_ptr(), dpos_vis=dpos_vis.data_ptr(),
             dtype_vis=dtyp_vis.data_ptr(), dw_proj=_ptr(dpw), db_proj=_ptr(dpb), dgamma=dgamma.data_ptr(),
             dbeta=dbeta.data_ptr(), d_pre=d_pre.data_ptr(), d_vis=_ptr(d_vis), d_feats=_ptr(d_feats))
-        with torch.cuda.device(dev), deterministic(dev, M, H, Dv):
+        with torch.cuda.device(dev), deterministic(dev, M, H, Dv), dropout_offset(ctx.seed_offset):
             _lib.check(_lib.lib().vb_embed_bwd(ctypes.byref(ctx.desc), ctypes.byref(a), ctypes.c_void_p(dy.data_ptr()),
                                                ctypes.byref(g), _stream()), "vb_embed_bwd")
         dfe = None
@@ -722,7 +771,7 @@ class _CrossEntropyFn(torch.autograd.Function):
     their gradient in place (vb_cross_entropy_bwd)."""
 
     @staticmethod
-    def forward(ctx, logits, labels, V):
+    def forward(ctx, logits, labels, V, count=None):
         n, Vp = logits.shape
         labels = labels.to(torch.int64).contiguous()
         lse = torch.empty(n, device=logits.device, dtype=torch.float32)
@@ -731,21 +780,23 @@ class _CrossEntropyFn(torch.autograd.Function):
             _lib.check(_lib.lib().vb_cross_entropy_fwd(ctypes.c_void_p(logits.data_ptr()), ctypes.c_int64(Vp),
                                                        ctypes.c_void_p(labels.data_ptr()), n, V, ctypes.c_void_p(lse.data_ptr()),
                                                        ctypes.c_void_p(rows.data_ptr()), _stream()), "vb_cross_entropy_fwd")
-        ctx.logits, ctx.labels, ctx.lse, ctx.V = logits, labels, lse, V
-        return rows.mean()
+        ctx.logits, ctx.labels, ctx.lse, ctx.V, ctx.count = logits, labels, lse, V, count
+        return rows.mean() if count is None else rows.sum() / count
 
     @staticmethod
     def backward(ctx, g):
         logits, labels, lse, V = ctx.logits, ctx.labels, ctx.lse, ctx.V
         n, Vp = logits.shape
-        scale = (g.float() / n).reshape(1).contiguous()
+        scale = (g.float() / (n if ctx.count is None else ctx.count)).reshape(1).contiguous()
         with torch.cuda.device(logits.device):
             _lib.check(_lib.lib().vb_cross_entropy_bwd(ctypes.c_void_p(logits.data_ptr()), ctypes.c_int64(Vp),
                                                        ctypes.c_void_p(labels.data_ptr()), n, V, Vp, ctypes.c_void_p(lse.data_ptr()),
                                                        ctypes.c_void_p(scale.data_ptr()), _stream()), "vb_cross_entropy_bwd")
         ctx.logits = None
-        return logits, None, None
+        return logits, None, None, None
 
 
-def cross_entropy_rows(logits, labels, V):
-    return _CrossEntropyFn.apply(logits, labels, V)
+def cross_entropy_rows(logits, labels, V, count=None):
+    """Mean cross-entropy over the rows; with `count` (a device scalar, fp32) the sum over the rows divided by it instead —
+    rows whose label is outside [0, V) contribute neither loss nor gradient, so capacity-padded rows drop out."""
+    return _CrossEntropyFn.apply(logits, labels, V, count)

@@ -107,6 +107,63 @@ def shard_batch(batch, rank, world_size):
     return out
 
 
+_TEXT_KEYS = {"input_ids": 0, "token_type_ids": 0, "input_mask": 0, "masked_lm_labels": -1}
+_REGION_KEYS = {"image_mask": 0, "visual_embeddings_type": 0, "confidence": 0}          # region dim last
+_REGION_ROW_KEYS = {"visual_embeddings": 0, "position_embeddings_visual": 0, "image_text_alignment": -1}  # region dim -2
+
+
+def pad_batch(batch, text_len, regions, entities=None):
+    """A reference batch dict padded to fixed shapes: text tensors to `text_len` positions, region tensors to `regions`
+    (CUDA graphs replay one captured shape; AllenNLP pads each batch only to its longest example, so without this no shape
+    would recur). Works for every head, 3-D VCR inputs included (the text / region dimension is found from the end).
+    Padding: ids, token types and masks 0, masked_lm_labels -1, features 0, image_text_alignment -1; the flickr head's soft
+    region targets (label [.., entities, regions]) get 0 and, with `entities`, flickr_position (-1) and label are padded to that
+    many entities too (without it the entity count of a flickr batch varies, and such batches need bucketing by it).
+    masked_lm_rows (flat indices b * (T + V) + t, -1 = capacity padding) are remapped to b * (text_len + regions) + t.
+    Semantics: the padded positions are masked keys, whose key bias of
+    -10000 gives them exactly zero probability in the fp32 softmax, so valid positions equal those of the unpadded batch to
+    within rounding (row statistics of shorter batches are summed in another order); padded positions hold finite values
+    nobody reads, and padded MLM rows carry no target."""
+    def pad(t, dim, size, value):
+        n = t.shape[dim]
+        if n > size:
+            raise ValueError(f"pad_batch: dimension {dim} of size {n} exceeds the padded size {size}")
+        if n == size:
+            return t
+        shape = list(t.shape)
+        shape[dim] = size - n
+        return torch.cat((t, t.new_full(shape, value)), dim=dim)
+
+    out = {}
+    for k, v in batch.items():
+        if not torch.is_tensor(v):
+            out[k] = v
+        elif k in _TEXT_KEYS:
+            out[k] = pad(v, -1, text_len, _TEXT_KEYS[k])
+        elif k in _REGION_KEYS:
+            out[k] = pad(v, -1, regions, _REGION_KEYS[k])
+        elif k in _REGION_ROW_KEYS:
+            out[k] = pad(v, -2, regions, _REGION_ROW_KEYS[k])
+        elif k == "label" and "flickr_position" in batch:
+            out[k] = pad(v, -1, regions, 0)
+            if entities is not None:
+                out[k] = pad(out[k], -2, entities, 0)
+        elif k == "flickr_position" and entities is not None:
+            out[k] = pad(v, -1, entities, -1)
+        elif k == "masked_lm_rows":
+            ids = batch["input_ids"]
+            T = ids.shape[-1]
+            V = batch["visual_embeddings"].shape[-2] if torch.is_tensor(batch.get("visual_embeddings")) else 0
+            b, t = torch.div(v, T + V, rounding_mode="floor"), v.remainder(T + V)
+            if T + V != text_len + regions:
+                out[k] = torch.where(v >= 0, b * (text_len + regions) + t, v)
+            else:
+                out[k] = v
+        else:
+            out[k] = v
+    return out
+
+
 class BatchPrefetcher:
     """Host→device staging of input batches on a copy stream, so the copy of batch i+1 overlaps the step on batch i.
 
@@ -122,13 +179,17 @@ class BatchPrefetcher:
             loss = step(batch)
     """
 
-    def __init__(self, device, mlm_rows=True):
+    def __init__(self, device, mlm_rows=True, mlm_rows_capacity=None):
+        """mlm_rows_capacity=N: `masked_lm_rows` always has N entries, the MLM targets followed by -1 ("no target"), so that every
+        pretraining batch of one shape gives one tensor shape (what a CUDA graph replays; the model reads -1 entries as padding
+        in graph-capturable mode, BertVisualModel.set_graph_capturable). A batch with more than N targets raises."""
         self.device = torch.device(device)
         self.stream = torch.cuda.Stream(device=self.device)
         self.mlm_rows = mlm_rows
+        self.mlm_rows_capacity = mlm_rows_capacity
 
     @staticmethod
-    def labelled_rows(host_batch):
+    def labelled_rows(host_batch, capacity=None):
         """Flat indices b * (T + V) + t of the MLM targets, from the HOST copy of the labels (what
         TrainVisualBERTObjective.forward accepts as `masked_lm_rows`): finding them on the device costs a host sync.
         Negative labels are "no target" (the reference's ignore index is -1); a label >= vocab contributes neither loss
@@ -141,11 +202,16 @@ class BatchPrefetcher:
         V = 0 if vis is None else vis.shape[-2]
         flat = labels.reshape(-1, T)
         b, t = torch.nonzero(flat >= 0, as_tuple=True)
-        return (b * (T + V) + t).to(torch.int64)
+        rows = (b * (T + V) + t).to(torch.int64)
+        if capacity is None:
+            return rows
+        if rows.numel() > capacity:
+            raise ValueError(f"BatchPrefetcher: the batch has {rows.numel()} MLM targets, more than mlm_rows_capacity = {capacity}")
+        return torch.cat((rows, torch.full((capacity - rows.numel(),), -1, dtype=torch.int64)))
 
     def stage(self, host_batch):
         if self.mlm_rows and "masked_lm_rows" not in host_batch:
-            rows = self.labelled_rows(host_batch)
+            rows = self.labelled_rows(host_batch, self.mlm_rows_capacity)
             if rows is not None:
                 host_batch = dict(host_batch, masked_lm_rows=rows.pin_memory())
         with torch.cuda.stream(self.stream):
