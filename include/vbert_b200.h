@@ -116,8 +116,10 @@ int vb_gemm_gp_tiled_ok(int32_t M, int32_t N);
 int vb_gemm(const vb_gemm_args* args, void* stream);
 
 /* ---- BertLayerNorm (M.py:162-175) -------------------------------------------------------- */
-/* y = gamma * (x - mean) / sqrt(var + eps) + beta over the last dim; x, y bf16 [rows, hidden];
- * mean / rstd (fp32 [rows]) are written when non-NULL (saved for backward). */
+/* y = gamma * (x - mean) / sqrt(var + eps) + beta over the last dim; x, y bf16 [rows, hidden] with row strides ldx, ldy;
+ * mean / rstd (fp32 [rows]) are written when non-NULL (saved for backward).
+ * The kernels move rows in 16-byte pieces: x, y, gamma and beta must be 16-byte aligned and ldx, ldy multiples of 8 that are
+ * >= hidden; in the backward dy, x, gamma, dx and dx_drop must be 16-byte aligned. A call that breaks this returns an error. */
 int vb_layernorm_fwd(const void* x, int64_t ldx, const float* gamma, const float* beta, void* y, int64_t ldy,
                      float* mean, float* rstd, int32_t rows, int32_t hidden, float eps, void* stream);
 /* dx = LN'(dy); dgamma/dbeta/dbias (fp32 [hidden]) are ACCUMULATED; dbias = column sum of the
@@ -169,7 +171,10 @@ int vb_attention_probs(const void* qkv, const float* mask_bias, float* probs, in
 
 /* ---- helpers ----------------------------------------------------------------------------- */
 /* (1 - cat(input_mask, image_mask)) * -10000 -> fp32 [batch, text+regions]  (M.py:1417, 1286-1294);
- * masks are int64 as the reference dataloaders produce them; image_mask may be NULL (all ones). */
+ * masks are int64 as the reference dataloaders produce them; image_mask may be NULL (all ones).
+ * The casts and the column sum move 16-byte vectors: src and dst of a cast, and x of vb_colsum_bf16, must be 16-byte aligned,
+ * and the column sum's ld a multiple of 8 that is >= cols; a call that breaks this returns an error. vb_cast_multi takes any
+ * alignment (a misaligned item is cast one element at a time). */
 int vb_mask_bias(const int64_t* input_mask, const int64_t* image_mask, float* out, int32_t batch, int32_t text_len,
                  int32_t num_regions, void* stream);
 int vb_cast_f32_to_bf16(const float* src, void* dst, int64_t n, void* stream); /* n % 8 == 0 */
@@ -195,7 +200,9 @@ int vb_colsum_bf16(const void* x, int64_t ld, float* out, int32_t rows, int32_t 
 /* logits bf16 [rows, ld] with valid columns [0, vocab); labels int64 [rows] in [0, vocab).
  * fwd: lse[row] = logsumexp(logits[row, :vocab]), loss_rows[row] = lse - logits[row, label].
  * bwd: logits[row, c] <- (softmax - onehot) * (*scale) for c < vocab and 0 for vocab <= c < padded_cols, IN PLACE
- *      (scale is a device scalar: upstream gradient / number of labelled rows). */
+ *      (scale is a device scalar: upstream gradient / number of labelled rows).
+ * Labels outside [0, vocab) contribute no loss and no gradient. logits must be 16-byte aligned (ld a multiple of 8); a call
+ * with a logits pointer that is not returns an error. rows = 0 launches nothing. */
 int vb_cross_entropy_fwd(const void* logits, int64_t ld, const int64_t* labels, int32_t rows, int32_t vocab, float* lse,
                          float* loss_rows, void* stream);
 int vb_cross_entropy_bwd(void* logits, int64_t ld, const int64_t* labels, int32_t rows, int32_t vocab, int32_t padded_cols,
@@ -345,7 +352,9 @@ typedef struct {
     void* d_feats; /* bf16 [batch*num_regions, visual_dim] or NULL: gradient w.r.t. the region features */
 } vb_embed_grads;
 
-/* y: bf16 [M, hidden] = dropout(LN(cat(text, visual))) */
+/* y: bf16 [M, hidden] = dropout(LN(cat(text, visual))). Ids and types outside their tables are clamped to the first or last
+ * row. The fp32 tables are read as 16-byte vectors: word, pos, type, pos_vis, type_vis, and acts->pre, acts->vis_proj and y, must
+ * be 16-byte aligned; in the backward dword, dpos and d_vis must be. A call that breaks this returns an error before launching. */
 int vb_embed_fwd(const vb_embed_desc* d, void* y, const vb_embed_acts* acts, void* stream);
 int vb_embed_bwd(const vb_embed_desc* d, const vb_embed_acts* acts, const void* dy, const vb_embed_grads* g, void* stream);
 

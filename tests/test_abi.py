@@ -91,6 +91,81 @@ def test_gemm_refuses_gelu_epilogues_with_dropout_or_addend(epi, extra):
     assert b"take no dropout and no addend" in L.vb_last_error()
 
 
+_A, _BAD = 0x10000, 0x10008   # a 16-byte aligned and an 8-byte (not 16-byte) aligned fake device pointer
+
+
+def _refused(rc, words):
+    from visualbert_b200 import _lib
+    assert rc != 0
+    assert words.encode() in _lib.lib().vb_last_error()
+
+
+def _p(v):
+    return ctypes.c_void_p(v)
+
+
+@pytest.mark.parametrize("bad", ["x", "y", "gamma", "beta", "ldx", "ldy", "ldx<H"])
+def test_layernorm_forward_refuses_what_its_vector_loads_cannot_take(bad):
+    """Every check of vb_layernorm_fwd runs before its first CUDA call: a misaligned pointer or row stride is an error."""
+    from visualbert_b200 import _lib
+    H = 64
+    a = dict(x=_A, y=_A, gamma=_A, beta=_A, ldx=H, ldy=H)
+    if bad in ("ldx", "ldy"):
+        a[bad] = H + 4
+    elif bad == "ldx<H":
+        a["ldx"] = H - 8
+    else:
+        a[bad] = _BAD
+    rc = _lib.lib().vb_layernorm_fwd(_p(a["x"]), ctypes.c_int64(a["ldx"]), _p(a["gamma"]), _p(a["beta"]), _p(a["y"]),
+                                     ctypes.c_int64(a["ldy"]), None, None, 4, H, ctypes.c_float(1e-12), None)
+    _refused(rc, "16-byte aligned" if bad in a and bad not in ("ldx", "ldy") else "must be multiples of 8 and >= H")
+
+
+@pytest.mark.parametrize("bad", ["dy", "x", "gamma", "dx", "dx_drop"])
+def test_layernorm_backward_refuses_a_misaligned_pointer(bad):
+    from visualbert_b200 import _lib
+    a = dict(dy=_A, x=_A, gamma=_A, dx=_A, dx_drop=_A)
+    a[bad] = _BAD
+    rc = _lib.lib().vb_layernorm_bwd(_p(a["dy"]), _p(a["x"]), _p(_A), _p(_A), _p(a["gamma"]), _p(a["dx"]), _p(a["dx_drop"]),
+                                     None, None, None, 4, 64, ctypes.c_float(0.1), ctypes.c_uint64(1), ctypes.c_uint32(0),
+                                     ctypes.c_float(0.0), ctypes.c_uint32(0), None)
+    _refused(rc, "16-byte aligned")
+
+
+@pytest.mark.parametrize("x,ld,words", [(_BAD, 64, "16-byte aligned"), (_A, 68, "multiple of 8"), (_A, 56, ">= N")])
+def test_colsum_refuses_a_misaligned_pointer_or_stride(x, ld, words):
+    from visualbert_b200 import _lib
+    _refused(_lib.lib().vb_colsum_bf16(_p(x), ctypes.c_int64(ld), _p(_A), 5, 64, None), words)
+
+
+@pytest.mark.parametrize("rows", [0, 3])
+def test_cross_entropy_refuses_misaligned_logits(rows):
+    from visualbert_b200 import _lib
+    L = _lib.lib()
+    _refused(L.vb_cross_entropy_fwd(_p(_BAD), ctypes.c_int64(16), _p(_A), rows, 9, _p(_A), _p(_A), None), "16-byte aligned")
+    _refused(L.vb_cross_entropy_bwd(_p(_BAD), ctypes.c_int64(16), _p(_A), rows, 9, 16, _p(_A), _p(_A), None), "16-byte aligned")
+
+
+@pytest.mark.parametrize("src,dst", [(_BAD, _A), (_A, _BAD)])
+def test_casts_refuse_a_misaligned_pointer(src, dst):
+    from visualbert_b200 import _lib
+    L = _lib.lib()
+    _refused(L.vb_cast_f32_to_bf16(_p(src), _p(dst), ctypes.c_int64(64), None), "16-byte aligned")
+    _refused(L.vb_cast_bf16_to_f32(_p(src), _p(dst), ctypes.c_int64(64), None), "16-byte aligned")
+
+
+@pytest.mark.parametrize("bad", ["word", "pos", "type", "pos_vis", "type_vis", "pre", "y"])
+def test_embedding_forward_refuses_misaligned_tables(bad):
+    """Refused before anything is launched (the projection GEMM included)."""
+    from visualbert_b200 import _lib
+    tabs = {k: (_BAD if k == bad else _A) for k in ("word", "pos", "type", "pos_vis", "type_vis", "pre", "y")}
+    d = _lib.EmbedDesc(batch=2, text_len=4, num_regions=0, hidden=64, visual_dim=0, vocab=10, max_pos=8, n_types=2, eps=1e-12,
+                       input_ids=_A, token_type_ids=_A, word=tabs["word"], pos=tabs["pos"], type=tabs["type"],
+                       pos_vis=tabs["pos_vis"], type_vis=tabs["type_vis"], gamma=_A, beta=_A)
+    acts = _lib.EmbedActs(vis_proj=0, pre=tabs["pre"], mean=_A, rstd=_A)
+    _refused(_lib.lib().vb_embed_fwd(ctypes.byref(d), _p(tabs["y"]), ctypes.byref(acts), None), "16-byte aligned")
+
+
 @pytest.mark.skipif(torch.cuda.is_available(), reason="checks the no-GPU behaviour")
 def test_product_path_fails_loudly_without_cuda():
     from visualbert_b200 import BertConfig, TrainVisualBERTObjective, _lib, synthetic

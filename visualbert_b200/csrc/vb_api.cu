@@ -326,6 +326,10 @@ static int check_embed(const vb_embed_desc* d) {
 int embed_fwd_api(const vb_embed_desc* d, void* y, const vb_embed_acts* s, cudaStream_t st) {
     VB_TRY(check_embed(d));
     VB_REQUIRE(y && s && s->pre && s->mean && s->rstd, "embed_fwd: null pointer");
+    // the embedding kernel reads the fp32 tables as float4 and moves the bf16 rows in 16-byte pieces: refused here, before the
+    // projection GEMM is launched
+    VB_REQUIRE(all_aligned16(d->word, d->pos, d->type, d->pos_vis, d->type_vis, s->pre, s->vis_proj, y),
+               "embed_fwd: the fp32 tables, pre, vis_proj and y must be 16-byte aligned");
     const int BV = d->batch * d->num_regions;
     if (BV > 0) {
         vb_gemm_args a = fwd_args(d->visual_feats, d->w_proj, s->vis_proj, BV, d->hidden, d->visual_dim);
@@ -363,6 +367,7 @@ int embed_bwd_api(const vb_embed_desc* d, const vb_embed_acts* s, const void* dy
                   cudaStream_t st) {
     VB_TRY(check_embed(d));
     VB_REQUIRE(s && dy && g && g->d_pre, "embed_bwd: null pointer");
+    VB_REQUIRE(all_aligned16(g->dword, g->dpos, g->d_vis), "embed_bwd: dword, dpos and d_vis must be 16-byte aligned");
     const int M = d->batch * (d->text_len + d->num_regions), H = d->hidden, BV = d->batch * d->num_regions;
     if (det_ws().ptr != nullptr) {   // every launch of the call fits the workspace, or nothing is launched
         const long long temp = embed_sort_temp_bytes(d->batch, d->text_len, d->num_regions);

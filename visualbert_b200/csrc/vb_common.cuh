@@ -101,6 +101,13 @@ void set_error(const char* fmt, ...);
         if (_rc) return _rc; \
     } while (0)
 
+// true when every pointer is 16-byte aligned (NULL counts as aligned): what a kernel that moves 16-byte vectors needs of the
+// pointers it is handed, checked by its entry point before the first CUDA call
+template <typename... T>
+inline bool all_aligned16(const T*... p) {
+    return ((reinterpret_cast<uintptr_t>(p) | ... | uintptr_t{0}) & 15) == 0;
+}
+
 // ---------------------------------------------------------------------------------------------
 // generic helpers
 // ---------------------------------------------------------------------------------------------

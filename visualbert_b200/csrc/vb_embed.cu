@@ -578,6 +578,7 @@ int mask_bias(const long long* input_mask, const long long* image_mask, float* o
 
 int cast_f32_bf16(const float* src, void* dst, long long n, cudaStream_t st) {
     VB_REQUIRE(n % 8 == 0, "cast: element count must be a multiple of 8");
+    VB_REQUIRE(all_aligned16(src, dst), "cast: src and dst must be 16-byte aligned");
     if (n == 0) return 0;
     const long long n8 = n / 8;
     long long blocks = (n8 + 255) / 256;
@@ -591,6 +592,7 @@ int cast_f32_bf16(const float* src, void* dst, long long n, cudaStream_t st) {
 }
 int cast_bf16_f32(const void* src, float* dst, long long n, cudaStream_t st) {
     VB_REQUIRE(n % 8 == 0, "cast: element count must be a multiple of 8");
+    VB_REQUIRE(all_aligned16(src, dst), "cast: src and dst must be 16-byte aligned");
     if (n == 0) return 0;
     const long long n8 = n / 8;
     long long blocks = (n8 + 255) / 256;
@@ -614,6 +616,8 @@ long long colsum_det_bytes(int M, int N) { return static_cast<long long>(colsum_
 
 int colsum(const void* x, long long ld, float* out, int M, int N, cudaStream_t st) {
     VB_REQUIRE(N % 8 == 0 && M > 0, "colsum: bad shape");
+    VB_REQUIRE(ld >= N && ld % 8 == 0, "colsum: ld=%lld must be a multiple of 8 and >= N=%d", ld, N);
+    VB_REQUIRE(x && out && all_aligned16(x), "colsum: x must be 16-byte aligned and out not NULL");
     const int gx = (N / 8 + 31) / 32;
     const int gy = colsum_gy(M, N);
     const DetWs det = det_ws();

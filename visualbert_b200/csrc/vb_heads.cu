@@ -107,6 +107,7 @@ ce_bwd_kernel(bf16* __restrict__ logits, long long ld, const long long* __restri
 int ce_fwd(const void* logits, long long ld, const long long* labels, int rows, int vocab, float* lse, float* loss,
            cudaStream_t st) {
     VB_REQUIRE(rows >= 0 && vocab > 0 && ld >= vocab && ld % 8 == 0, "cross-entropy: bad shape rows=%d vocab=%d ld=%lld", rows, vocab, ld);
+    VB_REQUIRE(all_aligned16(logits), "cross-entropy: logits must be 16-byte aligned");
     if (rows == 0) return 0;
     {
         ProfScope ps(st, PROF_OTHER, 2.0 * rows * vocab, 1);
@@ -120,6 +121,7 @@ int ce_bwd(void* logits, long long ld, const long long* labels, int rows, int vo
            const float* scale, cudaStream_t st) {
     VB_REQUIRE(rows >= 0 && vocab > 0 && padded >= vocab && padded % 8 == 0 && ld >= padded && ld % 8 == 0,
                "cross-entropy backward: bad shape");
+    VB_REQUIRE(all_aligned16(logits), "cross-entropy backward: logits must be 16-byte aligned");
     if (rows == 0) return 0;
     {
         ProfScope ps(st, PROF_OTHER, 4.0 * rows * padded, 1);

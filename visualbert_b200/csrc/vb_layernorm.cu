@@ -303,6 +303,10 @@ int ln_fwd(const void* x, long long ldx, const float* gamma, const float* beta, 
            float* mean, float* rstd, int rows, int H, float eps, cudaStream_t st) {
     VB_REQUIRE(H % 8 == 0 && H <= 1024 * 2, "layernorm: H=%d must be a multiple of 8 and <= 2048", H);
     VB_REQUIRE(rows > 0, "layernorm: no rows");
+    VB_REQUIRE(x && y && gamma && beta, "layernorm: x, y, gamma and beta must not be NULL");
+    VB_REQUIRE(ldx >= H && ldy >= H && ldx % 8 == 0 && ldy % 8 == 0,
+               "layernorm: ldx=%lld and ldy=%lld must be multiples of 8 and >= H=%d", ldx, ldy, H);
+    VB_REQUIRE(all_aligned16(x, y, gamma, beta), "layernorm: x, y, gamma and beta must be 16-byte aligned");
     const int nc = (H / 8 + 31) / 32;
     const int grid = (rows + kLnWarps - 1) / kLnWarps;
     const bf16* xb = static_cast<const bf16*>(x);
@@ -328,6 +332,8 @@ int ln_bwd(const void* dy, const void* x, const float* mean, const float* rstd, 
     VB_REQUIRE(H % 8 == 0 && H <= 1024, "layernorm backward: H=%d must be a multiple of 8 and <= 1024", H);
     VB_REQUIRE(rows > 0, "layernorm backward: no rows");
     VB_REQUIRE((dropout_p > 0.f) == (dx_drop != nullptr), "layernorm backward: dx_drop iff dropout_p > 0");
+    VB_REQUIRE(dy && x && mean && rstd && gamma && dx, "layernorm backward: dy, x, mean, rstd, gamma and dx must not be NULL");
+    VB_REQUIRE(all_aligned16(dy, x, gamma, dx, dx_drop), "layernorm backward: dy, x, gamma, dx and dx_drop must be 16-byte aligned");
     const int nc = (H / 8 + 31) / 32;
     const int grid = ln_bwd_grid(rows);
     const DetWs det = det_ws();
