@@ -9,18 +9,22 @@ The library has three attention paths; the sequence length alone picks one:
 Each case checks ctx, lse, dQ, dK and dV separately against the reference, that every output element is written (outputs are pre-filled with NaN), that nothing is read or written
 outside the tensors (they are views inside buffers whose guard bands hold NaN for inputs and a sentinel for outputs),
 and that two identical calls are bit-identical. With dropout, the reference applies the bits the forward stored in the
-keep buffer, so a match also shows that the forward applied exactly the stored bits."""
+keep buffer, so a match also shows that the forward applied exactly the stored bits.
+
+Every output (ctx, lse, drow = rowsum(dO ctx), dQ, dK, dV) must lie within the per-element bound of attn_ref_util.py of its
+fp64 reference. Besides unit-normal inputs, every route runs the input families of attn_ref_util.inputs: peaked rows (Q x 4 and a
++8 key bias that puts the row maximum in the last, partial key block or on key 0), a general fp32 key bias, and dO rows scaled
+by 2^-6 .. 2^6; and the staged kernels run long key loops (S = 1024, 1025, 2049) and 16 heads (H = 1024)."""
 import ctypes
 import re
 
 import pytest
 import torch
 
+import attn_ref_util as R
+
 pytestmark = pytest.mark.gpu
 
-CTX_TOL = 1.0e-2   # bf16 output rounding (2^-8 relative), relative to max |ref|
-GRAD_TOL = 2.0e-2  # per gradient, relative to max(max |ref|, problem scale), see _check_grads
-LSE_TOL = 2.0e-2   # absolute, natural-log domain
 GUARD_ROWS = 64    # guard rows around every [rows, cols] tensor: whole rows keep the views 16-byte aligned
 GUARD_FLAT = 256   # guard elements around the [B, A, S] fp32 tensors (1 KB)
 GUARD_KEEP = 1024  # guard bytes around the keep buffer
@@ -54,6 +58,14 @@ ROUTING_SEQS = [100, 200, 356]
 CASES = ([(B, S, A, 0.0) for S in SEQS for B in (1, 3) for A in (1, 2, 12)]
          + [(3, S, 12, P_FIRST) for S in DROP_SEQS]
          + [(24, S, 12, p) for S in WALK for p in (0.0, P_FIRST)])
+# the input families on every route: a partial and a full last key block of the wgmma and whole-head kernels, one and four
+# staged key blocks with a partial last one
+FAMILY_SEQS = [65, 192, 200, 256, 257, 449]
+FAMILY_CASES = ([(3, S, 2, p, fam) for fam in ("peaked", "bias", "rowscale") for S in FAMILY_SEQS for p in (0.0, P_FIRST)]
+                # long staged runs (16, 17 and 33 key blocks: 4, 5 and 9 stages) and 16 heads (cfg5, H = 1024)
+                + [(1, 1024, 2, 0.0, "unit"), (1, 1025, 2, P_FIRST, "peaked"), (1, 2049, 2, 0.0, "peaked"),
+                   (1, 2049, 2, 0.0, "bias"), (2, 164, 16, P_FIRST, "unit"), (2, 356, 16, 0.0, "unit"),
+                   (2, 356, 16, P_FIRST, "peaked")])
 
 
 def _setup():
@@ -85,26 +97,7 @@ class _Guarded:
 
 def _keep_bits(keep, B, S, A, half=0):
     """[B*A, S, S] 0/1 keep decisions from the keep buffer: half 0 = rows are queries, half 1 = its transpose."""
-    nkb = (S + 63) // 64
-    words = keep.view(torch.int64).view(2, B * A, nkb * 64, nkb)[half]
-    bits = (words.unsqueeze(-1) >> torch.arange(64, device=keep.device)) & 1
-    return bits.reshape(B * A, nkb * 64, nkb * 64)[:, :S, :S]
-
-
-def _reference(qkv, bias, dctx, keep, B, S, A, p):
-    """softmax(QK^T / 8 + bias) [* keep * 256 / (256 - round(256 p))] V in fp64, gradients by autograd."""
-    H = A * 64
-    x = qkv.double().requires_grad_(True)
-    q, k, v = x.view(B, S, 3, A, 64).permute(2, 0, 3, 1, 4)
-    sc = q @ k.transpose(-1, -2) / 8.0 + bias.double()[:, None, None, :]
-    lse = torch.logsumexp(sc, -1)
-    pr = torch.softmax(sc, -1)
-    if p > 0:
-        n = int(p * 256 + 0.5)
-        pr = pr * _keep_bits(keep, B, S, A).view(B, A, S, S).double() * (256.0 / (256 - n))
-    o = (pr @ v).permute(0, 2, 1, 3).reshape(B * S, H)
-    (g,) = torch.autograd.grad(o, x, dctx.double())
-    return o.detach(), lse.detach(), g
+    return R.keep_bits(keep, B * A, S, half)
 
 
 def _err(out, ref, scale=0.0):
@@ -112,19 +105,10 @@ def _err(out, ref, scale=0.0):
     return ((out - ref).abs().max() / max(ref.abs().max().item(), scale, 1e-30)).item()
 
 
-def _inputs(B, S, A, dev, seed, fully_masked=False):
-    """qkv and dO unit normal; ragged key lengths; with `fully_masked`, example 1 has no valid key (additive -10000, not
-    -inf: it attends uniformly over raw scores, M.py:1293)."""
-    g = torch.Generator(device=dev)
-    g.manual_seed(seed)
-    H = A * 64
-    qkv = torch.randn(B * S, 3 * H, device=dev, generator=g).bfloat16()
-    dctx = torch.randn(B * S, H, device=dev, generator=g).bfloat16()
-    lens = torch.randint(max(1, S // 2), S + 1, (B,), device=dev, generator=g)
-    bias = ((torch.arange(S, device=dev)[None, :] >= lens[:, None]).float() * -10000.0)
-    if fully_masked:
-        bias[1] = -10000.0
-    return qkv, bias.contiguous(), dctx
+def _inputs(B, S, A, dev, seed, fully_masked=False, family="unit"):
+    """qkv, bias, dO of an input family (attn_ref_util.inputs); with `fully_masked`, example 1 has no valid key (additive
+    -10000, not -inf: it attends uniformly over raw scores, M.py:1293)."""
+    return R.inputs(family, B, S, A, dev, seed, fully_masked)
 
 
 def _run(L, _lib, st, qkv, bias, dctx, B, S, A, p, dev, seed=99, stream=5, guarded=True):
@@ -143,7 +127,7 @@ def _run(L, _lib, st, qkv, bias, dctx, B, S, A, p, dev, seed=99, stream=5, guard
         "drow": _Guarded((B, A, S), torch.float32, gf, SENTINEL, dev),
     }
     T["qkv"].t.copy_(qkv); T["bias"].t.copy_(bias); T["dctx"].t.copy_(dctx)
-    for k in ("ctx", "lse", "dqkv"):
+    for k in ("ctx", "lse", "dqkv", "drow"):
         T[k].t.fill_(nan)
     keep = None
     if p > 0:
@@ -160,71 +144,67 @@ def _run(L, _lib, st, qkv, bias, dctx, B, S, A, p, dev, seed=99, stream=5, guard
     return T
 
 
-def _check_grads(dqkv, g, H, where):
-    """dQ, dK and dV each against the reference. dV = P^T dO involves no cancellation; dQ and dK go through the softmax
-    Jacobian P (dP - D), whose two terms cancel exactly at S = 1 (dQ = dK = 0) and nearly at S = 2. Their bound is
-    therefore taken against max(max |ref|, max |ref dV| / 4): for S >= 17 max |dQ| and max |dK| are above 0.6 max |dV|
-    for unit-normal inputs, so the floor only acts where the reference itself (nearly) vanishes."""
-    dv_scale = g[:, 2 * H:].abs().max().item()
-    for i, name in enumerate("QKV"):
-        scale = dv_scale / 4 if name != "V" else 0.0
-        e = _err(dqkv[:, i * H:(i + 1) * H], g[:, i * H:(i + 1) * H], scale)
-        assert e < GRAD_TOL, f"{where}: d{name} error {e:.3g}"
-
-
-def _check_case(B, S, A, p, seed, fully_masked):
-    """One forward + backward against the reference, with all checks described in the module docstring."""
+def _check_case(B, S, A, p, seed, fully_masked, family="unit"):
+    """One forward + backward against the reference, with all checks described in the module docstring. Returns the worst
+    error / bound per output."""
     _lib, L, dev, st = _setup()
     H = A * 64
-    where = f"{_path(S)} B={B} S={S} A={A} p={p}"
-    qkv, bias, dctx = _inputs(B, S, A, dev, seed, fully_masked)
+    where = f"{_path(S)} {family} B={B} S={S} A={A} p={p}"
+    qkv, bias, dctx = _inputs(B, S, A, dev, seed, fully_masked, family)
     T = _run(L, _lib, st, qkv, bias, dctx, B, S, A, p, dev)
     T2 = _run(L, _lib, st, qkv, bias, dctx, B, S, A, p, dev, guarded=False)
     torch.cuda.synchronize()
-    ctx, lse, dqkv = T["ctx"].t, T["lse"].t, T["dqkv"].t
+    ctx, lse, dqkv, drow = T["ctx"].t, T["lse"].t, T["dqkv"].t, T["drow"].t
 
     # every element written, nothing outside the tensors read (NaN guards) or written (sentinels)
-    for k in ("ctx", "lse", "dqkv"):
+    for k in ("ctx", "lse", "dqkv", "drow"):
         assert torch.isfinite(T[k].t).all(), f"{where}: {k} has unwritten (NaN) elements"
     for k, gt in T.items():
         assert gt.guards_intact(), f"{where}: guard band of {k} changed"
     # deterministic: no atomics, so a second call gives the same bits
-    for k in ("ctx", "lse", "dqkv") + (("keep",) if p > 0 else ()):
+    for k in ("ctx", "lse", "dqkv", "drow") + (("keep",) if p > 0 else ()):
         assert torch.equal(T[k].t, T2[k].t), f"{where}: {k} differs between two identical calls"
 
     keep = T["keep"].t if p > 0 else None
-    o, lse_ref, g = _reference(qkv, bias, dctx, keep, B, S, A, p)
-    e = _err(ctx, o)
-    assert e < CTX_TOL, f"{where}: ctx error {e:.3g}"
-    e = (lse.double() - lse_ref).abs().max().item()
-    assert e < LSE_TOL, f"{where}: lse error {e:.3g}"
-    _check_grads(dqkv, g, H, where)
+    q, k, v = R.dense_heads(qkv, B, S, A)
+    dO, c = R.dense_heads(dctx, B, S, A)[0], R.dense_heads(ctx, B, S, A)[0]
+    bits = _keep_bits(keep, B, S, A) if p > 0 else None
+    ref = R.reference(q, k, v, bias.repeat_interleave(A, 0), bits, R.drop_scale(p), dO, c)
+    dq, dk, dv = R.dense_heads(dqkv, B, S, A)
+    worst = R.check_all(dict(ctx=c, lse=lse.view(B * A, S), drow=drow.view(B * A, S), dq=dq, dk=dk, dv=dv), ref, where)
+    del ref
+    print(f"{where}: worst error / bound " + ", ".join(f"{n} {w:.3f}" for n, w in worst.items()))
 
     if p > 0:
-        n = int(p * 256 + 0.5)
-        q = n / 256
-        bits = _keep_bits(keep, B, S, A)
+        rate = int(p * 256 + 0.5) / 256
         if _path(S) != "staged":  # the mask kernel also writes the transpose (rows = keys); the staged path does not
             assert torch.equal(bits, _keep_bits(keep, B, S, A, half=1).transpose(1, 2)), f"{where}: transposed keep bits differ"
-        assert abs(bits.float().mean().item() - (1 - q)) < 5e-3, f"{where}: keep rate {bits.float().mean().item():.4f}"
+        assert abs(bits.float().mean().item() - (1 - rate)) < 5e-3, f"{where}: keep rate {bits.float().mean().item():.4f}"
         for kb in range((S + 63) // 64):  # per 64-key block: 6 standard deviations of a binomial rate
             blk = bits[:, :, kb * 64:(kb + 1) * 64].float()
-            tol = 6 * (q * (1 - q) / blk.numel()) ** 0.5
-            assert abs(blk.mean().item() - (1 - q)) < tol, f"{where}: keep rate {blk.mean().item():.4f} in key block {kb}"
-        o0, _, _ = _reference(qkv, bias, dctx, None, B, S, A, 0.0)
-        assert _err(ctx, o0) > 0.05, f"{where}: dropout did not change the output"
+            tol = 6 * (rate * (1 - rate) / blk.numel()) ** 0.5
+            assert abs(blk.mean().item() - (1 - rate)) < tol, f"{where}: keep rate {blk.mean().item():.4f} in key block {kb}"
+        o0 = R.reference(q, k, v, bias.repeat_interleave(A, 0), None, 1.0, dO, c)["ctx"][0]
+        assert _err(c, o0) > 0.05, f"{where}: dropout did not change the output"
+    if p > 0 and family == "unit":   # statistics sized for unit-normal rows
         # E[dropout(P)] = P: averaged over many rows the output stays close to the no-dropout one
-        assert abs(ctx.double().mean().item() - o0.mean().item()) < 5e-3, f"{where}: mean output moved"
+        assert abs(c.double().mean().item() - o0.mean().item()) < 5e-3, f"{where}: mean output moved"
         # for a fixed mask the output is linear in V: <dO, O> = <dV, V>
         lhs = (dctx.double() * ctx.double()).sum().item()
         rhs = (dqkv[:, 2 * H:].double() * qkv[:, 2 * H:].double()).sum().item()
         assert abs(lhs - rhs) < 2e-2 * max(abs(lhs), 1.0) + 2.0, f"{where}: <dO, O> = {lhs} but <dV, V> = {rhs}"
-
+    return worst
 
 
 @pytest.mark.parametrize("B,S,A,p", CASES)
 def test_attention_matches_reference(B, S, A, p):
     _check_case(B, S, A, p, seed=1000 * S + 10 * B + A, fully_masked=B == 3)
+
+
+@pytest.mark.parametrize("B,S,A,p,family", FAMILY_CASES)
+def test_attention_input_families(B, S, A, p, family):
+    """Peaked rows, a general key bias and row-scaled dO on every route; long staged runs and 16 heads."""
+    _check_case(B, S, A, p, seed=1000 * S + 10 * B + A + 7, fully_masked=family == "unit" and B > 1, family=family)
 
 
 def test_attention_fully_masked_example_stays_finite():

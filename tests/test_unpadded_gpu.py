@@ -2,7 +2,9 @@
 restatement and against the dense kernels on the same data, and BertVisualModel.set_unpadded against the goldens, the oracle
 and the padded path.
 
-The attention route is chosen from max_seq as the dense call chooses it from seq."""
+The attention route is chosen from max_seq as the dense call chooses it from seq. Every output of a varlen call (ctx, lse, drow,
+dQ, dK, dV) must lie within the per-element bound of attn_ref_util.py of its fp64 reference, with unit-normal and with peaked
+(Q x 4) rows."""
 import ctypes
 import math
 import re
@@ -11,12 +13,12 @@ import numpy as np
 import pytest
 import torch
 
+import attn_ref_util as R
 import golden_util
 import vb_oracle
 
 pytestmark = pytest.mark.gpu
 
-CTX_TOL, GRAD_TOL, LSE_TOL = 1.0e-2, 2.0e-2, 2.0e-2   # as in test_attention_reference_gpu.py
 GUARD_ROWS, GUARD_FLAT, SENTINEL = 64, 256, -12345.0
 P_DROP = 0.1
 
@@ -26,6 +28,7 @@ MIXES = [[0, 1, 63, 64, 65], [127, 128, 129, 1], [176, 177, 0, 191, 192], [193, 
          [257, 100, 0], [356, 0, 17, 200], [513, 64, 129]]
 CASES = ([(tuple(m), A, 0.0) for m in MIXES for A in (1, 12)]
          + [(tuple(m), 12, P_DROP) for m in MIXES[:2]])
+PEAKED_CASES = [(tuple(m), 2, p) for m in MIXES for p in (0.0, P_DROP)]
 
 
 def _setup():
@@ -66,7 +69,7 @@ def _run_varlen(lens, A, p, qkv, dctx, seed=99, stream=5, guarded=True):
          "dqkv": _Guarded(total * 3 * H, torch.bfloat16, gr * 3 * H, SENTINEL, dev),
          "drow": _Guarded(A * total, torch.float32, gf, SENTINEL, dev)}
     T["qkv"].t.copy_(qkv.reshape(-1)); T["dctx"].t.copy_(dctx.reshape(-1))
-    for k in ("ctx", "lse", "dqkv"):
+    for k in ("ctx", "lse", "dqkv", "drow"):
         T[k].t.fill_(nan)
     keep = None
     if p > 0:
@@ -90,71 +93,78 @@ def _keep_bits(keep, B, S, A):
     return bits.reshape(B * A, nkb * 64, nkb * 64)
 
 
-def _reference(lens, A, p, qkv, dctx, keep):
-    """Per sequence: softmax(QK^T / 8) [* keep / (1 - p_q)] V in fp64; lse [A, total]; gradients by autograd."""
-    H, B, S = A * 64, len(lens), max(lens)
-    x = qkv.double().requires_grad_(True)
-    outs, lses, r = [], [], 0
-    bits = _keep_bits(keep, B, S, A) if p > 0 else None
-    for b, n in enumerate(lens):
-        q, k, v = x[r:r + n].view(n, 3, A, 64).permute(1, 2, 0, 3)
-        sc = q @ k.transpose(-1, -2) / 8.0
-        lses.append(torch.logsumexp(sc, -1))
-        pr = torch.softmax(sc, -1)
-        if p > 0:
-            m = int(p * 256 + 0.5)
-            pr = pr * bits[b * A:(b + 1) * A, :n, :n].double() * (256.0 / (256 - m))
-        outs.append((pr @ v).permute(1, 0, 2).reshape(n, H))
-        r += n
-    o = torch.cat(outs)
-    (g,) = torch.autograd.grad(o, x, dctx.double())
-    return o.detach(), torch.cat(lses, 1).detach(), g
-
-
 def _err(out, ref, scale=0.0):
     out, ref = out.double(), ref.double()
     return ((out - ref).abs().max() / max(ref.abs().max().item(), scale, 1e-30)).item()
 
 
-def _inputs(lens, A, seed):
+def _inputs(lens, A, seed, peaked=False):
+    """qkv and dO unit normal; `peaked`: Q x 4 (scores of std ~4)."""
     g = torch.Generator(device="cuda:0")
     g.manual_seed(seed)
     total, H = sum(lens), A * 64
-    qkv = torch.randn(total, 3 * H, device="cuda:0", generator=g).bfloat16()
+    qkv = torch.randn(total, 3 * H, device="cuda:0", generator=g)
     dctx = torch.randn(total, H, device="cuda:0", generator=g).bfloat16()
-    return qkv, dctx
+    if peaked:
+        qkv[:, :H] *= 4.0
+    return qkv.bfloat16(), dctx
 
 
-def _check(lens, A, p, seed):
-    H = A * 64
-    where = f"lens={list(lens)} A={A} p={p}"
-    qkv, dctx = _inputs(lens, A, seed)
+def _check_reference(lens, A, p, qkv, dctx, T, where):
+    """Every output of one varlen call within the bound of attn_ref_util.py, sequence by sequence (no key bias; the keep bits
+    of sequence b are the [:n, :n] corner of its heads' blocks). Returns the worst error / bound per output."""
+    H, B, S, total = A * 64, len(lens), max(lens), sum(lens)
+    bits = _keep_bits(T["keep"], B, S, A) if p > 0 else None
+    ctx, dqkv = T["ctx"].t.view(total, H), T["dqkv"].t.view(total, 3 * H)
+    lse, drow = T["lse"].t.view(A, total), T["drow"].t.view(A, total)
+    outs, refs, bounds, r = {}, {}, {}, 0
+    for b, n in enumerate(lens):
+        if n == 0:
+            continue
+        q, k, v = R.varlen_heads(qkv, r, n, A)
+        dO, c = R.varlen_heads(dctx, r, n, A)[0], R.varlen_heads(ctx, r, n, A)[0]
+        keep = bits[b * A:(b + 1) * A, :n, :n] if p > 0 else None
+        ref = R.reference(q, k, v, None, keep, R.drop_scale(p), dO, c)
+        dq, dk, dv = R.varlen_heads(dqkv, r, n, A)
+        out = dict(ctx=c, lse=lse[:, r:r + n], drow=drow[:, r:r + n], dq=dq, dk=dk, dv=dv)
+        for name, o in out.items():
+            outs.setdefault(name, []).append(o)
+            refs.setdefault(name, []).append(ref[name][0])
+            bounds.setdefault(name, []).append(ref[name][1])
+        r += n
+    cat = lambda xs: torch.cat(xs, 1)
+    worst = {name: R.check(cat(outs[name]), cat(refs[name]), cat(bounds[name]), f"{where}: {name}") for name in outs}
+    print(f"{where}: worst error / bound " + ", ".join(f"{n} {w:.3f}" for n, w in worst.items()))
+    return worst
+
+
+def _check(lens, A, p, seed, peaked=False):
+    where = f"lens={list(lens)} A={A} p={p}" + (" peaked" if peaked else "")
+    qkv, dctx = _inputs(lens, A, seed, peaked)
     T = _run_varlen(lens, A, p, qkv, dctx)
     T2 = _run_varlen(lens, A, p, qkv, dctx, guarded=False)
     torch.cuda.synchronize()
-    for k in ("ctx", "lse", "dqkv"):
+    for k in ("ctx", "lse", "dqkv", "drow"):
         assert torch.isfinite(T[k].t).all(), f"{where}: {k} has unwritten (NaN) elements"
         assert torch.equal(T[k].t, T2[k].t), f"{where}: {k} differs between two identical calls"
     for k, gt in T.items():
         if k != "keep":
             assert gt.intact(), f"{where}: guard band of {k} changed"
-    total = sum(lens)
-    if total == 0:
+    if sum(lens) == 0:
         return
-    o, lse_ref, g = _reference(lens, A, p, qkv, dctx, T.get("keep"))
-    ctx, lse, dqkv = T["ctx"].t.view(total, H), T["lse"].t.view(A, total), T["dqkv"].t.view(total, 3 * H)
-    assert _err(ctx, o) < CTX_TOL, f"{where}: ctx error {_err(ctx, o):.3g}"
-    e = (lse.double() - lse_ref).abs().max().item()
-    assert e < LSE_TOL, f"{where}: lse error {e:.3g}"
-    dv_scale = g[:, 2 * H:].abs().max().item()
-    for i, name in enumerate("QKV"):
-        e = _err(dqkv[:, i * H:(i + 1) * H], g[:, i * H:(i + 1) * H], dv_scale / 4 if name != "V" else 0.0)
-        assert e < GRAD_TOL, f"{where}: d{name} error {e:.3g}"
+    _check_reference(lens, A, p, qkv, dctx, T, where)
 
 
 @pytest.mark.parametrize("lens,A,p", CASES)
 def test_varlen_attention_matches_reference(lens, A, p):
     _check(lens, A, p, seed=sum(lens) * 7 + A)
+
+
+@pytest.mark.parametrize("lens,A,p", PEAKED_CASES)
+def test_varlen_attention_peaked(lens, A, p):
+    """Scores of std ~4: the row maximum moves between key blocks, so the online-softmax rescales of the whole-head and staged
+    kernels carry weight."""
+    _check(lens, A, p, seed=sum(lens) * 11 + A, peaked=True)
 
 
 def test_varlen_attention_many_heads():
@@ -196,7 +206,8 @@ def test_varlen_matches_dense_on_same_data(lens):
     lse_d = torch.cat([lse[b, :, :n] for b, n in enumerate(lens)], 1)
     e_lse = (T["lse"].t.view(A, total) - lse_d).abs().max().item()
     print(f"lens={lens}: max rel diff ctx {e_ctx:.3g}, dqkv {e_d:.3g}, abs lse {e_lse:.3g}")
-    assert e_ctx < CTX_TOL and e_d < GRAD_TOL and e_lse < LSE_TOL
+    # the two calls run the same kernels on the same rows; they differ only where the dense call's tiles hold padded keys
+    assert e_ctx < 1e-2 and e_d < 2e-2 and e_lse < 2e-2
 
 
 @pytest.mark.parametrize("S,want", [(100, "wgmma"), (200, "head"), (356, "staged")])
