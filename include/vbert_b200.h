@@ -376,13 +376,46 @@ typedef struct {
     float lr;           /* group lr * schedule.get_lr(state['step']) */
     float weight_decay; /* group weight_decay (0 for the bias / LayerNorm group, model_wrapper.py:106-111) */
     int32_t first_chunk;
-    int32_t reserved;
+    int32_t reserved;   /* vb_bert_adam_step: ignored. vb_bert_adam_step_sched: the tensor's group, an index into `groups` */
 } vb_adam_tensor;     /* 56 bytes */
 /* table: device array [n_tensors] ordered by first_chunk; sumsq: device scratch [n_tensors] (overwritten).
  * b1/b2/eps/max_grad_norm are doubles because the reference forms (1 - b) in double precision; max_grad_norm <= 0
  * disables clipping (opt.py:272). */
 int vb_bert_adam_step(const vb_adam_tensor* table, int32_t n_tensors, int32_t n_chunks, float* sumsq, double b1, double b2,
                       double eps, double max_grad_norm, void* stream);
+
+/* BertAdam with the learning-rate schedule evaluated on the device (CUDA graphs). The same step as vb_bert_adam_step, with the
+ * same bits, except that each tensor's lr and weight decay come from its group and its own step counter when the kernels run:
+ *   lr = fp32(groups[g].lr * schedule(steps[t] / t_total))  (fp64, the operation order of optimization.py, one rounding to fp32)
+ * with g = table[t].reserved; table[t].lr and table[t].weight_decay are ignored. Every CTA of a tensor uses the step value from
+ * before the call, and the call then advances each of the n_tensors counters by exactly one (a third, small launch). Nothing is
+ * read back on the host, so a captured call replayed later reads the counters and the group table as they are then. */
+#define VB_SCHED_CONSTANT 0        /* ConstantLR: 1 */
+#define VB_SCHED_WARMUP_CONSTANT 1 /* WarmupConstantSchedule: x / warmup while x < warmup, then 1 */
+#define VB_SCHED_WARMUP_LINEAR 2   /* WarmupLinearSchedule: x / warmup, then max((x - 1) / (warmup - 1), 0) */
+#define VB_SCHED_WARMUP_COSINE 3   /* WarmupCosineSchedule: x / warmup, then 0.5 (1 + cos(pi cycles 2 (x - warmup) / (1 - warmup))) */
+typedef struct {
+    double lr;          /* the group's base lr (group['lr']) */
+    double warmup;      /* fraction of t_total, already max(warmup, 0), < 1 */
+    double t_total;     /* < 0: the multiplier is 1 whatever the kind; 0 is refused (the host schedule divides by it) */
+    double cycles;      /* VB_SCHED_WARMUP_COSINE only */
+    float weight_decay; /* fp32, as vb_adam_tensor.weight_decay */
+    int32_t schedule;   /* VB_SCHED_* */
+} vb_adam_group;        /* 40 bytes */
+/* table, groups: device arrays [n_tensors] (as for vb_bert_adam_step) and [n_groups]; steps: device int64 [n_tensors], the step
+ * counter of each tensor (state['step']), read and then advanced by one; sumsq: device scratch [n_tensors]; lr_out: NULL, or a
+ * device float [n_tensors] that receives the lr each tensor was updated with. In deterministic mode (vb_set_deterministic) the
+ * gradient norms take the fixed-order path, as in vb_bert_adam_step. The call checks its pointers, counts and b1 / b2 / eps; the
+ * contents of the device tables cannot be read on the host without a copy that a graph would freeze, so they are checked by
+ * vb_bert_adam_sched_check on the host copies the caller uploads. */
+int vb_bert_adam_step_sched(const vb_adam_tensor* table, int32_t n_tensors, int32_t n_chunks, const vb_adam_group* groups,
+                            int32_t n_groups, int64_t* steps, float* sumsq, float* lr_out, double b1, double b2, double eps,
+                            double max_grad_norm, void* stream);
+/* Host-side check of the tables vb_bert_adam_step_sched will read, on the HOST copies before they are uploaded: the chunk layout
+ * (first_chunk in order, n_chunks covering every tensor), each tensor's group index in [0, n_groups), each group's schedule kind,
+ * warmup in [0, 1) and t_total != 0. No CUDA call. */
+int vb_bert_adam_sched_check(const vb_adam_tensor* table, int32_t n_tensors, int32_t n_chunks, const vb_adam_group* groups,
+                             int32_t n_groups);
 
 #ifdef __cplusplus
 }

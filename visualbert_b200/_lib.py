@@ -70,6 +70,10 @@ AdamTensor = _struct("AdamTensor", [
     ("p", _P), ("g", _P), ("m", _P), ("v", _P), ("numel", c_i64), ("lr", c_f32), ("weight_decay", c_f32),
     ("first_chunk", c_int), ("reserved", c_int)])
 VB_ADAM_CHUNK = 32768
+AdamGroup = _struct("AdamGroup", [
+    ("lr", ctypes.c_double), ("warmup", ctypes.c_double), ("t_total", ctypes.c_double), ("cycles", ctypes.c_double),
+    ("weight_decay", c_f32), ("schedule", c_int)])
+VB_SCHED_CONSTANT, VB_SCHED_WARMUP_CONSTANT, VB_SCHED_WARMUP_LINEAR, VB_SCHED_WARMUP_COSINE = 0, 1, 2, 3
 CastItem = _struct("CastItem", [("src", _P), ("dst", _P), ("numel", c_i64), ("first_chunk", c_int), ("dst_fp32", c_int)])
 VB_CAST_CHUNK = 8192
 
@@ -83,6 +87,7 @@ EXPORTS = [
     "vb_encoder_bwd_varlen", "vb_attention_probs", "vb_encoder_attention_probs",
     "vb_encoder_infer_workspace", "vb_encoder_infer", "vb_encoder_infer_varlen",
     "vb_set_deterministic", "vb_deterministic_workspace_bytes", "vb_set_dropout_offset",
+    "vb_bert_adam_step_sched", "vb_bert_adam_sched_check",
 ]
 VB_ENCODER_ARENA_BUFFERS = 14
 ARENA_NAMES = ("qkv", "ctx", "lse", "pre1", "mean1", "rstd1", "x1", "u", "g", "pre2", "mean2", "rstd2", "keep_mask", "y")
@@ -126,6 +131,9 @@ def lib():
         h.vb_deterministic_workspace_bytes.restype = ctypes.c_int64
         h.vb_deterministic_workspace_bytes.argtypes = [c_i64, _I, _I, _I, _I]
         h.vb_set_dropout_offset.argtypes = [_P]
+        _D = ctypes.c_double
+        h.vb_bert_adam_step_sched.argtypes = [_P, _I, _I, _P, _I, _P, _P, _P, _D, _D, _D, _D, _P]
+        h.vb_bert_adam_sched_check.argtypes = [_P, _I, _I, _P, _I]
         _lib = h
     return _lib
 

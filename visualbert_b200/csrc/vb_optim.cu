@@ -7,6 +7,8 @@
 //                          p -= lr * (m / (sqrt(v) + eps) + wd * p)        (no bias correction, decoupled decay)
 // Both are HBM-bound: 4 B/param for (1), 28 B/param for (2) (read p, g, m, v; write p, m, v) — 32 B/param per step.
 // Work is cut in chunks of VB_ADAM_CHUNK elements; one CTA per chunk finds its tensor by binary search in the table.
+// vb_bert_adam_step_sched runs the same two kernels with the learning-rate schedule evaluated on the device from per-tensor step
+// counters (CUDA graphs), plus one small launch that advances the counters.
 #include "vb_internal.h"
 
 namespace vb {
@@ -72,11 +74,32 @@ __device__ __forceinline__ void adam_elem(float& p, float g, float& m, float& v,
     p -= lr * upd;
 }
 
+// The schedule multiplier of optimization.py at `step`, in its operation order. Every fp64 operation is an explicit _rn intrinsic
+// so that nothing is contracted into an FMA: the result has the bits of the host's Python doubles (cos aside: CUDA's against
+// the C library's, within an ulp).
+__device__ __noinline__ double schedule_multiplier(const vb_adam_group& gr, long long step) {
+    if (gr.t_total < 0.0) return 1.0;
+    const double x = __ddiv_rn(__ll2double_rn(step), gr.t_total);   // progress
+    if (gr.schedule == VB_SCHED_CONSTANT) return 1.0;
+    if (x < gr.warmup) return __ddiv_rn(x, gr.warmup);
+    if (gr.schedule == VB_SCHED_WARMUP_CONSTANT) return 1.0;
+    if (gr.schedule == VB_SCHED_WARMUP_LINEAR) {
+        const double y = __ddiv_rn(__dsub_rn(x, 1.0), __dsub_rn(gr.warmup, 1.0));
+        return y < 0.0 ? 0.0 : y;   // Python's max(y, 0.0): y itself unless 0.0 > y (keeps -0.0 and NaN as they are)
+    }
+    const double c = __ddiv_rn(__dsub_rn(x, gr.warmup), __dsub_rn(1.0, gr.warmup));   // VB_SCHED_WARMUP_COSINE
+    const double arg = __dmul_rn(__dmul_rn(__dmul_rn(3.141592653589793, gr.cycles), 2.0), c);
+    return __dmul_rn(0.5, __dadd_rn(1.0, cos(arg)));
+}
+
 // ORDERED = false: sumsq[t] is the tensor's sum of squares. ORDERED = true: sumsq holds one partial per chunk, and every CTA of
 // the tensor sums them in the same fixed order (thread i takes chunks i, i + 256, ... in order, then a fixed reduction tree).
-template <bool ORDERED>
+// SCHED = false: lr and weight decay from the tensor table. SCHED = true (vb_bert_adam_step_sched): from the tensor's group and
+// its step counter; thread 0 evaluates the schedule once per CTA and shares it, and the first CTA of a tensor reports its lr.
+template <bool ORDERED, bool SCHED>
 __device__ __forceinline__ void adam_update_body(const vb_adam_tensor* __restrict__ tab, int n_tensors, const float* __restrict__ sumsq,
-                                                 const AdamHyper& h) {
+                                                 const AdamHyper& h, const vb_adam_group* __restrict__ groups = nullptr,
+                                                 const long long* __restrict__ steps = nullptr, float* __restrict__ lr_out = nullptr) {
     const int t = find_tensor(tab, n_tensors, blockIdx.x);
     const vb_adam_tensor e = tab[t];
     const long long begin = static_cast<long long>(blockIdx.x - e.first_chunk) * kAdamChunk;
@@ -105,7 +128,20 @@ __device__ __forceinline__ void adam_update_body(const vb_adam_tensor* __restric
     const float* g = static_cast<const float*>(e.g);
     float* m = static_cast<float*>(e.m);
     float* v = static_cast<float*>(e.v);
-    const float lr = e.lr, wd = e.weight_decay;
+    float lr = e.lr, wd = e.weight_decay;
+    if constexpr (SCHED) {
+        __shared__ float lr_wd[2];
+        if (threadIdx.x == 0) {
+            const vb_adam_group gr = groups[e.reserved];
+            const float l = __double2float_rn(__dmul_rn(gr.lr, schedule_multiplier(gr, steps[t])));
+            lr_wd[0] = l;
+            lr_wd[1] = gr.weight_decay;
+            if (lr_out != nullptr && static_cast<int>(blockIdx.x) == e.first_chunk) lr_out[t] = l;
+        }
+        __syncthreads();
+        lr = lr_wd[0];
+        wd = lr_wd[1];
+    }
     const bool aligned = ((reinterpret_cast<uintptr_t>(p) | reinterpret_cast<uintptr_t>(g) | reinterpret_cast<uintptr_t>(m) |
                            reinterpret_cast<uintptr_t>(v)) & 15) == 0;
     long long scalar_from = begin;
@@ -134,11 +170,27 @@ __device__ __forceinline__ void adam_update_body(const vb_adam_tensor* __restric
 }
 __global__ void __launch_bounds__(kAdamThreads)
 adam_update_kernel(const vb_adam_tensor* __restrict__ tab, int n_tensors, const float* __restrict__ sumsq, const AdamHyper h) {
-    adam_update_body<false>(tab, n_tensors, sumsq, h);
+    adam_update_body<false, false>(tab, n_tensors, sumsq, h);
 }
 __global__ void __launch_bounds__(kAdamThreads)
 adam_update_ordered_kernel(const vb_adam_tensor* __restrict__ tab, int n_tensors, const float* __restrict__ part, const AdamHyper h) {
-    adam_update_body<true>(tab, n_tensors, part, h);
+    adam_update_body<true, false>(tab, n_tensors, part, h);
+}
+__global__ void __launch_bounds__(kAdamThreads)
+adam_update_sched_kernel(const vb_adam_tensor* __restrict__ tab, int n_tensors, const float* __restrict__ sumsq, const AdamHyper h,
+                         const vb_adam_group* __restrict__ groups, const long long* __restrict__ steps, float* __restrict__ lr_out) {
+    adam_update_body<false, true>(tab, n_tensors, sumsq, h, groups, steps, lr_out);
+}
+__global__ void __launch_bounds__(kAdamThreads)
+adam_update_sched_ordered_kernel(const vb_adam_tensor* __restrict__ tab, int n_tensors, const float* __restrict__ part,
+                                 const AdamHyper h, const vb_adam_group* __restrict__ groups, const long long* __restrict__ steps,
+                                 float* __restrict__ lr_out) {
+    adam_update_body<true, true>(tab, n_tensors, part, h, groups, steps, lr_out);
+}
+// after the update (stream order: every CTA of it has read its tensor's counter): each tensor's step counter advances by one
+__global__ void __launch_bounds__(kAdamThreads) adam_step_advance_kernel(long long* __restrict__ steps, int n_tensors) {
+    const int i = blockIdx.x * kAdamThreads + threadIdx.x;
+    if (i < n_tensors) steps[i] += 1;
 }
 
 int bert_adam_step(const vb_adam_tensor* table, int n_tensors, int n_chunks, float* sumsq, double b1, double b2, double eps,
@@ -174,6 +226,66 @@ int bert_adam_step(const vb_adam_tensor* table, int n_tensors, int n_chunks, flo
         adam_update_kernel<<<n_chunks, kAdamThreads, 0, st>>>(table, n_tensors, sumsq, h);
     }
     VB_CHECK_CUDA(cudaGetLastError());
+    return 0;
+}
+
+int bert_adam_step_sched(const vb_adam_tensor* table, int n_tensors, int n_chunks, const vb_adam_group* groups, int n_groups,
+                         long long* steps, float* sumsq, float* lr_out, double b1, double b2, double eps, double max_grad_norm,
+                         cudaStream_t st) {
+    VB_REQUIRE(table != nullptr && groups != nullptr && steps != nullptr && sumsq != nullptr,
+               "vb_bert_adam_step_sched: null table / groups / steps / scratch");
+    VB_REQUIRE(n_tensors > 0 && n_chunks >= n_tensors, "vb_bert_adam_step_sched: bad tensor / chunk counts");
+    VB_REQUIRE(n_groups > 0, "vb_bert_adam_step_sched: no groups");
+    VB_REQUIRE(b1 >= 0.0 && b1 < 1.0 && b2 >= 0.0 && b2 < 1.0 && eps >= 0.0, "vb_bert_adam_step_sched: bad b1 / b2 / eps");
+    const AdamHyper h{static_cast<float>(b1), static_cast<float>(1.0 - b1), static_cast<float>(b2), static_cast<float>(1.0 - b2),
+                      static_cast<float>(eps), static_cast<float>(max_grad_norm)};
+    const DetWs det = det_ws();
+    if (det.ptr != nullptr) {
+        VB_TRY_RC(det_require(4LL * n_chunks, "vb_bert_adam_step_sched"));
+        float* part = static_cast<float*>(det.ptr);
+        if (max_grad_norm > 0.0) {
+            ProfScope ps(st, PROF_OTHER, 0.0, 1);
+            adam_sumsq_part_kernel<<<n_chunks, kAdamThreads, 0, st>>>(table, n_tensors, part);
+        }
+        ProfScope ps(st, PROF_OTHER, 0.0, 1);
+        adam_update_sched_ordered_kernel<<<n_chunks, kAdamThreads, 0, st>>>(table, n_tensors, part, h, groups, steps, lr_out);
+    } else {
+        if (max_grad_norm > 0.0) {
+            VB_CHECK_CUDA(cudaMemsetAsync(sumsq, 0, sizeof(float) * n_tensors, st));
+            ProfScope ps(st, PROF_OTHER, 0.0, 1);
+            adam_sumsq_kernel<<<n_chunks, kAdamThreads, 0, st>>>(table, n_tensors, sumsq);
+        }
+        ProfScope ps(st, PROF_OTHER, 0.0, 1);
+        adam_update_sched_kernel<<<n_chunks, kAdamThreads, 0, st>>>(table, n_tensors, sumsq, h, groups, steps, lr_out);
+    }
+    {
+        ProfScope ps(st, PROF_OTHER, 0.0, 1);
+        adam_step_advance_kernel<<<(n_tensors + kAdamThreads - 1) / kAdamThreads, kAdamThreads, 0, st>>>(steps, n_tensors);
+    }
+    VB_CHECK_CUDA(cudaGetLastError());
+    return 0;
+}
+
+int bert_adam_sched_check(const vb_adam_tensor* table, int n_tensors, int n_chunks, const vb_adam_group* groups, int n_groups) {
+    VB_REQUIRE(table != nullptr && groups != nullptr, "vb_bert_adam_sched_check: null table / groups");
+    VB_REQUIRE(n_tensors > 0 && n_groups > 0, "vb_bert_adam_sched_check: no tensors / groups");
+    for (int g = 0; g < n_groups; ++g) {
+        const vb_adam_group& gr = groups[g];
+        VB_REQUIRE(gr.schedule >= VB_SCHED_CONSTANT && gr.schedule <= VB_SCHED_WARMUP_COSINE,
+                   "vb_bert_adam_sched_check: group %d has an unknown schedule kind %d", g, gr.schedule);
+        VB_REQUIRE(gr.warmup >= 0.0 && gr.warmup < 1.0, "vb_bert_adam_sched_check: group %d has warmup %g outside [0, 1)", g,
+                   gr.warmup);
+        VB_REQUIRE(gr.t_total != 0.0, "vb_bert_adam_sched_check: group %d has t_total 0", g);
+    }
+    long long chunk = 0;
+    for (int t = 0; t < n_tensors; ++t) {
+        const vb_adam_tensor& e = table[t];
+        VB_REQUIRE(e.reserved >= 0 && e.reserved < n_groups, "vb_bert_adam_sched_check: tensor %d has group index %d out of range "
+                   "[0, %d)", t, e.reserved, n_groups);
+        VB_REQUIRE(e.numel > 0 && e.first_chunk == chunk, "vb_bert_adam_sched_check: tensor %d: bad numel / first_chunk", t);
+        chunk += (e.numel + kAdamChunk - 1) / kAdamChunk;
+    }
+    VB_REQUIRE(chunk == n_chunks, "vb_bert_adam_sched_check: the tensors cover %lld chunks, not n_chunks = %d", chunk, n_chunks);
     return 0;
 }
 
@@ -235,5 +347,15 @@ int vb_cast_multi(const vb_cast_item* table, int32_t n_items, int32_t n_chunks, 
 int vb_bert_adam_step(const vb_adam_tensor* table, int32_t n_tensors, int32_t n_chunks, float* sumsq, double b1, double b2,
                       double eps, double max_grad_norm, void* stream) {
     return vb::bert_adam_step(table, n_tensors, n_chunks, sumsq, b1, b2, eps, max_grad_norm, static_cast<cudaStream_t>(stream));
+}
+int vb_bert_adam_step_sched(const vb_adam_tensor* table, int32_t n_tensors, int32_t n_chunks, const vb_adam_group* groups,
+                            int32_t n_groups, int64_t* steps, float* sumsq, float* lr_out, double b1, double b2, double eps,
+                            double max_grad_norm, void* stream) {
+    return vb::bert_adam_step_sched(table, n_tensors, n_chunks, groups, n_groups, reinterpret_cast<long long*>(steps), sumsq, lr_out,
+                                    b1, b2, eps, max_grad_norm, static_cast<cudaStream_t>(stream));
+}
+int vb_bert_adam_sched_check(const vb_adam_tensor* table, int32_t n_tensors, int32_t n_chunks, const vb_adam_group* groups,
+                             int32_t n_groups) {
+    return vb::bert_adam_sched_check(table, n_tensors, n_chunks, groups, n_groups);
 }
 }

@@ -6,8 +6,10 @@ Dropout stays correct because the model runs in graph-capturable mode (BertVisua
 is a device tensor that the graph itself increments, and the kernels read the dropout seed offset from device memory when they
 run (vb_set_dropout_offset). Every replay therefore draws the masks an eager step would draw at the same dropout state.
 
-The optimizer stays outside the graph (BertAdam computes each tensor's learning rate on the host); it updates the parameters in
-place, and every replay re-casts the compute weights from them.
+The optimizer step can be part of the graph: GraphedStep(model, sync, optimizer=opt) with a visualbert_b200.BertAdam switches it
+to graph-capturable mode (BertAdam.set_graph_capturable), where the kernels evaluate the learning-rate schedule from step
+counters in device memory. Without `optimizer` it stays outside, as any other optimizer must: it updates the parameters in place
+after the replay, and every replay re-casts the compute weights from them.
 """
 import collections
 
@@ -23,8 +25,9 @@ def _signature(batch):
 
 
 class _Captured:
-    def __init__(self, graph, inputs, outputs):
+    def __init__(self, graph, inputs, outputs, opt_signature=None, opt_params=()):
         self.graph, self.inputs, self.outputs = graph, inputs, outputs
+        self.opt_signature, self.opt_params = opt_signature, opt_params
 
 
 class GraphedStep:
@@ -41,12 +44,24 @@ class GraphedStep:
     cache of `max_graphs` entries, each with its own memory pool (replays of different shapes interleave in any order, so pools
     are not shared); an evicted graph is freed. Raises ValueError for what cannot be captured (see set_graph_capturable, the
     vqa_advanced head, MLM rows that are not given); nothing is cached then. Pretraining batches give one shape when their
-    masked_lm_rows have a fixed capacity (parallel.BatchPrefetcher(mlm_rows_capacity=N))."""
+    masked_lm_rows have a fixed capacity (parallel.BatchPrefetcher(mlm_rows_capacity=N)).
 
-    def __init__(self, model, sync, loss_scale=None, warmup=1, max_graphs=4):
+    optimizer: None (the caller steps its optimizer after each call), or a visualbert_b200.BertAdam, which is switched to
+    graph-capturable mode and stepped at the end of every step, after the all-reduce. Before each replay its group table is
+    uploaded if a group's lr, weight decay or schedule changed; a graph whose optimizer tables were rebuilt since its capture
+    (load_state_dict, a new set of tensors) or whose (b1, b2, e, max_grad_norm) changed is dropped and captured again. With
+    gradient accumulation the optimizer must stay outside (it steps once per several calls)."""
+
+    def __init__(self, model, sync, loss_scale=None, warmup=1, max_graphs=4, optimizer=None):
         if not model.training:
             raise ValueError("GraphedStep: the model must be in training mode")
-        self.model, self.sync = model, sync
+        if optimizer is not None:
+            from .optimization import BertAdam
+            if not isinstance(optimizer, BertAdam):
+                raise ValueError("GraphedStep: only a visualbert_b200.BertAdam can be captured with the step (its schedule runs on "
+                                 f"the device), not {type(optimizer).__name__}; step other optimizers after each call")
+            optimizer.set_graph_capturable(True)
+        self.model, self.sync, self.optimizer = model, sync, optimizer
         self.loss_scale = loss_scale
         self.warmup = int(warmup)
         self.max_graphs = int(max_graphs)
@@ -63,6 +78,8 @@ class GraphedStep:
         (loss if scale == 1.0 else loss * scale).backward()
         if self.sync.world_size() > 1:
             self.sync.allreduce(prescaled=True)
+        if self.optimizer is not None:
+            self.optimizer.step()
         return out
 
     def _eager(self, batch):
@@ -76,16 +93,29 @@ class GraphedStep:
         return out
 
     def _capture(self, batch):
+        opt = self.optimizer
+        if opt is not None and not opt._capturable:
+            raise ValueError("GraphedStep: the optimizer left graph-capturable mode (BertAdam.set_graph_capturable(False)); "
+                             "every replay would apply the captured step's learning rates")
         inputs = {k: (v.clone() if torch.is_tensor(v) else v) for k, v in batch.items()}
         graph = torch.cuda.CUDAGraph()
         torch.cuda.synchronize()
         with torch.cuda.graph(graph):   # a private memory pool per graph
             outputs = self._step(inputs)
-        return _Captured(graph, inputs, outputs)
+        if opt is None:
+            return _Captured(graph, inputs, outputs)
+        return _Captured(graph, inputs, outputs, opt._graph_signature(), opt._graph_params())
 
     def __call__(self, batch):
         sig = _signature(batch)
         entry = self.graphs.get(sig)
+        if entry is not None and self.optimizer is not None:
+            if entry.opt_signature != self.optimizer._graph_signature():   # the graph holds stale pointers or arguments
+                del self.graphs[sig]
+                entry.graph.reset()
+                entry = None
+            else:
+                self.optimizer.sync_group_table()   # a stream-ordered upload outside the graph, only on a change
         if entry is None:
             n = self._eager_calls.get(sig, 0)
             if n < self.warmup:
@@ -106,4 +136,7 @@ class GraphedStep:
                 if torch.is_tensor(v):
                     v.copy_(batch[k])
         entry.graph.replay()
+        if entry.opt_params:
+            # the optimizer kernels wrote the parameters through raw pointers, as the eager step does
+            torch.autograd.graph.increment_version(entry.opt_params)
         return entry.outputs
