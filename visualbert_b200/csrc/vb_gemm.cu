@@ -3,11 +3,13 @@
 // One warp-specialised kernel computes D[M,N] = epi(sum_k A(m,k) B(n,k)) in bf16 with fp32 accumulation,
 // one 128 x BLOCK_N tile per CTA (BLOCK_N = 256, or 128 for narrow / ragged N):
 //   warpgroup 0     TMA producer  (one elected thread: cp.async.bulk.tensor, 128B-swizzled 64-wide k-slabs,
-//                                  4-stage mbarrier ring)
-//   warpgroups 1-2  MMA + epilogue (wgmma.mma_async 64 x 128 x 16 from shared-memory descriptors, fp32 accumulators in
-//                                  registers, 64 rows per warpgroup; then the tile goes through shared memory so that a
-//                                  thread owns 16-column pieces of one row for bias / dropout / residual / GELU / GELU'
-//                                  and 32-byte stores, or fp32 red.add for split-K weight gradients)
+//                                  4-stage mbarrier ring; after the last k-slab, the epilogue operand — residual /
+//                                  gelu' / O — into the slots that drained first)
+//   warpgroups 1-2  MMA + epilogue (wgmma.mma_async 64 x 256 x 16, or 64 x 128 x 16 on 128-wide tiles, from shared-memory
+//                                  descriptors, fp32 accumulators in registers, 64 rows per warpgroup; bf16 outputs:
+//                                  bias / dropout / residual / GELU / GELU' on the accumulator fragment, stmatrix into
+//                                  the drained ring, a TMA store per 64 columns; fp32 outputs: the tile goes through
+//                                  shared memory for red.add of split-K weight gradients)
 //
 // Replaces every nn.Linear on the path (reference modeling.py:232-234 Q/K/V, 271 attention output,
 // 303 intermediate, 316 output, 1220 visual projection) together with the element-wise work that
@@ -99,13 +101,21 @@ struct Cfg {
     static constexpr int A_BYTES = BLOCK_M * BLOCK_K * 2;
     static constexpr int B_BYTES = BLOCK_N * BLOCK_K * 2;
     static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
-    // fp32 accumulator tile for the epilogue, written over the drained operand ring; +4 floats per row keeps the
-    // row-per-lane reads of the epilogue free of bank conflicts
+    // fp32 outputs: the accumulator tile goes through shared memory over the drained operand ring; +4 floats per row keeps the
+    // row-per-lane reads of that epilogue free of bank conflicts
     static constexpr int ACC_LD = BLOCK_N + 4;
     static constexpr int RING_BYTES = kStages * STAGE_BYTES > BLOCK_M * ACC_LD * 4 ? kStages * STAGE_BYTES : BLOCK_M * ACC_LD * 4;
+    // bf16 outputs: the ring is reused in 16 KB pieces (128 rows x 64 columns of bf16, 128B-swizzled like the k-slabs), taken
+    // in the order in which the slots drain (see piece_addr): pieces [0, OPND) receive the epilogue operand while the last
+    // k-blocks still compute, pieces [OPND, OPND + 2 OPND) stage the one or two bf16 outputs for the TMA stores
+    static constexpr int PIECE = 16384;
+    static constexpr int PIECES_PER_SLOT = STAGE_BYTES / PIECE;
+    static constexpr int OPND = BLOCK_N / 64;
+    static constexpr int OPND_SLOTS = (OPND + PIECES_PER_SLOT - 1) / PIECES_PER_SLOT;
+    static_assert(STAGE_BYTES % PIECE == 0 && 3 * OPND <= kStages * PIECES_PER_SLOT, "operand + two output tiles fit the ring");
     static constexpr int BAR_OFF = RING_BYTES;
-    static constexpr int NUM_BARS = 2 * kStages;
-    static constexpr int BIAS_OFF = BAR_OFF + NUM_BARS * 8;
+    static constexpr int NUM_BARS = 2 * kStages + 1;   // full / empty per slot, + the epilogue operand
+    static constexpr int BIAS_OFF = (BAR_OFF + NUM_BARS * 8 + 15) / 16 * 16;
     static constexpr int SMEM_BYTES = BIAS_OFF + BLOCK_N * 4 + 1024;  // +1024: manual 1 KB alignment
     static_assert(SMEM_BYTES <= 227 * 1024, "shared memory per block");
 };
@@ -157,40 +167,15 @@ __device__ __forceinline__ TileCoord decode_tile(int t, int n_blocks, int splits
     return c;
 }
 
-// Epilogue for 16 consecutive columns of one row held as fp32 in x[16]. All global traffic is
-// 32 bytes per thread per access (two 128-bit accesses): a thread owns a row, so 32-byte pieces are the
-// unit that keeps every DRAM/L2 sector fully written.
-__device__ __forceinline__ void load16_bf16(const bf16* p, float (&f)[16]) {
-    uint32_t r[8];
-    ldg_v8(p, r);
-#pragma unroll
-    for (int i = 0; i < 8; ++i) {
-        const float2 t = unpack_bf16x2(r[i]);
-        f[2 * i] = t.x;
-        f[2 * i + 1] = t.y;
-    }
-}
-__device__ __forceinline__ void store16_bf16(bf16* p, const float (&f)[16]) {
-    uint32_t r[8];
-#pragma unroll
-    for (int i = 0; i < 8; ++i) r[i] = pack_bf16x2(f[2 * i], f[2 * i + 1]);
-    stg_v8(p, r);
-}
-
-// `sbias` points at the 16 staged bias values of these columns in shared memory (or nullptr).
-// `ex` holds the 16 bf16 of the residual (addend) or of gelu'(u) (aux_in) for these columns, prefetched by the
-// caller before the accumulators are staged, so the row-strided global load never sits on the critical path.
-// EPI selects the epilogue at COMPILE time: the generic form (every option a run-time branch, all chunks unrolled) is several
-// times larger than one specialised path, and instruction-cache misses then stall the epilogue. A specialised kernel carries
-// only its path.
-// _T: gelu'(u) is kept in the TILE-NATIVE layout (vb_gemm_args.gp_tiled): the only reader of that tensor is the epilogue of the
-// backward GEMM, where the same thread holds the same 16 columns — so it is stored in 1 KB blocks (one per epilogue warp and
-// chunk, row r of the warp's 32 at block + 32 r bytes) that both epilogues access in contiguous pieces.
+// EPI selects the epilogue at COMPILE time: the generic form (every option a run-time branch) is several times larger than one
+// specialised path, and instruction-cache misses then stall the epilogue. A specialised kernel carries only its path.
+// _T: gelu'(u) is kept in the TILE-NATIVE layout (vb_gemm_args.gp_tiled, include/vbert_b200.h): the 64 KB of one tile are
+// contiguous, so the GELU epilogue stores them and the backward GEMM's epilogue loads them with one bulk copy per 16 KB.
 // EPI_DELTA: plain bf16 store plus the attention backward's D[b, head, s] = sum_d dO[row, head, d] * O[row, head, d] (vb_gemm_args.delta_*):
-// the GEMM that PRODUCES dO (input gradient of attention.output.dense) has, in each epilogue thread, 128 consecutive columns of one row —
-// two whole heads — so the row-wise dot product with O needs no exchange; O is read like a residual operand.
-// EPI_GELU_ONLY (VB_EPI_GELU_FWD of the ABI): D = gelu(u) and nothing else — the forward-only FFN-up GEMM. It takes the plain
-// bf16 store path (one coalesced store per element) with the gelu of the two-tensor epilogues.
+// the GEMM that PRODUCES dO (input gradient of attention.output.dense) has whole heads in each tile; O is loaded like a residual
+// operand, and each row's dot products are taken in column order from the staged dO and O once the tile is staged.
+// EPI_GELU_ONLY (VB_EPI_GELU_FWD of the ABI): D = gelu(u) and nothing else — the forward-only FFN-up GEMM, with the gelu of the
+// two-tensor epilogues.
 // EPI_SLAB (fp32 output, deterministic mode): split s STORES its partial tile to slab s of the workspace, D = slab base with
 // ldd = N, slab s at D + s * M * N, no bias; splitk_reduce_kernel then adds bias + the slabs in split order into the real D.
 enum { EPI_GENERIC = 0, EPI_BIAS = 1, EPI_RESID = 2, EPI_DROP_RESID = 3, EPI_GELU_FWD = 4, EPI_DGELU_BWD = 5, EPI_GELU_FWD_T = 6,
@@ -200,87 +185,35 @@ enum { EPI_GENERIC = 0, EPI_BIAS = 1, EPI_RESID = 2, EPI_DROP_RESID = 3, EPI_GEL
 __host__ __device__ constexpr bool epi_is_generic(int e) { return e == EPI_GENERIC || e == EPI_GENERIC_OFF; }
 __host__ __device__ constexpr bool epi_is_gelu(int e) { return e == EPI_GELU_FWD || e == EPI_GELU_FWD_T; }
 __host__ __device__ constexpr bool epi_is_dgelu(int e) { return e == EPI_DGELU_BWD || e == EPI_DGELU_BWD_T; }
+// the epilogue reads a [128, BLOCK_N] bf16 operand (residual, gelu'(u) or O): compile-time "may", run-time "does"
+__host__ __device__ constexpr bool epi_may_read(int e) {
+    return e == EPI_RESID || e == EPI_DROP_RESID || epi_is_dgelu(e) || e == EPI_DELTA || epi_is_generic(e);
+}
+__device__ __forceinline__ bool epi_reads(int e, const GemmParams& p) {
+    return e == EPI_RESID || e == EPI_DROP_RESID || epi_is_dgelu(e) || e == EPI_DELTA ||
+           (epi_is_generic(e) && (p.addend != nullptr || p.epilogue == VB_EPI_DGELU));
+}
 
-// TO_REGS: nothing is stored; the 16 bf16 results are returned packed in o0 (what goes to D) and, for the GELU epilogue,
-// o1 (what goes to aux_out) — the caller stores them.
-template <bool OUT_F32, int EPI = EPI_GENERIC, bool TO_REGS = false>
-__device__ __forceinline__ void epilogue16(const GemmParams& p, int row, int col, const float* sbias, const uint32_t (&ex)[8],
-                                           float (&x)[16], uint32_t* o0 = nullptr, uint32_t* o1 = nullptr) {
-    if (sbias != nullptr) {
-#pragma unroll
-        for (int i = 0; i < 4; ++i) {
-            const float4 b = *reinterpret_cast<const float4*>(sbias + 4 * i);  // warp-uniform address: broadcast
-            x[4 * i] += b.x; x[4 * i + 1] += b.y; x[4 * i + 2] += b.z; x[4 * i + 3] += b.w;
-        }
-    }
-    if constexpr (OUT_F32) {
-        float* d = reinterpret_cast<float*>(p.D) + static_cast<long long>(row) * p.ldd + col;
-#pragma unroll
-        for (int i = 0; i < 4; ++i) red_add_v4_f32(d + 4 * i, x[4 * i], x[4 * i + 1], x[4 * i + 2], x[4 * i + 3]);
-    } else {
-        constexpr bool kGeneric = epi_is_generic(EPI);
-        if (EPI == EPI_DROP_RESID || (kGeneric && p.drop_scale != 0.0f)) {
-            const unsigned long long e8 =
-                (static_cast<unsigned long long>(row) * static_cast<unsigned>(p.N) + col) >> 3;
-#pragma unroll
-            for (int h = 0; h < 2; ++h) {
-                const uint32_t keep = dropout_keep8(EPI == EPI_GENERIC_OFF ? p.drop_seed + *p.drop_offset : p.drop_seed, p.drop_stream, e8 + h,
-                                                    p.drop_thresh16);
-#pragma unroll
-                for (int i = 0; i < 8; ++i) x[8 * h + i] = ((keep >> i) & 1u) ? x[8 * h + i] * p.drop_scale : 0.0f;
-            }
-        }
-        if (EPI == EPI_RESID || EPI == EPI_DROP_RESID || (kGeneric && p.addend != nullptr)) {   // (EPI_DELTA reads ex in the caller)
-#pragma unroll
-            for (int i = 0; i < 8; ++i) {
-                const float2 t = unpack_bf16x2(ex[i]);
-                x[2 * i] += t.x;
-                x[2 * i + 1] += t.y;
-            }
-        }
-        bf16* d = reinterpret_cast<bf16*>(p.D) + static_cast<long long>(row) * p.ldd + col;
-        if (EPI == EPI_GELU_ONLY) {
-            // D <- gelu(u): the value the GELU epilogue below sends to aux_out, from the same function; its derivative is dropped
-#pragma unroll
-            for (int i = 0; i < 16; ++i) {
-                float gp;
-                gelu_fwd_bwd(x[i], x[i], gp);
-            }
-        } else if (epi_is_gelu(EPI) || (kGeneric && p.epilogue == VB_EPI_GELU)) {
-            // aux_out <- gelu(u) (operand of the next GEMM), D <- gelu'(u) (all the backward needs of u)
-            float gp[16];
-#pragma unroll
-            for (int i = 0; i < 16; ++i) gelu_fwd_bwd(x[i], x[i], gp[i]);
-            if constexpr (TO_REGS) {
-#pragma unroll
-                for (int i = 0; i < 8; ++i) { o0[i] = pack_bf16x2(gp[2 * i], gp[2 * i + 1]); o1[i] = pack_bf16x2(x[2 * i], x[2 * i + 1]); }
-                return;
-            }
-            store16_bf16(d, gp);
-            d = p.aux_out + static_cast<long long>(row) * p.ld_aux + col;
-        } else if (epi_is_dgelu(EPI) || (kGeneric && p.epilogue == VB_EPI_DGELU)) {
-#pragma unroll
-            for (int i = 0; i < 8; ++i) {
-                const float2 t = unpack_bf16x2(ex[i]);
-                x[2 * i] *= t.x;
-                x[2 * i + 1] *= t.y;
-            }
-        }
-        if constexpr (TO_REGS) {
-#pragma unroll
-            for (int i = 0; i < 8; ++i) o0[i] = pack_bf16x2(x[2 * i], x[2 * i + 1]);
-            return;
-        }
-        store16_bf16(d, x);
-    }
+template <int BLOCK_N, int TA, int TB>
+__device__ __forceinline__ void wgmma_tile(float (&acc)[BLOCK_N / 2], uint64_t ad, uint64_t bd, uint32_t accumulate) {
+    if constexpr (BLOCK_N == 256) wgmma_m64n256k16<TA, TB>(acc, ad, bd, accumulate);
+    else wgmma_m64n128k16<TA, TB>(acc, ad, bd, accumulate);
+}
+
+// byte offset of element (row, col) of a 128 x 256 tile in the tile-native gelu'(u) layout (include/vbert_b200.h): eight 8 KB
+// blocks (column half, 32-row group), in each eight 1 KB blocks of 16 columns, row r of the 32 at + 32 r
+__device__ __forceinline__ uint32_t tn_byte(int row, int col) {
+    return ((((col >> 7) * 4 + (row >> 5)) * 8 + ((col & 127) >> 4)) * 512 + (row & 31) * 16 + (col & 15)) * 2;
 }
 
 template <bool A_MN, bool B_MN, int BLOCK_N, bool OUT_F32, int EPI = EPI_GENERIC>
 __global__ void __launch_bounds__(kThreads, 1)
-gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const GemmParams p) {
+gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const GemmParams p,
+                  const __grid_constant__ CUtensorMap tmD, const __grid_constant__ CUtensorMap tmX, const __grid_constant__ CUtensorMap tmE) {
     using C = Cfg<BLOCK_N>;
-    static_assert(BLOCK_N % 128 == 0, "64 x 128 wgmma pieces");
+    static_assert(BLOCK_N == 128 || BLOCK_N == 256, "64 x 128 / 64 x 256 wgmma tiles");
     static_assert(!(EPI == EPI_GELU_FWD_T || EPI == EPI_DGELU_BWD_T) || BLOCK_N == 256, "tile-native gelu' is defined on 256-wide tiles");
+    static_assert(!(EPI == EPI_DELTA) || BLOCK_N == 256, "EPI_DELTA: four whole heads per tile");
     extern __shared__ uint8_t smem_raw[];
     const uint32_t raw = smem_u32(smem_raw);
     const uint32_t base = (raw + 1023u) & ~1023u;  // SWIZZLE_128B tiles need 1 KB alignment
@@ -293,6 +226,7 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
     auto b_tile = [&](int s) { return base + s * C::STAGE_BYTES + C::A_BYTES; };
     auto full_bar = [&](int s) { return base + C::BAR_OFF + 8 * s; };
     auto empty_bar = [&](int s) { return base + C::BAR_OFF + 8 * (kStages + s); };
+    const uint32_t opnd_bar = base + C::BAR_OFF + 8 * (2 * kStages);
 
     if (threadIdx.x == 0) {
         tma_prefetch_desc(&tmA);
@@ -301,6 +235,7 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
             mbar_init(full_bar(s), 1);
             mbar_init(empty_bar(s), 2);   // one arrival per MMA warpgroup
         }
+        mbar_init(opnd_bar, 1);
         fence_barrier_init();
     }
     __syncthreads();
@@ -311,6 +246,13 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
     const int n_blocks = (p.N + BLOCK_N - 1) / BLOCK_N;
     const int k_blocks = (p.K + BLOCK_K - 1) / BLOCK_K;
     const TileCoord tc = decode_tile(blockIdx.x, n_blocks, p.splits, k_blocks, m_blocks, p.m_fast != 0);
+    // piece k of the ring (bf16 outputs): the slots in the order in which they drain — the slot the next k-block would have
+    // used first (its last k-block is the oldest), PIECES_PER_SLOT pieces per slot
+    const int n_kb = tc.kb_end - tc.kb_begin;
+    auto piece_addr = [&](int k) {
+        return base + ((n_kb + k / C::PIECES_PER_SLOT) % kStages) * C::STAGE_BYTES + (k % C::PIECES_PER_SLOT) * C::PIECE;
+    };
+    const long long tn_tile = ((static_cast<long long>(tc.m_blk >> 1) * n_blocks + tc.n_blk) * 2 + (tc.m_blk & 1)) * (BLOCK_M * BLOCK_N);
 
     if (warp < 4) {
         reg_dec<40>();
@@ -340,6 +282,30 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
                 __syncwarp();
                 if (++stage == kStages) { stage = 0; phase ^= 1u; }
             }
+            if constexpr (!OUT_F32 && epi_may_read(EPI)) {
+                if (epi_reads(EPI, p)) {
+                    // the epilogue operand goes into the oldest slots as soon as their last k-blocks have retired, while the
+                    // MMAs of the newest ones still run: wait for them as for the next k-blocks
+                    for (int t = 0; t < C::OPND_SLOTS; ++t) {
+                        mbar_wait(empty_bar(stage), phase ^ 1u);
+                        if (++stage == kStages) { stage = 0; phase ^= 1u; }
+                    }
+                    if (elect_one()) {
+                        mbar_arrive_expect_tx(opnd_bar, C::OPND * C::PIECE);
+                        if (EPI == EPI_DGELU_BWD_T) {
+                            const uint8_t* src = reinterpret_cast<const uint8_t*>(p.aux_in) + tn_tile * 2;
+#pragma unroll
+                            for (int k = 0; k < C::OPND; ++k) bulk_load(piece_addr(k), src + k * C::PIECE, C::PIECE, opnd_bar);
+                        } else {
+                            tma_prefetch_desc(&tmE);
+#pragma unroll
+                            for (int k = 0; k < C::OPND; ++k)
+                                tma_load_2d(piece_addr(k), &tmE, opnd_bar, tc.n_blk * BLOCK_N + 64 * k, tc.m_blk * BLOCK_M);
+                        }
+                    }
+                    __syncwarp();
+                }
+            }
         }
         return;
     }
@@ -357,28 +323,24 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
             sbias[i] = (mine && col < p.N) ? __ldg(p.bias + col) : 0.f;
         }
     }
-    constexpr int NH = BLOCK_N / 128;
     // K-major: advance 16 elements (32 B) inside the swizzle row; MN-major: 16 k-rows (2 KB)
     constexpr uint32_t a_kstep = A_MN ? WGMMA_K * 128 : WGMMA_K * 2;
     constexpr uint32_t b_kstep = B_MN ? WGMMA_K * 128 : WGMMA_K * 2;
-    float acc[NH][64];
+    // fragment (wgmma_m64n128k16 / wgmma_m64n256k16): acc[4 j + 2 i + c] = tile[64 wg + 16 (warp % 4) + lane / 4 + 8 i][8 j + 2 (lane % 4) + c]
+    float acc[BLOCK_N / 2];
     {
         int stage = 0, prev = 0;
         uint32_t phase = 0;
         for (int kb = tc.kb_begin; kb < tc.kb_end; ++kb) {
             mbar_wait(full_bar(stage), phase);
-            // this warpgroup's 64 rows of A: 64 K-major rows or one 64-wide MN-major atom = 8 KB further in both layouts;
-            // the second 128 columns of B likewise start 16 KB further
+            // this warpgroup's 64 rows of A: 64 K-major rows or one 64-wide MN-major atom = 8 KB further in both layouts
             const uint32_t a0 = a_tile(stage) + wg * 8192, b0 = b_tile(stage);
             wgmma_fence();
 #pragma unroll
-            for (int k = 0; k < BLOCK_K / WGMMA_K; ++k) {
-                const uint64_t ad = wgmma_desc_sw128(a0 + k * a_kstep, kAtomBytes, 1024);
-#pragma unroll
-                for (int h = 0; h < NH; ++h)
-                    wgmma_m64n128k16<A_MN ? 1 : 0, B_MN ? 1 : 0>(acc[h], ad, wgmma_desc_sw128(b0 + h * 16384 + k * b_kstep, kAtomBytes, 1024),
-                                                                 (kb > tc.kb_begin || k > 0) ? 1u : 0u);
-            }
+            for (int k = 0; k < BLOCK_K / WGMMA_K; ++k)
+                wgmma_tile<BLOCK_N, A_MN ? 1 : 0, B_MN ? 1 : 0>(acc, wgmma_desc_sw128(a0 + k * a_kstep, kAtomBytes, 1024),
+                                                              wgmma_desc_sw128(b0 + k * b_kstep, kAtomBytes, 1024),
+                                                              (kb > tc.kb_begin || k > 0) ? 1u : 0u);
             wgmma_commit();
             // the MMAs of the previous k-block have retired: its slot may be refilled
             wgmma_wait<1>();
@@ -388,112 +350,231 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
         }
         wgmma_wait<0>();
     }
-
-    // ---------------- epilogue ----------------
-    // Thread -> element map: epilogue warp ew owns rows 32 (ew % 4) .. + 31 and the column half ew / 4 of the tile, in 16-column
-    // chunks; in step j a thread holds one chunk of one row. By default lane l takes chunk l / RPI of row RPI j + l % RPI of the
-    // warp's 32, so that one warp access covers RPI whole half-rows (RPI x 256 contiguous bytes of a bf16 output instead of 32
-    // bytes of 32 rows), and the staging reads of a quarter-warp hit 8 distinct 4-bank groups (ACC_LD = 4 mod 32). EPI_DELTA keeps
-    // one row per lane and chunk j in step j: a thread then holds whole heads of its row.
-    // Operands read by the epilogue (residual / gelu') are requested before the accumulators are staged.
-    const int ew = warp - 4;
-    const int q = ew & 3, half = ew >> 2;
-    const int col0 = tc.n_blk * BLOCK_N + half * (BLOCK_N / 2);
-    constexpr int NCH = BLOCK_N / 2 / 16;
-    constexpr int RPI = 32 / NCH;
-    constexpr bool kRowPerLane = EPI == EPI_DELTA;
-    auto wrow_of = [&](int j) { return kRowPerLane ? lane : RPI * j + lane % RPI; };   // row within the warp's 32
-    auto chunk_of = [&](int j) { return kRowPerLane ? j : lane / RPI; };
-    // tile-native gelu'(u) (M, N multiples of 256; vbert_b200.h): 1 KB warp blocks per chunk, row r of the warp's 32 at + 32 r bytes
-    const long long gp_warp_off =
-        ((((static_cast<long long>(tc.m_blk >> 1) * n_blocks + tc.n_blk) * 2 + (tc.m_blk & 1)) * kEpiWarps + ew) * NCH) * 512;
-    auto gp_off = [&](int j) { return gp_warp_off + chunk_of(j) * 512 + wrow_of(j) * 16; };
-    constexpr bool kEx = !OUT_F32 && EPI != EPI_BIAS && !epi_is_gelu(EPI) && EPI != EPI_GELU_ONLY;
-    uint32_t ex[kEx ? NCH : 1][8];
-    if constexpr (kEx) {
-        constexpr bool kWantAdd = EPI == EPI_RESID || EPI == EPI_DROP_RESID || EPI == EPI_DELTA;   // EPI_DELTA: addend = O
-        const int row0 = tc.m_blk * BLOCK_M + q * 32 + wrow_of(0), c0 = col0 + chunk_of(0) * 16;   // step j: row0 + (row step) j
-        const bf16* exb = nullptr;
-        long long ex_step = 0;
-        if (kWantAdd || (epi_is_generic(EPI) && p.addend != nullptr)) {
-            exb = p.addend + static_cast<long long>(row0) * p.ld_add + c0;
-            ex_step = kRowPerLane ? 16 : RPI * p.ld_add;
-        } else if (EPI == EPI_DGELU_BWD || (epi_is_generic(EPI) && p.epilogue == VB_EPI_DGELU)) {
-            exb = p.aux_in + static_cast<long long>(row0) * p.ld_aux + c0;
-            ex_step = kRowPerLane ? 16 : RPI * p.ld_aux;
-        } else if (EPI == EPI_DGELU_BWD_T) {
-            exb = p.aux_in + gp_off(0);
-            ex_step = kRowPerLane ? 512 : RPI * 16;
-        }
-#pragma unroll
-        for (int j = 0; j < NCH; ++j)
-            if (exb != nullptr && tc.m_blk * BLOCK_M + q * 32 + wrow_of(j) < p.M && col0 + chunk_of(j) * 16 < p.N) ldg_v8(exb + j * ex_step, ex[j]);
-    }
-
-    // both warpgroups' MMAs have retired (and with them every read of the ring): stage the accumulators over the ring
+    // both warpgroups' MMAs have retired (and with them every read of the ring): the ring may be overwritten
     named_bar_sync(1, kEpiWarps * 32);
-    float* sacc = reinterpret_cast<float*>(smem);
-    {
-        const int r0 = wg * 64 + ((warp & 3) << 4) + (lane >> 2);
+
+    if constexpr (OUT_F32) {
+        // ---------------- fp32 epilogue: split-K red.add or a deterministic slab store ----------------
+        // The tile goes through shared memory so that a thread owns 16-column pieces of one row: lane l of epilogue warp ew
+        // takes chunk l / RPI of row RPI k + l % RPI of rows 32 (ew % 4) .. + 31, column half ew / 4, so that one warp access
+        // covers whole half-rows.
+        float* sacc = reinterpret_cast<float*>(smem);
+        {
+            const int r0 = wg * 64 + ((warp & 3) << 4) + (lane >> 2);
 #pragma unroll
-        for (int h = 0; h < NH; ++h)
-#pragma unroll
-            for (int j = 0; j < 16; ++j)
+            for (int j = 0; j < BLOCK_N / 8; ++j)
 #pragma unroll
                 for (int i = 0; i < 2; ++i)
-                    *reinterpret_cast<float2*>(sacc + (r0 + 8 * i) * C::ACC_LD + h * 128 + j * 8 + 2 * (lane & 3)) =
-                        make_float2(acc[h][4 * j + 2 * i], acc[h][4 * j + 2 * i + 1]);
-    }
-    named_bar_sync(1, kEpiWarps * 32);
-
-    [[maybe_unused]] float hsum = 0.f;
+                    *reinterpret_cast<float2*>(sacc + (r0 + 8 * i) * C::ACC_LD + j * 8 + 2 * (lane & 3)) =
+                        make_float2(acc[4 * j + 2 * i], acc[4 * j + 2 * i + 1]);
+        }
+        named_bar_sync(1, kEpiWarps * 32);
+        const int ew = warp - 4;
+        const int q = ew & 3, half = ew >> 2;
+        constexpr int NCH = BLOCK_N / 2 / 16;
+        constexpr int RPI = 32 / NCH;
 #pragma unroll
-    for (int k = 0; k < NCH; ++k) {
-        const int lrow = q * 32 + wrow_of(k), cc = half * (BLOCK_N / 2) + chunk_of(k) * 16;   // in the tile
-        const int row = tc.m_blk * BLOCK_M + lrow;
-        const int col = tc.n_blk * BLOCK_N + cc;
-        if (row < p.M && col < p.N) {
-            float x[16];
+        for (int k = 0; k < NCH; ++k) {
+            const int lrow = q * 32 + RPI * k + lane % RPI, cc = half * (BLOCK_N / 2) + (lane / RPI) * 16;   // in the tile
+            const int row = tc.m_blk * BLOCK_M + lrow;
+            const int col = tc.n_blk * BLOCK_N + cc;
+            if (row < p.M && col < p.N) {
+                float x[16];
 #pragma unroll
-            for (int i = 0; i < 4; ++i) {
-                const float4 v = *reinterpret_cast<const float4*>(sacc + lrow * C::ACC_LD + cc + 4 * i);
-                x[4 * i] = v.x; x[4 * i + 1] = v.y; x[4 * i + 2] = v.z; x[4 * i + 3] = v.w;
-            }
-            const float* sb = has_bias ? sbias + cc : nullptr;
-            const uint32_t (&e)[8] = ex[kEx ? k : 0];
-            if constexpr (EPI == EPI_GELU_FWD_T) {
-                // gelu'(u) into the tile-native buffer, gelu(u) row-major
-                uint32_t o0[8], o1[8];
-                epilogue16<OUT_F32, EPI, true>(p, row, col, sb, e, x, o0, o1);
-                stg_v8(reinterpret_cast<bf16*>(p.D) + gp_off(k), o0);
-                stg_v8(p.aux_out + static_cast<long long>(row) * p.ld_aux + col, o1);
-            } else if constexpr (EPI == EPI_SLAB) {
-                float* d = reinterpret_cast<float*>(p.D) + (static_cast<long long>(blockIdx.x / (m_blocks * n_blocks)) * p.M + row) * p.ldd + col;
-#pragma unroll
-                for (int i = 0; i < 4; ++i) *reinterpret_cast<float4*>(d + 4 * i) = make_float4(x[4 * i], x[4 * i + 1], x[4 * i + 2], x[4 * i + 3]);
-            } else if constexpr (EPI == EPI_DELTA) {
-                uint32_t o0[8];
-                epilogue16<OUT_F32, EPI, true>(p, row, col, sb, e, x, o0);
-                stg_v8(reinterpret_cast<bf16*>(p.D) + static_cast<long long>(row) * p.ldd + col, o0);
-#pragma unroll
-                for (int i = 0; i < 8; ++i) {   // dot product of the ROUNDED dO (what the attention kernel will read) with O
-                    const float2 a = unpack_bf16x2(o0[i]), b = unpack_bf16x2(e[i]);
-                    hsum = fmaf(a.x, b.x, fmaf(a.y, b.y, hsum));
+                for (int i = 0; i < 4; ++i) {
+                    const float4 v = *reinterpret_cast<const float4*>(sacc + lrow * C::ACC_LD + cc + 4 * i);
+                    x[4 * i] = v.x; x[4 * i + 1] = v.y; x[4 * i + 2] = v.z; x[4 * i + 3] = v.w;
                 }
+                if constexpr (EPI == EPI_SLAB) {
+                    float* d = reinterpret_cast<float*>(p.D) + (static_cast<long long>(blockIdx.x / (m_blocks * n_blocks)) * p.M + row) * p.ldd + col;
+#pragma unroll
+                    for (int i = 0; i < 4; ++i) *reinterpret_cast<float4*>(d + 4 * i) = make_float4(x[4 * i], x[4 * i + 1], x[4 * i + 2], x[4 * i + 3]);
+                } else {
+                    if (has_bias) {
+#pragma unroll
+                        for (int i = 0; i < 4; ++i) {
+                            const float4 b = *reinterpret_cast<const float4*>(sbias + cc + 4 * i);
+                            x[4 * i] += b.x; x[4 * i + 1] += b.y; x[4 * i + 2] += b.z; x[4 * i + 3] += b.w;
+                        }
+                    }
+                    float* d = reinterpret_cast<float*>(p.D) + static_cast<long long>(row) * p.ldd + col;
+#pragma unroll
+                    for (int i = 0; i < 4; ++i) red_add_v4_f32(d + 4 * i, x[4 * i], x[4 * i + 1], x[4 * i + 2], x[4 * i + 3]);
+                }
+            }
+        }
+    } else {
+        // ---------------- bf16 epilogue in the accumulator fragment ----------------
+        // Per element, in this order: + bias, dropout, + residual, then GELU (two outputs) / x gelu'(u) / gelu only. The operand
+        // comes from shared memory (loaded by the producer warp) and the results are staged there, both with ldmatrix /
+        // stmatrix on 8 x 8 blocks; each warpgroup then stores its 64 rows with TMA (out-of-bounds rows and columns clipped).
+        constexpr bool kGeneric = epi_is_generic(EPI);
+        constexpr bool kTwoOut = epi_is_gelu(EPI) || kGeneric;    // generic: GELU at run time
+        const bool two_out = epi_is_gelu(EPI) || (kGeneric && p.epilogue == VB_EPI_GELU);
+        const bool reads = epi_may_read(EPI) && epi_reads(EPI, p);
+        const bool is_dgelu = epi_is_dgelu(EPI) || (kGeneric && p.epilogue == VB_EPI_DGELU);
+        const bool add = EPI == EPI_RESID || EPI == EPI_DROP_RESID || (kGeneric && p.addend != nullptr);
+        const bool drop = EPI == EPI_DROP_RESID || (kGeneric && p.drop_scale != 0.0f);
+        const int w4 = warp & 3, qd = lane & 3;
+        const int frow0 = 64 * wg + 16 * w4 + (lane >> 2);            // tile row of acc[.. + 0], +8 for acc[.. + 2]
+        const int mrow = 64 * wg + 16 * w4 + ((lane >> 3) & 1) * 8 + (lane & 7);   // row this lane addresses in ldmatrix / stmatrix
+        const int mj = lane >> 4;                                      // ... and its 8-column block within a pair
+        // row-major tiles: 64-column pieces, row r at + 128 r, its 16-byte blocks permuted by r % 8 (the TMA 128B swizzle);
+        // piece p0 + col / 64 holds the columns of `col`
+        auto rm_addr = [&](int p0, int col) {
+            return piece_addr(p0 + (col >> 6)) + mrow * 128 + ((((col & 63) >> 3) ^ (mrow & 7)) << 4);
+        };
+        auto tn_addr = [&](int pbase, int col) {   // tile-native staging / operand
+            const uint32_t o = tn_byte(mrow, col);
+            return piece_addr(pbase + (o >> 14)) + (o & (C::PIECE - 1));
+        };
+
+        // dropout keep words: lane qd draws the word of 8-column group 4 t + qd of its two rows; the quad exchanges them below
+        constexpr int KW = BLOCK_N / 128;   // words per row: 4 groups (one byte each) of the lane's BLOCK_N / 32
+        uint32_t kw[2][KW];
+        if (drop) {
+            const uint32_t key0 = dropout_key(EPI == EPI_GENERIC_OFF ? p.drop_seed + *p.drop_offset : p.drop_seed, p.drop_stream);
+#pragma unroll
+            for (int i = 0; i < 2; ++i) {
+                const unsigned long long e0 =
+                    (static_cast<unsigned long long>(tc.m_blk * BLOCK_M + frow0 + 8 * i) * static_cast<unsigned>(p.N) + tc.n_blk * BLOCK_N) >> 3;
+#pragma unroll
+                for (int s = 0; s < KW; ++s) {
+                    uint32_t w = 0;
+#pragma unroll
+                    for (int b = 0; b < 4; ++b) w |= dropout_keep8_key(key0, e0 + 4 * (4 * s + b) + qd, p.drop_thresh16) << (8 * b);
+                    kw[i][s] = w;
+                }
+            }
+        }
+        // the words of the quad's four lanes: kq[i][s][q] = kw[i][s] of lane q
+        uint32_t kq[2][KW][4];
+        if (drop) {
+#pragma unroll
+            for (int i = 0; i < 2; ++i)
+#pragma unroll
+                for (int s = 0; s < KW; ++s)
+#pragma unroll
+                    for (int q = 0; q < 4; ++q) kq[i][s][q] = __shfl_sync(0xffffffffu, kw[i][s], (lane & ~3) | q);
+        }
+        if (reads) mbar_wait(opnd_bar, 0);
+
+#pragma unroll
+        for (int jp = 0; jp < BLOCK_N / 16; ++jp) {
+            // registers k = 0..3 of this pair: 8-column block j = 2 jp + k / 2, row frow0 + 8 (k % 2) = acc[8 jp + 2 k], +1
+            float* x = acc + 8 * jp;
+            const int mcol = 16 * jp + 8 * mj;   // the column block this lane addresses
+            if (has_bias) {
+#pragma unroll
+                for (int k = 0; k < 4; ++k) {
+                    const float2 b = *reinterpret_cast<const float2*>(sbias + 8 * (2 * jp + k / 2) + 2 * qd);
+                    x[2 * k] += b.x; x[2 * k + 1] += b.y;
+                }
+            }
+            if (drop) {
+#pragma unroll
+                for (int k = 0; k < 4; ++k) {
+                    const int j = 2 * jp + k / 2;   // group j was drawn by lane j % 4 of the quad: byte (j / 4) % 4 of its word j / 16
+                    const uint32_t keep = kq[k % 2][j / 16][j & 3] >> (8 * ((j >> 2) & 3) + 2 * qd);
+                    x[2 * k] = (keep & 1u) ? x[2 * k] * p.drop_scale : 0.0f;
+                    x[2 * k + 1] = (keep & 2u) ? x[2 * k + 1] * p.drop_scale : 0.0f;
+                }
+            }
+            uint32_t e[4] = {0u, 0u, 0u, 0u};
+            if (reads) {
+                if (EPI == EPI_DGELU_BWD_T) ldmatrix_x4(tn_addr(0, mcol), e);
+                else ldmatrix_x4(rm_addr(0, mcol), e);
+            }
+            if (add) {
+#pragma unroll
+                for (int k = 0; k < 4; ++k) {
+                    const float2 t = unpack_bf16x2(e[k]);
+                    x[2 * k] += t.x;
+                    x[2 * k + 1] += t.y;
+                }
+            }
+            uint32_t o0[4], o1[4];
+            if (EPI == EPI_GELU_ONLY) {
+                // D <- gelu(u): the value the GELU epilogue below sends to aux_out, from the same function; its derivative is dropped
+#pragma unroll
+                for (int k = 0; k < 8; ++k) {
+                    float gp;
+                    gelu_fwd_bwd(x[k], x[k], gp);
+                }
+            } else if (kTwoOut && two_out) {
+                // aux_out <- gelu(u) (operand of the next GEMM), D <- gelu'(u) (all the backward needs of u)
+                float gp[8];
+#pragma unroll
+                for (int k = 0; k < 8; ++k) gelu_fwd_bwd(x[k], x[k], gp[k]);
+#pragma unroll
+                for (int k = 0; k < 4; ++k) o1[k] = pack_bf16x2(gp[2 * k], gp[2 * k + 1]);
+            } else if (is_dgelu) {
+#pragma unroll
+                for (int k = 0; k < 4; ++k) {
+                    const float2 t = unpack_bf16x2(e[k]);
+                    x[2 * k] *= t.x;
+                    x[2 * k + 1] *= t.y;
+                }
+            }
+#pragma unroll
+            for (int k = 0; k < 4; ++k) o0[k] = pack_bf16x2(x[2 * k], x[2 * k + 1]);
+            if (kTwoOut && two_out) {
+                // gelu'(u) -> D (tile-native or row-major), gelu(u) -> aux_out (row-major)
+                stmatrix_x4(EPI == EPI_GELU_FWD_T ? tn_addr(C::OPND, mcol) : rm_addr(C::OPND, mcol), o1);
+                stmatrix_x4(rm_addr(2 * C::OPND, mcol), o0);
             } else {
-                epilogue16<OUT_F32, EPI>(p, row, col, sb, e, x);
+                stmatrix_x4(rm_addr(C::OPND, mcol), o0);
+            }
+            if ((jp & 3) == 3) {
+                // 64 columns of this warpgroup's 64 rows are staged: one thread stores them while the others go on (the
+                // generic proxy's writes made visible to TMA first)
+                fence_proxy_async_smem();
+                named_bar_sync(2 + wg, 128);
+                if ((threadIdx.x & 127) == 0) {
+                    const int b = jp >> 2, gcol = tc.n_blk * BLOCK_N + 64 * b, grow = tc.m_blk * BLOCK_M + 64 * wg;
+                    if (EPI == EPI_GELU_FWD_T) {
+                        // column half h of rows 64 wg .. + 63 is the 16 KB piece 2 h + wg of the tile's 64 KB
+                        if ((jp & 7) == 7) {
+                            const int pc = 2 * (jp >> 3) + wg;
+                            bulk_store(reinterpret_cast<uint8_t*>(p.D) + tn_tile * 2 + pc * C::PIECE, piece_addr(C::OPND + pc), C::PIECE);
+                        }
+                        tma_store_2d(&tmX, piece_addr(2 * C::OPND + b) + wg * 8192, gcol, grow);
+                    } else {
+                        tma_store_2d(&tmD, piece_addr(C::OPND + b) + wg * 8192, gcol, grow);
+                        if (kTwoOut && two_out) tma_store_2d(&tmX, piece_addr(2 * C::OPND + b) + wg * 8192, gcol, grow);
+                    }
+                    bulk_commit();
+                }
             }
         }
         if constexpr (EPI == EPI_DELTA) {
-            if ((k & 3) == 3) {   // four chunks are exactly one head (col0 is a multiple of 64)
-                const int c4 = col - 48;
+            // D = rowsum(dO * O) per head from the staged, ROUNDED dO (what the attention kernel will read) and O, both in
+            // shared memory: thread t of the warpgroup sums heads 2 (t / 64), +1 of row t % 64, each in column order
+            const int t = threadIdx.x & 127, r = 64 * wg + (t & 63), row = tc.m_blk * BLOCK_M + r;
+#pragma unroll
+            for (int hh = 0; hh < 2; ++hh) {
+                const int h = 2 * (t >> 6) + hh;   // head h of the tile = 64-column piece h
+                float sum = 0.f;
+#pragma unroll
+                for (int c = 0; c < 8; ++c) {
+                    const uint32_t off = r * 128 + ((c ^ (r & 7)) << 4);
+                    const uint4 dv = *reinterpret_cast<const uint4*>(smem + (piece_addr(C::OPND + h) - base) + off);
+                    const uint4 ov = *reinterpret_cast<const uint4*>(smem + (piece_addr(h) - base) + off);
+                    const uint32_t du[4] = {dv.x, dv.y, dv.z, dv.w}, ou[4] = {ov.x, ov.y, ov.z, ov.w};
+#pragma unroll
+                    for (int i = 0; i < 4; ++i) {
+                        const float2 x = unpack_bf16x2(du[i]), y = unpack_bf16x2(ou[i]);
+                        sum = fmaf(x.x, y.x, fmaf(x.y, y.y, sum));
+                    }
+                }
+                const int c4 = tc.n_blk * BLOCK_N + 64 * h;
                 if (row < p.M && c4 < p.N) {
                     const int bi = row / p.delta_seq, si = row - bi * p.delta_seq;
-                    p.delta_out[(static_cast<long long>(bi) * (p.N >> 6) + (c4 >> 6)) * p.delta_seq + si] = hsum;
+                    p.delta_out[(static_cast<long long>(bi) * (p.N >> 6) + (c4 >> 6)) * p.delta_seq + si] = sum;
                 }
-                hsum = 0.f;
             }
         }
+        if ((threadIdx.x & 127) == 0) bulk_wait_read0();   // the shared memory stays valid until TMA has read it; the global writes drain after exit
     }
 }
 
@@ -588,8 +669,12 @@ int num_sms() {
     return n[dev];
 }
 
+// the tensor maps of one call: A and B (k-slab loads), and for bf16 outputs D and aux_out (64 x 64 stores of a warpgroup's rows)
+// and the epilogue operand (64-column x 128-row loads); maps a call does not use stay zero
+struct GemmMaps { CUtensorMap a, b, d, x, e; };
+
 template <bool A_MN, bool B_MN, int BLOCK_N, bool OUT_F32, int EPI = EPI_GENERIC>
-static int launch(const CUtensorMap& ta, const CUtensorMap& tb, const GemmParams& p, cudaStream_t st) {
+static int launch(const GemmMaps& m, const GemmParams& p, cudaStream_t st) {
     using C = Cfg<BLOCK_N>;
     auto kern = gemm_wgmma_kernel<A_MN, B_MN, BLOCK_N, OUT_F32, EPI>;
     static int configured[kMaxDevices] = {0};
@@ -598,7 +683,7 @@ static int launch(const CUtensorMap& ta, const CUtensorMap& tb, const GemmParams
     VB_REQUIRE(tiles < (1LL << 31), "vb_gemm: too many tiles");
     {
         ProfScope ps(st, OUT_F32 ? PROF_GEMM_WGRAD : (B_MN ? PROF_GEMM_DGRAD : PROF_GEMM_FWD), 2.0 * p.M * p.N * p.K, 1);
-        VB_CHECK_CUDA(launch_pdl(kern, dim3(static_cast<unsigned>(tiles)), dim3(kThreads), C::SMEM_BYTES, st, ta, tb, p));
+        VB_CHECK_CUDA(launch_pdl(kern, dim3(static_cast<unsigned>(tiles)), dim3(kThreads), C::SMEM_BYTES, st, m.a, m.b, p, m.d, m.x, m.e));
     }
     VB_CHECK_CUDA(cudaGetLastError());
     return 0;
@@ -678,9 +763,10 @@ int gemm(const vb_gemm_args& a, cudaStream_t st) {
                "vb_gemm: fp32-accumulate output supports bias only");
     VB_REQUIRE(a.dropout_p >= 0.0f && a.dropout_p < 1.0f, "vb_gemm: dropout_p out of range");
     VB_REQUIRE(!a.delta_out || (gemm_delta_ok(a.M, a.N) && a.delta_ctx && a.delta_seq > 0 && a.M % a.delta_seq == 0 && !a.d_fp32 &&
-                                !a.a_mn_major && a.b_mn_major && !a.bias && !a.addend && a.dropout_p == 0.0f && a.epilogue == VB_EPI_NONE &&
-                                (reinterpret_cast<uintptr_t>(a.delta_ctx) & 31) == 0),
+                                !a.a_mn_major && a.b_mn_major && !a.bias && !a.addend && a.dropout_p == 0.0f && a.epilogue == VB_EPI_NONE),
                "vb_gemm: delta_out needs a plain bf16 input-gradient GEMM (b_mn_major, no bias / addend / dropout) and vb_gemm_delta_ok(M, N)");
+    // delta_ctx is read like an addend of row stride N (vb_gemm_delta_ok: N % 64 == 0), through a TMA tensor map
+    VB_REQUIRE(!a.delta_out || (reinterpret_cast<uintptr_t>(a.delta_ctx) & 31) == 0, "vb_gemm: delta_ctx must be 32-byte aligned");
     VB_REQUIRE(!a.gp_tiled || (gemm_gp_tiled_ok(a.M, a.N) && !a.d_fp32 && !a.a_mn_major && (a.epilogue == VB_EPI_GELU || a.epilogue == VB_EPI_DGELU)),
                "vb_gemm: gp_tiled needs a GELU / DGELU epilogue and vb_gemm_gp_tiled_ok(M, N)");
     VB_REQUIRE(!a.gp_tiled || a.epilogue != VB_EPI_DGELU || a.b_mn_major,
@@ -727,19 +813,25 @@ int gemm(const vb_gemm_args& a, cudaStream_t st) {
     }
     const bool slab = a.d_fp32 && p.splits > 1 && det.ptr != nullptr;
 
-    CUtensorMap ta, tb;
-    int rc;
-    if (!a.a_mn_major) rc = make_tmap_bf16(&ta, a.A, a.K, a.M, a.lda, BLOCK_M);
-    else               rc = make_tmap_bf16(&ta, a.A, a.M, a.K, a.lda, BLOCK_K);
-    if (rc) return rc;
-    if (!a.b_mn_major) rc = make_tmap_bf16(&tb, a.B, a.K, a.N, a.ldb, bn256 ? 256 : 128);
-    else               rc = make_tmap_bf16(&tb, a.B, a.N, a.K, a.ldb, BLOCK_K);
-    if (rc) return rc;
+    GemmMaps mp;
+    memset(&mp, 0, sizeof(mp));
+    if (!a.a_mn_major) VB_TRY_RC(make_tmap_bf16(&mp.a, a.A, a.K, a.M, a.lda, BLOCK_M));
+    else               VB_TRY_RC(make_tmap_bf16(&mp.a, a.A, a.M, a.K, a.lda, BLOCK_K));
+    if (!a.b_mn_major) VB_TRY_RC(make_tmap_bf16(&mp.b, a.B, a.K, a.N, a.ldb, bn256 ? 256 : 128));
+    else               VB_TRY_RC(make_tmap_bf16(&mp.b, a.B, a.N, a.K, a.ldb, BLOCK_K));
+    if (!a.d_fp32) {
+        // bf16 outputs leave through TMA and the epilogue operand arrives through it: the argument checks above guarantee the
+        // 16-byte alignment of every base and row stride that TMA needs (the tile-native gelu'(u) moves as contiguous bulk copies)
+        if (!a.gp_tiled || a.epilogue != VB_EPI_GELU) VB_TRY_RC(make_tmap_bf16(&mp.d, a.D, a.N, a.M, a.ldd, 64));
+        if (a.aux_out) VB_TRY_RC(make_tmap_bf16(&mp.x, a.aux_out, a.N, a.M, a.ld_aux, 64));
+        if (p.addend) VB_TRY_RC(make_tmap_bf16(&mp.e, p.addend, a.N, a.M, p.ld_add, BLOCK_M));
+        else if (a.aux_in && !a.gp_tiled) VB_TRY_RC(make_tmap_bf16(&mp.e, a.aux_in, a.N, a.M, a.ld_aux, BLOCK_M));
+    }
 
     if (slab) {
         GemmParams q = p;
         q.D = det.ptr; q.ldd = a.N; q.bias = nullptr;
-        const int rc2 = bn256 ? launch<true, true, 256, true, EPI_SLAB>(ta, tb, q, st) : launch<true, true, 128, true, EPI_SLAB>(ta, tb, q, st);
+        const int rc2 = bn256 ? launch<true, true, 256, true, EPI_SLAB>(mp, q, st) : launch<true, true, 128, true, EPI_SLAB>(mp, q, st);
         if (rc2) return rc2;
         const long long n4 = static_cast<long long>(a.M) * a.N / 4;
         long long blocks = (n4 + 255) / 256;
@@ -756,7 +848,7 @@ int gemm(const vb_gemm_args& a, cudaStream_t st) {
         // dropout with the seed offset in device memory: the generic epilogue (it applies bias, dropout and addend in the order of
         // the specialised ones, so the bits equal a call with seed + *offset by value)
 #define VB_DISPATCH_OFF(AM, BM) \
-    (bn256 ? launch<AM, BM, 256, false, EPI_GENERIC_OFF>(ta, tb, p, st) : launch<AM, BM, 128, false, EPI_GENERIC_OFF>(ta, tb, p, st))
+    (bn256 ? launch<AM, BM, 256, false, EPI_GENERIC_OFF>(mp, p, st) : launch<AM, BM, 128, false, EPI_GENERIC_OFF>(mp, p, st))
         if (!a.a_mn_major && !a.b_mn_major) return VB_DISPATCH_OFF(false, false);
         if (!a.a_mn_major && a.b_mn_major) return VB_DISPATCH_OFF(false, true);
         if (a.a_mn_major && a.b_mn_major) return VB_DISPATCH_OFF(true, true);
@@ -764,7 +856,7 @@ int gemm(const vb_gemm_args& a, cudaStream_t st) {
 #undef VB_DISPATCH_OFF
     }
     if (a.epilogue == VB_EPI_GELU_FWD)
-        return bn256 ? launch<false, false, 256, false, EPI_GELU_ONLY>(ta, tb, p, st) : launch<false, false, 128, false, EPI_GELU_ONLY>(ta, tb, p, st);
+        return bn256 ? launch<false, false, 256, false, EPI_GELU_ONLY>(mp, p, st) : launch<false, false, 128, false, EPI_GELU_ONLY>(mp, p, st);
     if (bn256 && !a.d_fp32) {
         // specialised epilogues for the shapes of the layer (forward and input-gradient GEMMs); anything else: generic
         const bool drop = a.dropout_p > 0.0f, add = a.addend != nullptr;
@@ -775,28 +867,28 @@ int gemm(const vb_gemm_args& a, cudaStream_t st) {
         if (a.delta_out) epi = EPI_DELTA;
         if (!a.a_mn_major && !a.b_mn_major) {
             switch (epi) {
-                case EPI_BIAS: return launch<false, false, 256, false, EPI_BIAS>(ta, tb, p, st);
-                case EPI_RESID: return launch<false, false, 256, false, EPI_RESID>(ta, tb, p, st);
-                case EPI_DROP_RESID: return launch<false, false, 256, false, EPI_DROP_RESID>(ta, tb, p, st);
-                case EPI_GELU_FWD: return launch<false, false, 256, false, EPI_GELU_FWD>(ta, tb, p, st);
-                case EPI_GELU_FWD_T: return launch<false, false, 256, false, EPI_GELU_FWD_T>(ta, tb, p, st);
-                default: return launch<false, false, 256, false>(ta, tb, p, st);
+                case EPI_BIAS: return launch<false, false, 256, false, EPI_BIAS>(mp, p, st);
+                case EPI_RESID: return launch<false, false, 256, false, EPI_RESID>(mp, p, st);
+                case EPI_DROP_RESID: return launch<false, false, 256, false, EPI_DROP_RESID>(mp, p, st);
+                case EPI_GELU_FWD: return launch<false, false, 256, false, EPI_GELU_FWD>(mp, p, st);
+                case EPI_GELU_FWD_T: return launch<false, false, 256, false, EPI_GELU_FWD_T>(mp, p, st);
+                default: return launch<false, false, 256, false>(mp, p, st);
             }
         }
         if (!a.a_mn_major && a.b_mn_major) {
             switch (epi) {
-                case EPI_BIAS: return launch<false, true, 256, false, EPI_BIAS>(ta, tb, p, st);
-                case EPI_RESID: return launch<false, true, 256, false, EPI_RESID>(ta, tb, p, st);
-                case EPI_DGELU_BWD: return launch<false, true, 256, false, EPI_DGELU_BWD>(ta, tb, p, st);
-                case EPI_DELTA: return launch<false, true, 256, false, EPI_DELTA>(ta, tb, p, st);
-                case EPI_DGELU_BWD_T: return launch<false, true, 256, false, EPI_DGELU_BWD_T>(ta, tb, p, st);
-                default: return launch<false, true, 256, false>(ta, tb, p, st);
+                case EPI_BIAS: return launch<false, true, 256, false, EPI_BIAS>(mp, p, st);
+                case EPI_RESID: return launch<false, true, 256, false, EPI_RESID>(mp, p, st);
+                case EPI_DGELU_BWD: return launch<false, true, 256, false, EPI_DGELU_BWD>(mp, p, st);
+                case EPI_DELTA: return launch<false, true, 256, false, EPI_DELTA>(mp, p, st);
+                case EPI_DGELU_BWD_T: return launch<false, true, 256, false, EPI_DGELU_BWD_T>(mp, p, st);
+                default: return launch<false, true, 256, false>(mp, p, st);
             }
         }
     }
 
 #define VB_DISPATCH(AM, BM, F32)                                         \
-    (bn256 ? launch<AM, BM, 256, F32>(ta, tb, p, st) : launch<AM, BM, 128, F32>(ta, tb, p, st))
+    (bn256 ? launch<AM, BM, 256, F32>(mp, p, st) : launch<AM, BM, 128, F32>(mp, p, st))
     if (!a.d_fp32) {
         if (!a.a_mn_major && !a.b_mn_major) return VB_DISPATCH(false, false, false);
         if (!a.a_mn_major && a.b_mn_major) return VB_DISPATCH(false, true, false);
