@@ -243,7 +243,12 @@ typedef struct {
     void* keep_mask; /* vb_attention_keep_bytes(batch, seq, heads) bytes; only touched when attn_dropout > 0 */
 } vb_layer_acts;
 
-/* fp32 parameter-gradient accumulators (+=), nn.Linear layout */
+/* fp32 parameter-gradient accumulators (+=), nn.Linear layout. A NULL field is not computed (a frozen parameter): a NULL dw_*
+ * skips that weight-gradient GEMM, a NULL db_qkv / db_inter that column sum. A LayerNorm backward forms dgamma, dbeta and the
+ * bias gradient of the Linear in front of it in one pass, so (dln1_gamma, dln1_beta, db_attn_out) and (dln2_gamma, dln2_beta,
+ * db_out) are each all set or all NULL; all NULL runs that LayerNorm backward without column reductions (and without its
+ * deterministic-mode partials), a partly NULL group is refused. Holds for vb_layer_bwd, vb_encoder_bwd and
+ * vb_encoder_bwd_varlen in every mode. */
 typedef struct {
     float* dw_qkv; float* db_qkv; float* dw_attn_out; float* db_attn_out; float* dln1_gamma; float* dln1_beta;
     float* dw_inter; float* db_inter; float* dw_out; float* db_out; float* dln2_gamma; float* dln2_beta;
@@ -261,7 +266,8 @@ typedef struct {
 
 /* x_in, x_out: bf16 [M, H]. x_out = BertLayer(x_in). */
 int vb_layer_fwd(const vb_layer_desc* d, const void* x_in, void* x_out, const vb_layer_acts* acts, void* stream);
-/* dy: gradient w.r.t. x_out; dx: gradient w.r.t. x_in (may alias dy). */
+/* dy: gradient w.r.t. x_out; dx: gradient w.r.t. x_in (may alias dy). dx may be NULL: the input gradient is not needed, and the
+ * input-gradient GEMM of the QKV projection (with its residual addend) is not launched. */
 int vb_layer_bwd(const vb_layer_desc* d, const void* x_in, const vb_layer_acts* acts, const void* dy, void* dx,
                  const vb_layer_grads* grads, const vb_layer_scratch* scratch, void* stream);
 
@@ -279,7 +285,9 @@ int64_t vb_encoder_arena_layout(int32_t batch, int32_t seq, int32_t hidden, int3
                                 int64_t* offsets /* [VB_ENCODER_ARENA_BUFFERS] */);
 /* x_in bf16 [M, H]; the output of layer l is arena buffer 13 (y) of slot l. */
 int vb_encoder_fwd(const vb_layer_desc* descs, int32_t n_layers, const void* x_in, void* arena, void* stream);
-/* dy: gradient w.r.t. the LAST layer's output; dx: gradient w.r.t. x_in; grads: HOST array [n_layers]. */
+/* dy: gradient w.r.t. the LAST layer's output; dx: gradient w.r.t. x_in; grads: HOST array [n_layers] (NULL fields: see
+ * vb_layer_grads; every entry is checked before the first launch). dx may be NULL (also in vb_encoder_bwd_varlen): the lowest
+ * layer's input-gradient GEMM is not launched, and the gradient between layers travels in scratch->d_x1 instead of dx. */
 int vb_encoder_bwd(const vb_layer_desc* descs, int32_t n_layers, const void* x_in, void* arena, const void* dy, void* dx,
                    const vb_layer_grads* grads, const vb_layer_scratch* scratch, void* stream);
 /* The attention maps of every layer of a dense vb_encoder_fwd call (analysis mode, M.py:1316-1324, 1430-1444): probs fp32
@@ -344,6 +352,10 @@ typedef struct {
     float* mean; float* rstd; /* [M] */
 } vb_embed_acts;
 
+/* A NULL table (dword, dpos, dtype, dpos_vis, dtype_vis) receives no scatter: a frozen table. In deterministic mode its rows
+ * still take part in the key sort, so the sum order of every other table is that of the call with every table given, bit for
+ * bit. A NULL dw_proj / db_proj skips the projection's weight-gradient GEMM / column sum; dgamma and dbeta both NULL run the
+ * embedding LayerNorm backward without column reductions (one of them NULL: that one is not written). */
 typedef struct {
     float* dword; float* dpos; float* dtype; float* dpos_vis; float* dtype_vis; /* fp32 tables, += */
     float* dw_proj; float* db_proj; float* dgamma; float* dbeta;

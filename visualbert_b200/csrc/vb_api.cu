@@ -117,10 +117,23 @@ static long long layer_bwd_det_bytes(int M, int H, int I) {
     return ln_bwd_det_bytes(M, H) > c ? ln_bwd_det_bytes(M, H) : c;
 }
 
+// A NULL gradient field is not computed (frozen parameters): its weight-gradient GEMM or column sum is not launched. A LayerNorm
+// backward forms dgamma, dbeta and the bias gradient of the Linear in front of it in one pass, so those three are all given or
+// all NULL (the pass then runs without column reductions).
+static int check_grads(const vb_layer_grads* g) {
+    VB_REQUIRE(g != nullptr, "layer_bwd: null grads");
+    const int ln1 = !!g->dln1_gamma + !!g->dln1_beta + !!g->db_attn_out, ln2 = !!g->dln2_gamma + !!g->dln2_beta + !!g->db_out;
+    VB_REQUIRE(ln1 == 0 || ln1 == 3, "layer_bwd: dln1_gamma, dln1_beta and db_attn_out are computed together: give all three or none");
+    VB_REQUIRE(ln2 == 0 || ln2 == 3, "layer_bwd: dln2_gamma, dln2_beta and db_out are computed together: give all three or none");
+    return 0;
+}
+
+// dx NULL: the input gradient is not needed, and the input-gradient GEMM of the QKV projection is not launched
 int layer_bwd(const vb_layer_desc* d, const void* x_in, const vb_layer_acts* s, const void* dy, void* dx,
               const vb_layer_grads* g, const vb_layer_scratch* w, cudaStream_t st, const LayerRows& rows = kDenseRows) {
     VB_TRY(check_layer(d, rows));
-    VB_REQUIRE(x_in && s && dy && dx && g && w, "layer_bwd: null pointer");
+    VB_REQUIRE(x_in && s && dy && g && w, "layer_bwd: null pointer");
+    VB_TRY(check_grads(g));
     const bool vl = rows.cu_seqlens != nullptr;
     const int M = vl ? rows.total : d->batch * d->seq, H = d->hidden, I = d->inter;
     VB_TRY(det_require(layer_bwd_det_bytes(M, H, I), "layer backward"));
@@ -131,23 +144,23 @@ int layer_bwd(const vb_layer_desc* d, const void* x_in, const vb_layer_acts* s, 
     // ---- BertOutput: LN2, output.dense ----
     VB_TRY(ln_bwd(dy, s->pre2, s->mean2, s->rstd2, d->ln2_gamma, w->d_pre, hd ? w->d_pre_drop : nullptr, g->dln2_gamma,
                   g->dln2_beta, g->db_out, M, H, d->hidden_dropout, d->seed, drop_stream(d->layer_index, kSiteFfnOut),
-                  0.f, 0, st));
-    VB_TRY(gemm(wgrad_args(dpm, s->g, g->dw_out, M, H, I), st));
+                  0.f, 0, st, g->db_out == nullptr));
+    if (g->dw_out) VB_TRY(gemm(wgrad_args(dpm, s->g, g->dw_out, M, H, I), st));
     vb_gemm_args a = dgrad_args(dpm, d->w_out, w->d_big, M, H, I);  // d_g, then * gelu'(u) -> d_u
     a.epilogue = VB_EPI_DGELU; a.aux_in = s->u; a.ld_aux = I;
     a.gp_tiled = gemm_gp_tiled_ok(M, I) ? 1 : 0;
     VB_TRY(gemm(a, st));
     // ---- BertIntermediate ----
-    VB_TRY(colsum(w->d_big, I, g->db_inter, M, I, st));
-    VB_TRY(gemm(wgrad_args(w->d_big, s->x1, g->dw_inter, M, I, H), st));
+    if (g->db_inter) VB_TRY(colsum(w->d_big, I, g->db_inter, M, I, st));
+    if (g->dw_inter) VB_TRY(gemm(wgrad_args(w->d_big, s->x1, g->dw_inter, M, I, H), st));
     a = dgrad_args(w->d_big, d->w_inter, w->d_x1, M, I, H);
     a.addend = w->d_pre; a.ld_add = H;  // + residual branch of BertOutput
     VB_TRY(gemm(a, st));
     // ---- BertSelfOutput: LN1, attention.output.dense ----
     VB_TRY(ln_bwd(w->d_x1, s->pre1, s->mean1, s->rstd1, d->ln1_gamma, w->d_pre, hd ? w->d_pre_drop : nullptr,
                   g->dln1_gamma, g->dln1_beta, g->db_attn_out, M, H, d->hidden_dropout, d->seed,
-                  drop_stream(d->layer_index, kSiteAttnOut), 0.f, 0, st));
-    VB_TRY(gemm(wgrad_args(dpm, s->ctx, g->dw_attn_out, M, H, H), st));
+                  drop_stream(d->layer_index, kSiteAttnOut), 0.f, 0, st, g->db_attn_out == nullptr));
+    if (g->dw_attn_out) VB_TRY(gemm(wgrad_args(dpm, s->ctx, g->dw_attn_out, M, H, H), st));
     a = dgrad_args(dpm, d->w_attn_out, w->d_ctx, M, H, H);
     // D = rowsum(dO * O) of the attention backward falls out of this GEMM's epilogue (a thread holds two whole heads of a row);
     // the staged attention kernels compute D themselves
@@ -163,8 +176,9 @@ int layer_bwd(const vb_layer_desc* d, const void* x_in, const vb_layer_acts* s, 
     else
         VB_TRY(attn_bwd(s->qkv, d->mask_bias, s->ctx, s->lse, s->keep_mask, w->d_ctx, w->d_big, w->drow, d->batch, d->seq, d->heads, H,
                         d->attn_dropout, d->seed, drop_stream(d->layer_index, kSiteAttnProbs), st, fused_delta));
-    VB_TRY(colsum(w->d_big, 3 * H, g->db_qkv, M, 3 * H, st));
-    VB_TRY(gemm(wgrad_args(w->d_big, x_in, g->dw_qkv, M, 3 * H, H), st));
+    if (g->db_qkv) VB_TRY(colsum(w->d_big, 3 * H, g->db_qkv, M, 3 * H, st));
+    if (g->dw_qkv) VB_TRY(gemm(wgrad_args(w->d_big, x_in, g->dw_qkv, M, 3 * H, H), st));
+    if (dx == nullptr) return 0;
     a = dgrad_args(w->d_big, d->w_qkv, dx, M, 3 * H, H);
     a.addend = w->d_pre; a.ld_add = H;  // + residual branch of BertSelfOutput
     VB_TRY(gemm(a, st));
@@ -220,7 +234,12 @@ int encoder_fwd(const vb_layer_desc* descs, int n, const void* x_in, void* arena
 
 int encoder_bwd(const vb_layer_desc* descs, int n, const void* x_in, void* arena, const void* dy, void* dx,
                 const vb_layer_grads* grads, const vb_layer_scratch* w, cudaStream_t st, const LayerRows& rows = kDenseRows) {
-    VB_REQUIRE(descs && n > 0 && x_in && arena && dy && dx && grads && w, "encoder_bwd: null pointer / no layers");
+    VB_REQUIRE(descs && n > 0 && x_in && arena && dy && grads && w, "encoder_bwd: null pointer / no layers");
+    for (int l = 0; l < n; ++l) VB_TRY(check_grads(&grads[l]));   // a refused call launches nothing
+    // the gradient between layers ping-pongs inside `dx` (vb_layer_bwd allows dx to alias dy). Without dx it travels in
+    // scratch.d_x1: a layer's d_x1 is dead once its LN1 backward has run, and the layer below reads its dy only in its first
+    // kernel (the LN2 backward), before its FFN-up input-gradient GEMM rewrites d_x1.
+    void* const carry = dx != nullptr ? dx : w->d_x1;
     const void* g_in = dy;
     for (int l = n - 1; l >= 0; --l) {
         vb_layer_acts a;
@@ -233,9 +252,8 @@ int encoder_bwd(const vb_layer_desc* descs, int n, const void* x_in, void* arena
             arena_acts(&descs[l - 1], arena, l - 1, &ap, &yp, rows);
             xl = yp;
         }
-        // the gradient buffer ping-pongs inside `dx` (vb_layer_bwd allows dx to alias dy)
-        VB_TRY(layer_bwd(&descs[l], xl, &a, g_in, dx, &grads[l], w, st, rows));
-        g_in = dx;
+        VB_TRY(layer_bwd(&descs[l], xl, &a, g_in, l > 0 ? carry : dx, &grads[l], w, st, rows));
+        g_in = carry;
     }
     return 0;
 }
@@ -378,7 +396,7 @@ int embed_bwd_api(const vb_embed_desc* d, const vb_embed_acts* s, const void* dy
         VB_TRY(det_require(need, "embed_bwd"));
     }
     VB_TRY(ln_bwd(dy, s->pre, s->mean, s->rstd, d->gamma, g->d_pre, nullptr, g->dgamma, g->dbeta, nullptr, M, H, 0.f,
-                  d->seed, 0, d->dropout, kEmbedDropStream, st));
+                  d->seed, 0, d->dropout, kEmbedDropStream, st, !g->dgamma && !g->dbeta));
     EmbedBwdParams p;
     memset(&p, 0, sizeof(p));
     p.de = static_cast<const bf16*>(g->d_pre);
@@ -391,8 +409,8 @@ int embed_bwd_api(const vb_embed_desc* d, const vb_embed_acts* s, const void* dy
     p.vocab = d->vocab; p.max_pos = d->max_pos; p.n_types = d->n_types;
     VB_TRY(embed_bwd(p, st));
     if (BV > 0) {
-        VB_TRY(colsum(g->d_vis, H, g->db_proj, BV, H, st));
-        VB_TRY(gemm(wgrad_args(g->d_vis, d->visual_feats, g->dw_proj, BV, H, d->visual_dim), st));
+        if (g->db_proj) VB_TRY(colsum(g->d_vis, H, g->db_proj, BV, H, st));
+        if (g->dw_proj) VB_TRY(gemm(wgrad_args(g->d_vis, d->visual_feats, g->dw_proj, BV, H, d->visual_dim), st));
         if (g->d_feats) VB_TRY(gemm(dgrad_args(g->d_vis, d->w_proj, g->d_feats, BV, H, d->visual_dim), st));
     }
     return 0;

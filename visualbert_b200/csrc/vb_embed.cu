@@ -122,9 +122,9 @@ __global__ void __launch_bounds__(kEmbWarps * 32) embed_fwd_off_kernel(const Emb
 // examples at a fixed sequence position (a warp task = (position s, 32 examples)), so each table row receives one vector
 // reduction per task instead of one scalar atomic per element (which made atomic contention the bulk of the kernel's time).
 // smem: [n_types][H] text types, [n_types][H] visual types, [H] visual position row 0 (block accumulators, flushed once)
-template <int NC>
-__global__ void __launch_bounds__(kEmbWarps * 32)
-embed_bwd_kernel(const EmbedBwdParams p, int cb, int nb) {
+// FROZEN (embed_bwd_frozen_kernel): some gradient tables are NULL (frozen); they receive nothing.
+template <int NC, bool FROZEN>
+__device__ __forceinline__ void embed_bwd_body(const EmbedBwdParams& p, int cb, int nb) {
     extern __shared__ float acc[];
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int H = p.H, chunks = H >> 3, S = p.T + p.V, nt = p.n_types;
@@ -147,7 +147,8 @@ embed_bwd_kernel(const EmbedBwdParams p, int cb, int nb) {
             bf16* dv = nullptr;
             int ty;
             if (text) {
-                g0 = p.dword + static_cast<long long>(clampi(p.ids[static_cast<long long>(b) * p.T + s], p.vocab)) * H;
+                if (!FROZEN || p.dword != nullptr)
+                    g0 = p.dword + static_cast<long long>(clampi(p.ids[static_cast<long long>(b) * p.T + s], p.vocab)) * H;
                 ty = clampi(p.tt[static_cast<long long>(b) * p.T + s], nt);
             } else {
                 dv = p.dvis + (static_cast<long long>(b) * p.V + (s - p.T)) * H;
@@ -176,7 +177,8 @@ embed_bwd_kernel(const EmbedBwdParams p, int cb, int nb) {
             }
         }
         // flush the task: position row (text: global table row s; visual: the block's accumulator of visual position 0), types
-        float* prow = text ? p.dpos + static_cast<long long>(s < p.max_pos ? s : p.max_pos - 1) * H : nullptr;
+        float* prow = text && (!FROZEN || p.dpos != nullptr) ? p.dpos + static_cast<long long>(s < p.max_pos ? s : p.max_pos - 1) * H
+                                                              : nullptr;
         float* a0 = acc + (text ? 0 : nt) * H;
 #pragma unroll
         for (int c = 0; c < NC; ++c) {
@@ -188,7 +190,7 @@ embed_bwd_kernel(const EmbedBwdParams p, int cb, int nb) {
                 }
 #pragma unroll
                 for (int i = 0; i < 8; ++i) {
-                    if (prow == nullptr) atomicAdd(acc + 2 * nt * H + ch * 8 + i, psum[c][i]);
+                    if (FROZEN ? !text : prow == nullptr) atomicAdd(acc + 2 * nt * H + ch * 8 + i, psum[c][i]);
                     atomicAdd(a0 + ch * 8 + i, t0[c][i]);
                     if (nt > 1) atomicAdd(a0 + H + ch * 8 + i, t1[c][i]);
                 }
@@ -197,10 +199,19 @@ embed_bwd_kernel(const EmbedBwdParams p, int cb, int nb) {
     }
     __syncthreads();
     for (int i = threadIdx.x; i < nt * H; i += blockDim.x) {
-        atomicAdd(p.dtype + i, acc[i]);
-        atomicAdd(p.dtype_vis + i, acc[nt * H + i]);
+        if (!FROZEN || p.dtype != nullptr) atomicAdd(p.dtype + i, acc[i]);
+        if (!FROZEN || p.dtype_vis != nullptr) atomicAdd(p.dtype_vis + i, acc[nt * H + i]);
     }
-    for (int i = threadIdx.x; i < H; i += blockDim.x) atomicAdd(p.dpos_vis + i, acc[2 * nt * H + i]);
+    if (!FROZEN || p.dpos_vis != nullptr)
+        for (int i = threadIdx.x; i < H; i += blockDim.x) atomicAdd(p.dpos_vis + i, acc[2 * nt * H + i]);
+}
+template <int NC>
+__global__ void __launch_bounds__(kEmbWarps * 32) embed_bwd_kernel(const EmbedBwdParams p, int cb, int nb) {
+    embed_bwd_body<NC, false>(p, cb, nb);
+}
+template <int NC>
+__global__ void __launch_bounds__(kEmbWarps * 32, 1) embed_bwd_frozen_kernel(const EmbedBwdParams p, int cb, int nb) {
+    embed_bwd_body<NC, true>(p, cb, nb);
 }
 
 __global__ void mask_bias_kernel(const long long* __restrict__ input_mask, const long long* __restrict__ image_mask,
@@ -299,14 +310,14 @@ constexpr int kSegWin = 64;
 
 __device__ __forceinline__ float* embed_key_row(const EmbedBwdParams& p, unsigned k) {
     const long long H = p.H;
-    if (k < static_cast<unsigned>(p.vocab)) return p.dword + k * H;
+    if (k < static_cast<unsigned>(p.vocab)) return p.dword ? p.dword + k * H : nullptr;
     k -= p.vocab;
-    if (k < static_cast<unsigned>(p.max_pos)) return p.dpos + k * H;
+    if (k < static_cast<unsigned>(p.max_pos)) return p.dpos ? p.dpos + k * H : nullptr;
     k -= p.max_pos;
-    if (k < static_cast<unsigned>(p.n_types)) return p.dtype + k * H;
+    if (k < static_cast<unsigned>(p.n_types)) return p.dtype ? p.dtype + k * H : nullptr;
     k -= p.n_types;
     if (k == 0) return p.dpos_vis;
-    return p.dtype_vis + (k - 1) * H;
+    return p.dtype_vis ? p.dtype_vis + (k - 1) * H : nullptr;
 }
 
 // one thread per row of de: its (key, row) items; the visual rows are also copied to dvis (the projection's weight-gradient input)
@@ -374,7 +385,9 @@ __device__ __forceinline__ void seg_flush(float* dst, bool add, int H, int lane,
 }
 
 // one warp per window; slots: [2][windows][H] fp32 (0: head partials, 1: tail partials)
-template <int NC>
+// FROZEN: some tables are NULL (frozen). Their items stay in the sort, so every window and sum order is that of the full call,
+// but their runs are neither summed nor flushed.
+template <int NC, bool FROZEN = false>
 __global__ void __launch_bounds__(kEmbWarps * 32)
 embed_seg_kernel(const EmbedBwdParams p, const unsigned* __restrict__ keys, const int* __restrict__ vals, int n, float* __restrict__ slots) {
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -390,6 +403,9 @@ embed_seg_kernel(const EmbedBwdParams p, const unsigned* __restrict__ keys, cons
     int run_beg = beg;
     for (int i = beg; i < end; ++i) {
         const unsigned k = keys[i];
+        if constexpr (FROZEN) {
+            if (embed_key_row(p, k) == nullptr) { run_beg = i + 1; continue; }
+        }
         seg_add_row<NC>(p, vals[i], lane, acc);
         const bool run_end = i + 1 == n || keys[i + 1] != k;
         if (run_end || i + 1 == end) {
@@ -403,7 +419,7 @@ embed_seg_kernel(const EmbedBwdParams p, const unsigned* __restrict__ keys, cons
 }
 
 // one warp per window: the window a crossing run started in adds its tail partial and the head partials of the following windows
-template <int NC>
+template <int NC, bool FROZEN = false>
 __global__ void __launch_bounds__(kEmbWarps * 32)
 embed_seg_join_kernel(const EmbedBwdParams p, const unsigned* __restrict__ keys, int n, const float* __restrict__ slots) {
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -413,6 +429,9 @@ embed_seg_join_kernel(const EmbedBwdParams p, const unsigned* __restrict__ keys,
     const unsigned k = keys[end - 1];
     const bool starts_here = !(beg > 0 && keys[beg - 1] == k && keys[beg] == k);
     if (!starts_here || end == n || keys[end] != k) return;
+    if constexpr (FROZEN) {
+        if (embed_key_row(p, k) == nullptr) return;
+    }
     float acc[NC][8];
 #pragma unroll
     for (int c = 0; c < NC; ++c)
@@ -523,14 +542,15 @@ static int embed_bwd_det(const EmbedBwdParams& p, const DetWs& det, cudaStream_t
     VB_CHECK_CUDA(cub::DeviceRadixSort::SortPairs(sort_temp, tb, kb, vb, static_cast<int>(n), 0, end_bit, st));
     const unsigned* keys = kb.Current();
     const int* vals = vb.Current();
-#define VB_SEG(NC)                                                                                                        \
-    embed_seg_kernel<NC><<<seg_grid, kEmbWarps * 32, 0, st>>>(p, keys, vals, static_cast<int>(n), slots);                \
-    embed_seg_join_kernel<NC><<<seg_grid, kEmbWarps * 32, 0, st>>>(p, keys, static_cast<int>(n), slots)
+#define VB_SEG(NC, F)                                                                                                     \
+    embed_seg_kernel<NC, F><<<seg_grid, kEmbWarps * 32, 0, st>>>(p, keys, vals, static_cast<int>(n), slots);             \
+    embed_seg_join_kernel<NC, F><<<seg_grid, kEmbWarps * 32, 0, st>>>(p, keys, static_cast<int>(n), slots)
+    const bool frozen = !p.dword || !p.dpos || !p.dtype || !p.dpos_vis || !p.dtype_vis;
     switch (nc) {
-        case 1: VB_SEG(1); break;
-        case 2: VB_SEG(2); break;
-        case 3: VB_SEG(3); break;
-        default: VB_SEG(4); break;
+        case 1: if (frozen) { VB_SEG(1, true); } else { VB_SEG(1, false); } break;
+        case 2: if (frozen) { VB_SEG(2, true); } else { VB_SEG(2, false); } break;
+        case 3: if (frozen) { VB_SEG(3, true); } else { VB_SEG(3, false); } break;
+        default: if (frozen) { VB_SEG(4, true); } else { VB_SEG(4, false); } break;
     }
 #undef VB_SEG
     VB_CHECK_CUDA(cudaGetLastError());
@@ -543,6 +563,8 @@ int embed_bwd(const EmbedBwdParams& p, cudaStream_t st) {
                "embed backward: gradient tables must be 16-byte aligned");
     const DetWs det = det_ws();
     if (det.ptr != nullptr) return embed_bwd_det(p, det, st);
+    const bool frozen = !p.dword || !p.dpos || !p.dtype || !p.dpos_vis || !p.dtype_vis;
+    if (!p.dword && !p.dpos && !p.dtype && !p.dpos_vis && !p.dtype_vis && p.V == 0) return 0;   // nothing to scatter or copy
     const long long rows = static_cast<long long>(p.B) * (p.T + p.V);
     const int cb = p.B < 32 ? p.B : 32, nb = (p.B + cb - 1) / cb;   // a warp task: one sequence position, up to 32 examples
     const long long tasks = static_cast<long long>(p.T + p.V) * nb;
@@ -554,11 +576,20 @@ int embed_bwd(const EmbedBwdParams& p, cudaStream_t st) {
     const int nc = (p.H / 8 + 31) / 32;
     {
         ProfScope ps(st, PROF_EMBED, 6.0 * rows * p.H, 1);
-        switch (nc) {
-            case 1: embed_bwd_kernel<1><<<grid, kEmbWarps * 32, smem, st>>>(p, cb, nb); break;
-            case 2: embed_bwd_kernel<2><<<grid, kEmbWarps * 32, smem, st>>>(p, cb, nb); break;
-            case 3: embed_bwd_kernel<3><<<grid, kEmbWarps * 32, smem, st>>>(p, cb, nb); break;
-            default: embed_bwd_kernel<4><<<grid, kEmbWarps * 32, smem, st>>>(p, cb, nb); break;
+        if (frozen) {
+            switch (nc) {
+                case 1: embed_bwd_frozen_kernel<1><<<grid, kEmbWarps * 32, smem, st>>>(p, cb, nb); break;
+                case 2: embed_bwd_frozen_kernel<2><<<grid, kEmbWarps * 32, smem, st>>>(p, cb, nb); break;
+                case 3: embed_bwd_frozen_kernel<3><<<grid, kEmbWarps * 32, smem, st>>>(p, cb, nb); break;
+                default: embed_bwd_frozen_kernel<4><<<grid, kEmbWarps * 32, smem, st>>>(p, cb, nb); break;
+            }
+        } else {
+            switch (nc) {
+                case 1: embed_bwd_kernel<1><<<grid, kEmbWarps * 32, smem, st>>>(p, cb, nb); break;
+                case 2: embed_bwd_kernel<2><<<grid, kEmbWarps * 32, smem, st>>>(p, cb, nb); break;
+                case 3: embed_bwd_kernel<3><<<grid, kEmbWarps * 32, smem, st>>>(p, cb, nb); break;
+                default: embed_bwd_kernel<4><<<grid, kEmbWarps * 32, smem, st>>>(p, cb, nb); break;
+            }
         }
     }
     VB_CHECK_CUDA(cudaGetLastError());

@@ -12,7 +12,8 @@ int ln_fwd(const void* x, long long ldx, const float* gamma, const float* beta, 
            float* rstd, int rows, int H, float eps, cudaStream_t st);
 int ln_bwd(const void* dy, const void* x, const float* mean, const float* rstd, const float* gamma, void* dx,
            void* dx_drop, float* dgamma, float* dbeta, float* dbias, int rows, int H, float dropout_p,
-           unsigned long long seed, unsigned stream_id, float in_dropout_p, unsigned in_stream_id, cudaStream_t st);
+           unsigned long long seed, unsigned stream_id, float in_dropout_p, unsigned in_stream_id, cudaStream_t st,
+           bool rows_only = false);   // rows_only: dgamma, dbeta and dbias are all NULL and no column reduction runs
 // The attention kernels that serve a call, from its sequence length (varlen calls: the longest one): the wgmma kernels up to
 // 192 (their backward keeps Q, K, V, dO and P/dS of the whole head in shared memory), the whole-head mma.sync kernels up to
 // 256, the staged kernels beyond. The two fused routes take a pre-computed D = rowsum(dO * O) (delta_ready below).

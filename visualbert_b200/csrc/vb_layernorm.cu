@@ -103,7 +103,9 @@ __device__ __forceinline__ int slot(int a, int h, int ch, int chunks) { return (
 // PART = false: the block's column sums go to dgamma / dbeta / dbias by atomicAdd. PART = true (deterministic mode): dgamma is
 // the workspace and block b STORES its sums to dgamma[(b * 3 + array) * H + col]; partials_reduce adds them in block order.
 // OFF = true (vb_set_dropout_offset): the dropout seed is drop_seed + *drop_offset, read once global memory may be touched.
-template <int NC, bool PART, bool OFF = false>
+// SUMS = false (a caller whose dgamma, dbeta and dbias are all frozen): a pure row pass — dx and dx_drop only, no shared-memory
+// accumulators, no atomics and no partial stores; PART is then meaningless and dgamma / dbeta / dbias are not read.
+template <int NC, bool PART, bool OFF = false, bool SUMS = true>
 __device__ __forceinline__ void
 ln_bwd_body(const bf16* __restrict__ dy, const bf16* __restrict__ x, const float* __restrict__ mean,
             const float* __restrict__ rstd, const float* __restrict__ gamma, bf16* __restrict__ dx,
@@ -117,7 +119,8 @@ ln_bwd_body(const bf16* __restrict__ dy, const bf16* __restrict__ x, const float
     float4* sgam = sm4;
     float4* acc = sm4 + 2 * chunks + warp * 6 * chunks;
     pdl_trigger();
-    for (int i = threadIdx.x; i < kLnWarps * 6 * chunks; i += blockDim.x) sm4[2 * chunks + i] = make_float4(0.f, 0.f, 0.f, 0.f);
+    if constexpr (SUMS)
+        for (int i = threadIdx.x; i < kLnWarps * 6 * chunks; i += blockDim.x) sm4[2 * chunks + i] = make_float4(0.f, 0.f, 0.f, 0.f);
     pdl_wait();  // the accumulators are cleared while the previous kernel drains; global memory is touched from here on
     // OFF: the hash keys of the summed seed wait in shared memory (the 64-bit sum held in registers spills the NC = 4 build)
     __shared__ uint32_t s_key[2];   // [0]: hidden dropout (drop_stream), [1]: in_dropout (in_stream)
@@ -214,18 +217,21 @@ ln_bwd_body(const bf16* __restrict__ dy, const bf16* __restrict__ x, const float
                     for (int i = 0; i < 8; ++i) o[i] = ((keep >> i) & 1u) ? o[i] * drop_scale : 0.f;
                     stg_v4(dx_drop + rbase + ch * 8, pack8(o));
                 }
-                const float* d = dv[c];
-                const float* h = xh[c];
-                float4 a;
-                a = acc[slot(0, 0, ch, chunks)]; a.x = fmaf(d[0], h[0], a.x); a.y = fmaf(d[1], h[1], a.y); a.z = fmaf(d[2], h[2], a.z); a.w = fmaf(d[3], h[3], a.w); acc[slot(0, 0, ch, chunks)] = a;
-                a = acc[slot(0, 1, ch, chunks)]; a.x = fmaf(d[4], h[4], a.x); a.y = fmaf(d[5], h[5], a.y); a.z = fmaf(d[6], h[6], a.z); a.w = fmaf(d[7], h[7], a.w); acc[slot(0, 1, ch, chunks)] = a;
-                a = acc[slot(1, 0, ch, chunks)]; a.x += d[0]; a.y += d[1]; a.z += d[2]; a.w += d[3]; acc[slot(1, 0, ch, chunks)] = a;
-                a = acc[slot(1, 1, ch, chunks)]; a.x += d[4]; a.y += d[5]; a.z += d[6]; a.w += d[7]; acc[slot(1, 1, ch, chunks)] = a;
-                a = acc[slot(2, 0, ch, chunks)]; a.x += o[0]; a.y += o[1]; a.z += o[2]; a.w += o[3]; acc[slot(2, 0, ch, chunks)] = a;
-                a = acc[slot(2, 1, ch, chunks)]; a.x += o[4]; a.y += o[5]; a.z += o[6]; a.w += o[7]; acc[slot(2, 1, ch, chunks)] = a;
+                if constexpr (SUMS) {
+                    const float* d = dv[c];
+                    const float* h = xh[c];
+                    float4 a;
+                    a = acc[slot(0, 0, ch, chunks)]; a.x = fmaf(d[0], h[0], a.x); a.y = fmaf(d[1], h[1], a.y); a.z = fmaf(d[2], h[2], a.z); a.w = fmaf(d[3], h[3], a.w); acc[slot(0, 0, ch, chunks)] = a;
+                    a = acc[slot(0, 1, ch, chunks)]; a.x = fmaf(d[4], h[4], a.x); a.y = fmaf(d[5], h[5], a.y); a.z = fmaf(d[6], h[6], a.z); a.w = fmaf(d[7], h[7], a.w); acc[slot(0, 1, ch, chunks)] = a;
+                    a = acc[slot(1, 0, ch, chunks)]; a.x += d[0]; a.y += d[1]; a.z += d[2]; a.w += d[3]; acc[slot(1, 0, ch, chunks)] = a;
+                    a = acc[slot(1, 1, ch, chunks)]; a.x += d[4]; a.y += d[5]; a.z += d[6]; a.w += d[7]; acc[slot(1, 1, ch, chunks)] = a;
+                    a = acc[slot(2, 0, ch, chunks)]; a.x += o[0]; a.y += o[1]; a.z += o[2]; a.w += o[3]; acc[slot(2, 0, ch, chunks)] = a;
+                    a = acc[slot(2, 1, ch, chunks)]; a.x += o[4]; a.y += o[5]; a.z += o[6]; a.w += o[7]; acc[slot(2, 1, ch, chunks)] = a;
+                }
             }
         }
     }
+    if constexpr (!SUMS) return;
     __syncthreads();
     // reduce the 8 warp slabs and flush: one global atomic per column per array per block
     const float* accf = reinterpret_cast<const float*>(sm4 + 2 * chunks);
@@ -264,6 +270,15 @@ template <int NC>
 __global__ void __launch_bounds__(kLnWarps * 32, 2)
 ln_bwd_part_off_kernel(VB_LN_BWD_PARAMS, const unsigned long long* __restrict__ drop_offset) {
     ln_bwd_body<NC, true, true>(VB_LN_BWD_ARGS, drop_offset);
+}
+template <int NC>
+__global__ void __launch_bounds__(kLnWarps * 32, 2)
+ln_bwd_rows_kernel(VB_LN_BWD_PARAMS) { ln_bwd_body<NC, false, false, false>(VB_LN_BWD_ARGS); }
+// NC = 4 with the offset spills at 2 blocks per SM (128 registers): one block per SM there, two everywhere else
+template <int NC>
+__global__ void __launch_bounds__(kLnWarps * 32, NC == 4 ? 1 : 2)
+ln_bwd_rows_off_kernel(VB_LN_BWD_PARAMS, const unsigned long long* __restrict__ drop_offset) {
+    ln_bwd_body<NC, false, true, false>(VB_LN_BWD_ARGS, drop_offset);
 }
 #undef VB_LN_BWD_PARAMS
 #undef VB_LN_BWD_ARGS
@@ -328,7 +343,8 @@ int ln_fwd(const void* x, long long ldx, const float* gamma, const float* beta, 
 
 int ln_bwd(const void* dy, const void* x, const float* mean, const float* rstd, const float* gamma, void* dx,
            void* dx_drop, float* dgamma, float* dbeta, float* dbias, int rows, int H, float dropout_p,
-           unsigned long long seed, unsigned stream_id, float in_dropout_p, unsigned in_stream_id, cudaStream_t st) {
+           unsigned long long seed, unsigned stream_id, float in_dropout_p, unsigned in_stream_id, cudaStream_t st,
+           bool rows_only) {
     VB_REQUIRE(H % 8 == 0 && H <= 1024, "layernorm backward: H=%d must be a multiple of 8 and <= 1024", H);
     VB_REQUIRE(rows > 0, "layernorm backward: no rows");
     VB_REQUIRE((dropout_p > 0.f) == (dx_drop != nullptr), "layernorm backward: dx_drop iff dropout_p > 0");
@@ -336,13 +352,43 @@ int ln_bwd(const void* dy, const void* x, const float* mean, const float* rstd, 
     VB_REQUIRE(all_aligned16(dy, x, gamma, dx, dx_drop), "layernorm backward: dy, x, gamma, dx and dx_drop must be 16-byte aligned");
     const int nc = (H / 8 + 31) / 32;
     const int grid = ln_bwd_grid(rows);
+    VB_REQUIRE(!rows_only || (!dgamma && !dbeta && !dbias), "layernorm backward: a row-only call takes no column sums");
     const DetWs det = det_ws();
-    if (det.ptr != nullptr) VB_TRY_RC(det_require(ln_bwd_det_bytes(rows, H), "layernorm backward"));
+    if (det.ptr != nullptr && !rows_only) VB_TRY_RC(det_require(ln_bwd_det_bytes(rows, H), "layernorm backward"));
     // the offset kernels only when this call draws dropout bits (hidden dropout or the embeddings' in_dropout)
     const unsigned long long* off = (dropout_p > 0.f || in_dropout_p > 0.f) ? drop_offset() : nullptr;
     const DropQ dq = dropout_quantise(dropout_p), iq = dropout_quantise(in_dropout_p);
     const float scale = dq.scale, in_scale = iq.scale;
     const unsigned th = dq.thr8, in_th = iq.thr8;
+    if (rows_only) {   // same arithmetic per row, no column reductions: deterministic mode has nothing to order
+        const size_t rsmem = static_cast<size_t>(2 * (H / 8)) * sizeof(float4);
+        {
+            ProfScope ps(st, PROF_LN_BWD, (dx_drop ? 8.0 : 6.0) * rows * H, 1);
+#define VB_LN_ROWS(K, NC, ...)                                                                               \
+    VB_CHECK_CUDA(launch_pdl(K<NC>, dim3(grid), dim3(kLnWarps * 32), rsmem, st,                             \
+        static_cast<const bf16*>(dy), static_cast<const bf16*>(x), mean, rstd, gamma, static_cast<bf16*>(dx), \
+        static_cast<bf16*>(dx_drop), nullptr, nullptr, nullptr, rows, H, scale, th, seed, stream_id,          \
+        in_scale, in_th, __VA_ARGS__))
+            if (off != nullptr) {
+                switch (nc) {
+                    case 1: VB_LN_ROWS(ln_bwd_rows_off_kernel, 1, in_stream_id, off); break;
+                    case 2: VB_LN_ROWS(ln_bwd_rows_off_kernel, 2, in_stream_id, off); break;
+                    case 3: VB_LN_ROWS(ln_bwd_rows_off_kernel, 3, in_stream_id, off); break;
+                    default: VB_LN_ROWS(ln_bwd_rows_off_kernel, 4, in_stream_id, off); break;
+                }
+            } else {
+                switch (nc) {
+                    case 1: VB_LN_ROWS(ln_bwd_rows_kernel, 1, in_stream_id); break;
+                    case 2: VB_LN_ROWS(ln_bwd_rows_kernel, 2, in_stream_id); break;
+                    case 3: VB_LN_ROWS(ln_bwd_rows_kernel, 3, in_stream_id); break;
+                    default: VB_LN_ROWS(ln_bwd_rows_kernel, 4, in_stream_id); break;
+                }
+            }
+#undef VB_LN_ROWS
+        }
+        VB_CHECK_CUDA(cudaGetLastError());
+        return 0;
+    }
     const size_t smem = static_cast<size_t>(2 * (H / 8) + kLnWarps * 6 * (H / 8)) * sizeof(float4);
     static int cfg1[kMaxDevices] = {0}, cfg2[kMaxDevices] = {0}, cfg3[kMaxDevices] = {0}, cfg4[kMaxDevices] = {0};
     VB_CHECK_CUDA(ensure_dyn_smem(ln_bwd_kernel<1>, 100 * 1024, cfg1));
@@ -432,6 +478,6 @@ int vb_layernorm_bwd(const void* dy, const void* x, const float* mean, const flo
                      int32_t hidden, float dropout_p, uint64_t dropout_seed, uint32_t dropout_stream,
                      float in_dropout_p, uint32_t in_dropout_stream, void* stream) {
     return vb::ln_bwd(dy, x, mean, rstd, gamma, dx, dx_drop, dgamma, dbeta, dbias, rows, hidden, dropout_p,
-                      dropout_seed, dropout_stream, in_dropout_p, in_dropout_stream, static_cast<cudaStream_t>(stream));
+                      dropout_seed, dropout_stream, in_dropout_p, in_dropout_stream, static_cast<cudaStream_t>(stream), false);
 }
 }

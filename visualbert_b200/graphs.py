@@ -50,7 +50,10 @@ class GraphedStep:
     graph-capturable mode and stepped at the end of every step, after the all-reduce. Before each replay its group table is
     uploaded if a group's lr, weight decay or schedule changed; a graph whose optimizer tables were rebuilt since its capture
     (load_state_dict, a new set of tensors) or whose (b1, b2, e, max_grad_norm) changed is dropped and captured again. With
-    gradient accumulation the optimizer must stay outside (it steps once per several calls)."""
+    gradient accumulation the optimizer must stay outside (it steps once per several calls).
+
+    The set of trainable parameters (requires_grad) is part of the signature: after a parameter is frozen or unfrozen the next
+    calls warm up and capture again, as for a new input shape."""
 
     def __init__(self, model, sync, loss_scale=None, warmup=1, max_graphs=4, optimizer=None):
         if not model.training:
@@ -107,7 +110,8 @@ class GraphedStep:
         return _Captured(graph, inputs, outputs, opt._graph_signature(), opt._graph_params())
 
     def __call__(self, batch):
-        sig = _signature(batch)
+        # which parameters train is part of the signature: a graph writes the gradients of the set it was captured with
+        sig = (_signature(batch), tuple(p.requires_grad for p in self.model.parameters()))
         entry = self.graphs.get(sig)
         if entry is not None and self.optimizer is not None:
             if entry.opt_signature != self.optimizer._graph_signature():   # the graph holds stale pointers or arguments

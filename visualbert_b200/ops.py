@@ -205,24 +205,30 @@ def mask_bias(input_mask, image_mask):
     return out
 
 
-def _grad_targets(params, adjacent_groups=()):
+def _grad_targets(params, adjacent_groups=(), trainable=None):
     """Direct-accumulate mode — OPT-IN: only parameters a gradient owner has flagged with `_vb_direct_grad = True`
     (parallel.FlatGradSync does, for the views of its flat buffer) get their gradients written straight into `.grad`
     by the kernels (all gradient outputs of the C ABI are `+=`), with autograd receiving None. Everyone else — plain
     optimizers, DDP with gradient_as_bucket_view, tensor / post-accumulate hooks, torch.autograd.grad — goes through
     AccumulateGrad as usual: the caller allocates fresh zero buffers and returns them to autograd.
     Additionally every `.grad` must be a contiguous fp32 tensor of the parameter's shape, and the parameters of each
-    adjacent group must be laid out back to back."""
-    for p in params:
+    adjacent group must be laid out back to back.
+    trainable (default: every requires_grad): flags per parameter. Frozen parameters are ignored — their entry is None and
+    nothing is written to their `.grad` — and an adjacent group is only checked when all its members train."""
+    if trainable is None:
+        trainable = [p.requires_grad for p in params]
+    for p, t in zip(params, trainable):
         g = p.grad
-        if (not getattr(p, "_vb_direct_grad", False) or g is None or g.dtype != torch.float32 or not g.is_contiguous()
-                or g.device != p.device or g.shape != p.shape):
+        if t and (not getattr(p, "_vb_direct_grad", False) or g is None or g.dtype != torch.float32 or not g.is_contiguous()
+                  or g.device != p.device or g.shape != p.shape):
             return None
+    live = {id(p) for p, t in zip(params, trainable) if t}
     for group in adjacent_groups:
-        for a, b in zip(group[:-1], group[1:]):
-            if a.grad.data_ptr() + a.grad.numel() * 4 != b.grad.data_ptr():
-                return None
-    return [p.grad for p in params]
+        if all(id(p) in live for p in group):
+            for a, b in zip(group[:-1], group[1:]):
+                if a.grad.data_ptr() + a.grad.numel() * 4 != b.grad.data_ptr():
+                    return None
+    return [p.grad if t else None for p, t in zip(params, trainable)]
 
 
 class WeightBank:
@@ -343,49 +349,79 @@ def attention_probs(qkv, mbias, B, S, A):
     return probs
 
 
-_GRAD_FIELDS = ("dw_qkv", "db_qkv", "dw_attn_out", "db_attn_out", "dln1_gamma", "dln1_beta",
-                "dw_inter", "db_inter", "dw_out", "db_out", "dln2_gamma", "dln2_beta")   # vb_layer_grads
+# vb_layer_grads fields and the indices (in bert_layer order) of the parameters each one holds, packed back to back
+_GRAD_FIELDS = (("dw_qkv", (0, 2, 4)), ("db_qkv", (1, 3, 5)), ("dw_attn_out", (6,)), ("db_attn_out", (7,)), ("dln1_gamma", (8,)),
+                ("dln1_beta", (9,)), ("dw_inter", (10,)), ("db_inter", (11,)), ("dw_out", (12,)), ("db_out", (13,)),
+                ("dln2_gamma", (14,)), ("dln2_beta", (15,)))
+# a LayerNorm backward computes these three together (vb_layer_grads): all three pointers are given or none
+_LN_GROUPS = (("db_attn_out", "dln1_gamma", "dln1_beta"), ("db_out", "dln2_gamma", "dln2_beta"))
 
 
-def _grad_sizes(H, I):
-    return [3 * H * H, 3 * H, H * H, H, H, H, I * H, I, H * I, H, H, H]
+def encoder_grad_plan(params, trainable, input_grad):
+    """What the backward of an encoder call computes, from the parameters' requires_grad flags alone: a frozen parameter gets
+    no gradient work unless it shares one output with a trainable one.
+    params: 16 tensors per layer in bert_layer order; trainable: their flags; input_grad: whether the encoder input needs a
+    gradient. Returns (l0, layers): l0 is the lowest layer the backward must reach (0 when the input needs a gradient, L when
+    nothing does): layers below it can run forward-only. layers[l] (for l >= l0) = (direct, {field: kind}) with kind
+    "grad" (the kernels accumulate into the parameter's own `.grad`), "buffer" (into a zeroed fp32 buffer: handed to autograd,
+    or added to `.grad` afterwards when only part of a packed output trains) or "null" (not computed). direct: every trainable
+    tensor of the layer is a `_vb_direct_grad` view (_grad_targets), so no buffer reaches autograd."""
+    L = len(params) // 16
+    live = [any(trainable[16 * l: 16 * l + 16]) for l in range(L)]
+    l0 = 0 if input_grad else next((l for l in range(L) if live[l]), L)
+    layers = []
+    for l in range(l0, L):
+        ps, tr = params[16 * l: 16 * l + 16], trainable[16 * l: 16 * l + 16]
+        direct = _grad_targets(ps, ((ps[0], ps[2], ps[4]), (ps[1], ps[3], ps[5])), tr) is not None
+        kinds = {}
+        for name, idx in _GRAD_FIELDS:
+            n = sum(tr[i] for i in idx)
+            kinds[name] = "null" if n == 0 else ("grad" if direct and n == len(idx) else "buffer")
+        for group in _LN_GROUPS:   # a frozen member of a group that runs is computed into a buffer and dropped
+            if any(kinds[f] != "null" for f in group):
+                for f in group:
+                    if kinds[f] == "null":
+                        kinds[f] = "buffer"
+        layers.append((direct, kinds))
+    return l0, layers
 
 
-def _layer_grads(params, L, H, I, dev):
-    """The vb_layer_grads array of an L-layer backward and the buffer behind it: None when every pointer is a parameter's own
-    `.grad` (_grad_targets; q|k|v are one packed output, so each layer's q, k, v weights and biases must be adjacent), else
-    one zeroed flat fp32 buffer that _autograd_grads cuts up."""
-    groups = []
-    for l in range(L):
-        qw, qb, kw, kb, vw, vb = params[16 * l: 16 * l + 6]
-        groups += [(qw, kw, vw), (qb, kb, vb)]
-    direct = _grad_targets(params, groups)
+def _field_shape(name, H, I):
+    return {"dw_qkv": (H, H), "dw_attn_out": (H, H), "dw_inter": (I, H), "dw_out": (H, I), "db_inter": (I,)}.get(name, (H,))
+
+
+def _layer_grads(params, trainable, plan, H, I, dev):
+    """The vb_layer_grads array of a backward over the layers of `plan` (encoder_grad_plan's layers, for params[16 * l0:]) and
+    the fp32 buffer behind its "buffer" fields: None when there are none. Returns (grads, flat, pieces); pieces lists
+    (parameter index, view of flat) for every trainable parameter whose gradient is in flat."""
+    L = len(plan)
     grads = (_lib.LayerGrads * L)()
-    if direct is not None:
-        for l in range(L):
-            t = direct[16 * l: 16 * l + 16]
-            for name, g in zip(_GRAD_FIELDS, (t[0], t[1]) + tuple(t[6:16])):
-                setattr(grads[l], name, g.data_ptr())
-        return grads, None
-    sizes = _grad_sizes(H, I)
-    flat = torch.zeros(L * sum(sizes), device=dev, dtype=torch.float32)
-    o = flat.data_ptr()
-    for l in range(L):
-        for name, sz in zip(_GRAD_FIELDS, sizes):
-            setattr(grads[l], name, o)
-            o += 4 * sz
-    return grads, flat
-
-
-def _autograd_grads(flat, L, H, I):
-    """The 16 parameter gradients per layer, in bert_layer order, as views of _layer_grads' flat buffer."""
-    out = []
-    for part in flat.view(L, -1).unbind(0):
-        dwqkv, dbqkv, dwo, dbo, dg1, db1, dwi, dbi, dwout, dbout, dg2, db2 = torch.split(part, _grad_sizes(H, I))
-        dwq, dwk, dwv = dwqkv.view(3, H, H).unbind(0)
-        dbq, dbk, dbv = dbqkv.view(3, H).unbind(0)
-        out += [dwq, dbq, dwk, dbk, dwv, dbv, dwo.view(H, H), dbo, dg1, db1, dwi.view(I, H), dbi, dwout.view(H, I), dbout, dg2, db2]
-    return tuple(out)
+    sizes = []
+    for direct, kinds in plan:
+        for name, idx in _GRAD_FIELDS:
+            if kinds[name] == "buffer":
+                n = 1
+                for d in _field_shape(name, H, I):
+                    n *= d
+                sizes.append(n * len(idx))
+    flat = torch.zeros(sum(sizes), device=dev, dtype=torch.float32) if sizes else None
+    pieces, o = [], 0
+    for l, (direct, kinds) in enumerate(plan):
+        for name, idx in _GRAD_FIELDS:
+            kind = kinds[name]
+            if kind == "grad":
+                setattr(grads[l], name, params[16 * l + idx[0]].grad.data_ptr())
+            elif kind == "buffer":
+                shape = _field_shape(name, H, I)
+                n = 1
+                for d in shape:
+                    n *= d
+                setattr(grads[l], name, flat.data_ptr() + 4 * o)
+                for j, i in enumerate(idx):
+                    if trainable[16 * l + i]:
+                        pieces.append((16 * l + i, flat[o + j * n: o + (j + 1) * n].view(shape)))
+                o += n * len(idx)
+    return grads, flat, pieces
 
 
 def _stamp(descs, L, meta, mbias):
@@ -402,6 +438,13 @@ class EncoderPlan:
 
     def __init__(self):
         self.key = None
+        self.parts = {}
+
+    def part(self, first):
+        """The plan of the call over layers first.. of a split encoder (bert_encoder): each part keeps its own descriptors."""
+        if first not in self.parts:
+            self.parts[first] = EncoderPlan()
+        return self.parts[first]
 
     def prepare(self, caches, params, B, S, H, A, I, mbias, meta, dev, varlen=None):
         """-> (descs, weights, arena stride per layer, buffer offsets). varlen (unpadded calls): dict(cu_seqlens, max_seq,
@@ -498,24 +541,32 @@ class _EncoderFn(torch.autograd.Function):
         if douts[L - 1] is None:   # nothing downstream depends on the encoder output
             return (None,) * (3 + 16 * L)
         dy = douts[L - 1].to(_BF16).contiguous()
-        grads, flat = _layer_grads(ctx.params, L, H, I, dev)
+        # the flags autograd recorded at the forward: a frozen parameter gets NULL pointers, and without an input gradient
+        # (dx NULL) the lowest layer's input-gradient GEMM is not launched
+        trainable = ctx.needs_input_grad[3:]
+        plan = encoder_grad_plan(ctx.params, trainable, True)[1]
+        grads, flat, pieces = _layer_grads(ctx.params, trainable, plan, H, I, dev)
         with torch.cuda.device(dev), deterministic(dev, M, H, I), dropout_offset(meta.get("seed_offset")):
             w = _bwd_scratch(dev, M, H, I, A, meta["hidden_dropout"] > 0)
             sc = _lib.LayerScratch(**{k: _ptr(t) for k, t in w.items()})
-            dx = torch.empty(oshape, device=dev, dtype=_BF16)
+            dx = torch.empty(oshape, device=dev, dtype=_BF16) if ctx.needs_input_grad[0] else None
             _stamp(descs, L, meta, mbias)   # a later forward with the same plan key has stamped its own step since
             if vl is None:
                 _lib.check(_lib.lib().vb_encoder_bwd(descs, L, ctypes.c_void_p(x.data_ptr()), ctypes.c_void_p(ctx.arena.data_ptr()),
-                                                     ctypes.c_void_p(dy.data_ptr()), ctypes.c_void_p(dx.data_ptr()), grads,
+                                                     ctypes.c_void_p(dy.data_ptr()), ctypes.c_void_p(_ptr(dx)), grads,
                                                      ctypes.byref(sc), _stream()), "vb_encoder_bwd")
             else:
                 _lib.check(_lib.lib().vb_encoder_bwd_varlen(descs, L, vl["cu_seqlens"].data_ptr(), M, x.data_ptr(),
-                                                            ctx.arena.data_ptr(), dy.data_ptr(), dx.data_ptr(), grads, ctypes.byref(sc),
+                                                            ctx.arena.data_ptr(), dy.data_ptr(), _ptr(dx), grads, ctypes.byref(sc),
                                                             _stream()), "vb_encoder_bwd_varlen")
         ctx.arena = None
-        if flat is None:
-            return (dx, None, None) + (None,) * (16 * L)
-        return (dx, None, None) + _autograd_grads(flat, L, H, I)
+        out = [None] * (16 * L)
+        for i, g in pieces:
+            if plan[i // 16][0]:
+                ctx.params[i].grad.add_(g)   # the trainable part of a packed output computed into a buffer
+            else:
+                out[i] = g
+        return (dx, None, None) + tuple(out)
 
 
 def _encoder_infer(x, mbias, meta, params):
@@ -564,11 +615,26 @@ def bert_encoder(x, mbias, meta, params):
     layer's — followed, with attn_maps, by the L detached fp32 [B, A, S, S] attention maps.
 
     When no graph can be recorded (grad mode off, or neither x nor any parameter requires grad) the call takes the
-    forward-only route (_encoder_infer); every other call keeps its activations in the arena of _EncoderFn."""
+    forward-only route (_encoder_infer); every other call keeps its activations in the arena of _EncoderFn. When x needs no
+    gradient, the layers below the lowest one with a trainable parameter (l0) take the forward-only route too and get no arena
+    slot: no backward reaches them. Their descriptors keep their layer indices, so outputs and dropout bits are those of one
+    call over every layer."""
     if not (torch.is_grad_enabled() and (x.requires_grad or any(p.requires_grad for p in params))):
         return _encoder_infer(x, mbias, meta, params)
-    outs = _EncoderFn.apply(x, mbias, meta, *params)
-    return outs if meta.get("all_layers", True) else outs[len(params) // 16 - 1:]
+    L = len(params) // 16
+    all_layers = meta.get("all_layers", True)
+    l0 = 0 if x.requires_grad else next(l for l in range(L) if any(p.requires_grad for p in params[16 * l: 16 * l + 16]))
+    if l0 == 0:
+        outs = _EncoderFn.apply(x, mbias, meta, *params)
+        return outs if all_layers else outs[L - 1:]
+    plan = meta["plan"]
+    low = _encoder_infer(x, mbias, dict(meta, caches=meta["caches"][:l0], plan=plan.part(0)), params[:16 * l0])
+    n_low = l0 if all_layers else 1
+    high = _EncoderFn.apply(low[n_low - 1], mbias, dict(meta, caches=meta["caches"][l0:], plan=plan.part(l0),
+                                                          layer_index0=meta["layer_index0"] + l0, all_layers=True),
+                            *params[16 * l0:])
+    outs = low[:n_low] + high[:L - l0] if all_layers else high[L - l0 - 1:L - l0]
+    return outs + low[n_low:] + high[L - l0:]
 
 
 def unpad_plan(valid):
@@ -656,19 +722,19 @@ class _EmbedFn(torch.autograd.Function):
         M = B * (T + V)
         dy = dy.to(_BF16).contiguous()
         f32 = torch.float32
-        direct = _grad_targets(ctx.params) if V > 0 else None
+        # a frozen table gets a NULL pointer (vb_embed_grads): no scatter, GEMM or reduction writes it
+        trainable = ctx.needs_input_grad[5:14]
+        direct = _grad_targets(ctx.params, trainable=trainable) if V > 0 else None
         if direct is not None:
             dword, dpos, dtyp, dtyp_vis, dpos_vis, dpw, dpb, dgamma, dbeta = direct
         else:
-            dword = torch.zeros_like(word, dtype=f32)
-            dpos = torch.zeros_like(pos, dtype=f32)
-            dtyp = torch.zeros_like(typ, dtype=f32)
-            dtyp_vis = torch.zeros_like(typ_vis, dtype=f32)
-            dpos_vis = torch.zeros_like(pos_vis, dtype=f32)
-            dgamma = torch.zeros_like(gamma, dtype=f32)
-            dbeta = torch.zeros_like(beta, dtype=f32)
-            dpw = torch.zeros(H, Dv, device=dev, dtype=f32) if V > 0 else None
-            dpb = torch.zeros(H, device=dev, dtype=f32) if V > 0 else None
+            zeros = lambda t, shape, live: torch.zeros(shape, device=dev, dtype=f32) if live else None
+            dword, dpos, dtyp, dtyp_vis, dpos_vis, dgamma, dbeta = (
+                zeros(t, t.shape, live) for t, live in zip((word, pos, typ, typ_vis, pos_vis, gamma, beta),
+                                                           (trainable[0], trainable[1], trainable[2], trainable[3], trainable[4],
+                                                            trainable[7], trainable[8])))
+            dpw = zeros(None, (H, Dv), V > 0 and trainable[5])
+            dpb = zeros(None, (H,), V > 0 and trainable[6])
         with _unfilled():
             d_pre = torch.empty(M, H, device=dev, dtype=_BF16)
             if V > 0:
@@ -678,9 +744,9 @@ class _EmbedFn(torch.autograd.Function):
                 d_vis = d_feats = None
         a = _lib.EmbedActs(vis_proj=0, pre=pre.data_ptr(), mean=mean.data_ptr(), rstd=rstd.data_ptr())
         g = _lib.EmbedGrads(
-            dword=dword.data_ptr(), dpos=dpos.data_ptr(), dtype=dtyp.data_ptr(), dpos_vis=dpos_vis.data_ptr(),
-            dtype_vis=dtyp_vis.data_ptr(), dw_proj=_ptr(dpw), db_proj=_ptr(dpb), dgamma=dgamma.data_ptr(),
-            dbeta=dbeta.data_ptr(), d_pre=d_pre.data_ptr(), d_vis=_ptr(d_vis), d_feats=_ptr(d_feats))
+            dword=_ptr(dword), dpos=_ptr(dpos), dtype=_ptr(dtyp), dpos_vis=_ptr(dpos_vis), dtype_vis=_ptr(dtyp_vis),
+            dw_proj=_ptr(dpw), db_proj=_ptr(dpb), dgamma=_ptr(dgamma), dbeta=_ptr(dbeta), d_pre=d_pre.data_ptr(),
+            d_vis=_ptr(d_vis), d_feats=_ptr(d_feats))
         with torch.cuda.device(dev), deterministic(dev, M, H, Dv), dropout_offset(ctx.seed_offset):
             _lib.check(_lib.lib().vb_embed_bwd(ctypes.byref(ctx.desc), ctypes.byref(a), ctypes.c_void_p(dy.data_ptr()),
                                                ctypes.byref(g), _stream()), "vb_embed_bwd")
@@ -743,23 +809,27 @@ class _MlmDecoderFn(torch.autograd.Function):
         with _unfilled():
             dt = torch.empty(n, H, device=t.device, dtype=_BF16)
         _gemm(t.device, A=dlogits.data_ptr(), lda=Vp, B=table.data_ptr(), ldb=H, b_mn_major=1, M=n, N=H, K=Vp, D=dt.data_ptr(), ldd=H)
-        direct = _grad_targets((E, bias))
+        # a frozen table skips the [V, H] weight-gradient GEMM, a frozen bias its column sum
+        need_E, need_b = ctx.needs_input_grad[1], ctx.needs_input_grad[2]
+        direct = _grad_targets((E, bias), trainable=(need_E, need_b))
         if direct is not None:
             dE, db = direct
-            db_pad = torch.zeros(Vp, device=t.device, dtype=torch.float32)
         else:
-            dE = torch.zeros(V, H, device=t.device, dtype=torch.float32)
-            db_pad = torch.zeros(Vp, device=t.device, dtype=torch.float32)
+            dE = torch.zeros(V, H, device=t.device, dtype=torch.float32) if need_E else None
+        db_pad = torch.zeros(Vp, device=t.device, dtype=torch.float32) if need_b else None
         with deterministic(t.device, n, H, 0, V):
-            _gemm(t.device, A=dlogits.data_ptr(), lda=Vp, a_mn_major=1, B=t.data_ptr(), ldb=H, b_mn_major=1, M=V, N=H, K=n,
-                  D=dE.data_ptr(), ldd=H, d_fp32=1, splits=1)
-            with torch.cuda.device(t.device):
-                _lib.check(_lib.lib().vb_colsum_bf16(ctypes.c_void_p(dlogits.data_ptr()), ctypes.c_int64(Vp),
-                                                     ctypes.c_void_p(db_pad.data_ptr()), n, Vp, _stream()), "vb_colsum_bf16")
+            if need_E:
+                _gemm(t.device, A=dlogits.data_ptr(), lda=Vp, a_mn_major=1, B=t.data_ptr(), ldb=H, b_mn_major=1, M=V, N=H, K=n,
+                      D=dE.data_ptr(), ldd=H, d_fp32=1, splits=1)
+            if need_b:
+                with torch.cuda.device(t.device):
+                    _lib.check(_lib.lib().vb_colsum_bf16(ctypes.c_void_p(dlogits.data_ptr()), ctypes.c_int64(Vp),
+                                                         ctypes.c_void_p(db_pad.data_ptr()), n, Vp, _stream()), "vb_colsum_bf16")
         if direct is not None:
-            db.add_(db_pad[:V])
+            if need_b:
+                db.add_(db_pad[:V])
             return dt, None, None, None, None
-        return dt, dE, db_pad[:V].clone(), None, None
+        return dt, dE, None if db_pad is None else db_pad[:V].clone(), None, None
 
 
 def mlm_decoder(t, E, bias, cache, train=False):
