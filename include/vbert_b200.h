@@ -328,6 +328,33 @@ int vb_encoder_bwd_varlen(const vb_layer_desc* descs, int32_t n_layers, const in
  * y_all NULL or bf16 [n_layers, total, hidden]. There are no attention maps of a variable-length call. */
 int vb_encoder_infer_varlen(const vb_layer_desc* descs, int32_t n_layers, const int32_t* cu_seqlens, int32_t total,
                             const void* x_in, void* workspace, void* y_last, void* y_all, void* stream);
+/* Activation checkpointing: a training forward and backward over ONE arena slot (`slot`: vb_encoder_arena_layout bytes, or
+ * vb_encoder_arena_layout_varlen bytes for the _varlen calls) plus n_layers - 1 checkpoint regions (`ckpt`), instead of an arena
+ * of n_layers slots. Region l holds layer l's output y (bf16 [M, hidden]) and its LayerNorm-2 mean and rstd (fp32 [M]).
+ * vb_encoder_ckpt_layout: bytes per region (a multiple of 256); offsets (NULL or [3]) receives the byte offsets of y, mean2,
+ * rstd2 (256-byte aligned); packed_rows < 0: dense (M = batch * seq), else the row count of a variable-length call. -1 on a bad
+ * shape.
+ * vb_encoder_fwd_ckpt: layers 0 .. n-2 run as in vb_encoder_infer, through the slot, and write their output and LN2 statistics
+ * into their region; the top layer runs the vb_encoder_fwd forward into the slot, its output in slot buffer 13 (y), reading its
+ * input from region n-2. probs: NULL, or the attention maps of vb_encoder_infer (dense only), written per layer from the qkv it
+ * just produced.
+ * vb_encoder_bwd_ckpt: the backward of vb_encoder_bwd with the same arguments' meaning. The top layer's backward reads the slot;
+ * each lower layer is recomputed into the slot up to its FFN-down GEMM (no LN2 forward: its output and statistics are in the
+ * region) with the launches and dropout streams of vb_encoder_fwd, then run backward. Every output and gradient bit equals the
+ * arena calls' in deterministic mode, and vb_set_dropout_offset applies as there. The slot and ckpt of the forward are handed to
+ * the backward unchanged; the backward writes the slot and leaves ckpt as it is. n_layers == 1: ckpt may be NULL and the calls
+ * are vb_encoder_fwd / vb_encoder_bwd. Every descriptor and gradient entry is checked before the first launch. */
+int64_t vb_encoder_ckpt_layout(int32_t batch, int32_t seq, int32_t hidden, int32_t heads, int32_t inter, int64_t packed_rows,
+                               int64_t* offsets /* [3] */);
+int vb_encoder_fwd_ckpt(const vb_layer_desc* descs, int32_t n_layers, const void* x_in, void* ckpt, void* slot, float* probs,
+                        void* stream);
+int vb_encoder_bwd_ckpt(const vb_layer_desc* descs, int32_t n_layers, const void* x_in, void* ckpt, void* slot, const void* dy,
+                        void* dx, const vb_layer_grads* grads, const vb_layer_scratch* scratch, void* stream);
+int vb_encoder_fwd_ckpt_varlen(const vb_layer_desc* descs, int32_t n_layers, const int32_t* cu_seqlens, int32_t total,
+                               const void* x_in, void* ckpt, void* slot, void* stream);
+int vb_encoder_bwd_ckpt_varlen(const vb_layer_desc* descs, int32_t n_layers, const int32_t* cu_seqlens, int32_t total,
+                               const void* x_in, void* ckpt, void* slot, const void* dy, void* dx, const vb_layer_grads* grads,
+                               const vb_layer_scratch* scratch, void* stream);
 
 /* ---- BertEmbeddingsWithVisualEmbedding (M.py:1169-1257) ----------------------------------- */
 typedef struct {

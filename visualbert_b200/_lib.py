@@ -88,9 +88,11 @@ EXPORTS = [
     "vb_encoder_infer_workspace", "vb_encoder_infer", "vb_encoder_infer_varlen",
     "vb_set_deterministic", "vb_deterministic_workspace_bytes", "vb_set_dropout_offset",
     "vb_bert_adam_step_sched", "vb_bert_adam_sched_check",
+    "vb_encoder_ckpt_layout", "vb_encoder_fwd_ckpt", "vb_encoder_bwd_ckpt", "vb_encoder_fwd_ckpt_varlen", "vb_encoder_bwd_ckpt_varlen",
 ]
 VB_ENCODER_ARENA_BUFFERS = 14
 ARENA_NAMES = ("qkv", "ctx", "lse", "pre1", "mean1", "rstd1", "x1", "u", "g", "pre2", "mean2", "rstd2", "keep_mask", "y")
+CKPT_NAMES = ("y", "mean2", "rstd2")   # the buffers of one checkpoint region (vb_encoder_ckpt_layout)
 
 
 class VBertLibraryError(RuntimeError):
@@ -134,6 +136,12 @@ def lib():
         _D = ctypes.c_double
         h.vb_bert_adam_step_sched.argtypes = [_P, _I, _I, _P, _I, _P, _P, _P, _D, _D, _D, _D, _P]
         h.vb_bert_adam_sched_check.argtypes = [_P, _I, _I, _P, _I]
+        h.vb_encoder_ckpt_layout.restype = ctypes.c_int64
+        h.vb_encoder_ckpt_layout.argtypes = [_I, _I, _I, _I, _I, c_i64, _P]
+        h.vb_encoder_fwd_ckpt.argtypes = [_P, _I, _P, _P, _P, _P, _P]
+        h.vb_encoder_bwd_ckpt.argtypes = [_P, _I, _P, _P, _P, _P, _P, _P, _P, _P]
+        h.vb_encoder_fwd_ckpt_varlen.argtypes = [_P, _I, _P, _I, _P, _P, _P, _P]
+        h.vb_encoder_bwd_ckpt_varlen.argtypes = [_P, _I, _P, _I, _P, _P, _P, _P, _P, _P, _P, _P]
         _lib = h
     return _lib
 

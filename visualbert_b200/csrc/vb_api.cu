@@ -72,11 +72,13 @@ static int check_layer(const vb_layer_desc* d, const LayerRows& r) {
 }
 
 // for_bwd = false (vb_encoder_infer): the same launches with the same arguments, but nothing only a backward reads is stored —
-// s->u is not touched (the FFN-up epilogue writes gelu(u) alone) and s->lse, s->mean1/2, s->rstd1/2 may be NULL
+// s->u is not touched (the FFN-up epilogue writes gelu(u) alone) and s->lse, s->mean1/2, s->rstd1/2 may be NULL.
+// ln2 = false (the recompute of vb_encoder_bwd_ckpt): stop after step 6; the LN2 output and statistics are already kept, and
+// x_out may be NULL.
 int layer_fwd(const vb_layer_desc* d, const void* x_in, void* x_out, const vb_layer_acts* s, cudaStream_t st,
-              const LayerRows& rows = kDenseRows, bool for_bwd = true) {
+              const LayerRows& rows = kDenseRows, bool for_bwd = true, bool ln2 = true) {
     VB_TRY(check_layer(d, rows));
-    VB_REQUIRE(x_in && x_out && s, "layer_fwd: null pointer");
+    VB_REQUIRE(x_in && (x_out || !ln2) && s, "layer_fwd: null pointer");
     const bool vl = rows.cu_seqlens != nullptr;
     const int M = vl ? rows.total : d->batch * d->seq, H = d->hidden, I = d->inter;
     vb_gemm_args a = fwd_args(x_in, d->w_qkv, s->qkv, M, 3 * H, H);
@@ -106,7 +108,7 @@ int layer_fwd(const vb_layer_desc* d, const void* x_in, void* x_out, const vb_la
     a.bias = d->b_out; a.addend = s->x1; a.ld_add = H;
     a.dropout_p = d->hidden_dropout; a.dropout_seed = d->seed; a.dropout_stream = drop_stream(d->layer_index, kSiteFfnOut);
     VB_TRY(gemm(a, st));
-    VB_TRY(ln_fwd(s->pre2, H, d->ln2_gamma, d->ln2_beta, x_out, H, s->mean2, s->rstd2, M, H, kLnEps, st));
+    if (ln2) VB_TRY(ln_fwd(s->pre2, H, d->ln2_gamma, d->ln2_beta, x_out, H, s->mean2, s->rstd2, M, H, kLnEps, st));
     return 0;
 }
 
@@ -332,6 +334,111 @@ int encoder_attention_probs(const vb_layer_desc* descs, int n, void* arena, floa
     return 0;
 }
 
+// ---- activation checkpointing: one arena slot for the whole stack, plus each lower layer's output and LN2 statistics ----
+enum { kCkY, kCkMean2, kCkRstd2, kCkBuffers };
+
+long long ckpt_layout(long long M, int H, long long* off) {
+    const long long sizes[kCkBuffers] = {M * H * 2, M * 4, M * 4};
+    long long o = 0;
+    for (int i = 0; i < kCkBuffers; ++i) {
+        if (off) off[i] = o;
+        o += align256(sizes[i]);
+    }
+    return o;
+}
+
+// every descriptor and gradient entry of a checkpointed call, before its first launch: a refused call launches nothing
+static int check_ckpt_call(const vb_layer_desc* descs, int n, const void* ckpt, const LayerRows& rows, const char* what) {
+    VB_REQUIRE(descs && n > 0, "%s: null descriptors / no layers", what);
+    VB_REQUIRE(n == 1 || ckpt != nullptr, "%s: ckpt is NULL with %d layers", what, n);
+    const vb_layer_desc& d0 = descs[0];
+    for (int l = 0; l < n; ++l) {
+        VB_TRY(check_layer(&descs[l], rows));
+        VB_REQUIRE(descs[l].batch == d0.batch && descs[l].seq == d0.seq && descs[l].hidden == d0.hidden && descs[l].heads == d0.heads &&
+                   descs[l].inter == d0.inter && (descs[l].attn_dropout > 0.f) == (d0.attn_dropout > 0.f),
+                   "%s: layers differ in shape", what);
+    }
+    return 0;
+}
+
+// the slot's activations with LN2's statistics taken from checkpoint l, and the checkpointed output y of layer l
+static void ckpt_acts(const vb_layer_desc* d, void* ckpt, void* slot, int l, vb_layer_acts* a, void** y, const LayerRows& rows) {
+    void* slot_y;
+    arena_acts(d, slot, 0, a, &slot_y, rows);
+    long long off[kCkBuffers];
+    const long long M = rows.cu_seqlens != nullptr ? rows.total : static_cast<long long>(d->batch) * d->seq;
+    char* base = static_cast<char*>(ckpt) + l * ckpt_layout(M, d->hidden, off);
+    a->mean2 = reinterpret_cast<float*>(base + off[kCkMean2]);
+    a->rstd2 = reinterpret_cast<float*>(base + off[kCkRstd2]);
+    *y = base + off[kCkY];
+}
+
+// Layers 0 .. n-2 run forward-only through the slot and keep their output and LN2 mean / rstd in their checkpoint region; the top
+// layer runs the arena forward into the slot, so the backward finds its activations in place.
+int encoder_fwd_ckpt(const vb_layer_desc* descs, int n, const void* x_in, void* ckpt, void* slot, float* probs, cudaStream_t st,
+                     const LayerRows& rows = kDenseRows) {
+    VB_TRY(check_ckpt_call(descs, n, ckpt, rows, "encoder_fwd_ckpt"));
+    VB_REQUIRE(x_in && slot, "encoder_fwd_ckpt: null x_in / slot");
+    const vb_layer_desc& d0 = descs[0];
+    const long long per_layer = static_cast<long long>(d0.batch) * d0.heads * d0.seq * d0.seq;
+    const void* x = x_in;
+    for (int l = 0; l < n; ++l) {
+        vb_layer_acts a;
+        void* y;
+        if (l < n - 1) {
+            ckpt_acts(&descs[l], ckpt, slot, l, &a, &y, rows);
+            VB_TRY(layer_fwd(&descs[l], x, y, &a, st, rows, false));
+        } else {
+            arena_acts(&descs[l], slot, 0, &a, &y, rows);
+            VB_TRY(layer_fwd(&descs[l], x, y, &a, st, rows));
+        }
+        if (probs)
+            VB_TRY(attn_probs(a.qkv, descs[l].mask_bias, probs + l * per_layer, d0.batch, d0.seq, d0.heads, d0.hidden, st));
+        x = y;
+    }
+    return 0;
+}
+
+// The top layer's backward runs on the slot as vb_encoder_fwd_ckpt left it. Each lower layer l is then recomputed into the slot
+// up to its FFN-down GEMM (steps 1-6 of layer_fwd with the training epilogues, from checkpoint l-1 or x_in) and run backward with
+// the checkpointed LN2 statistics: its launches, arguments and dropout streams are those of vb_encoder_fwd, so the slot holds what
+// the arena slot of layer l held. The gradient between layers travels as in encoder_bwd, in `dx` or scratch.d_x1; the recompute
+// writes only the slot, so that carry crosses it unchanged.
+int encoder_bwd_ckpt(const vb_layer_desc* descs, int n, const void* x_in, void* ckpt, void* slot, const void* dy, void* dx,
+                     const vb_layer_grads* grads, const vb_layer_scratch* w, cudaStream_t st, const LayerRows& rows = kDenseRows) {
+    VB_TRY(check_ckpt_call(descs, n, ckpt, rows, "encoder_bwd_ckpt"));
+    VB_REQUIRE(x_in && slot && dy && grads && w, "encoder_bwd_ckpt: null pointer");
+    const vb_layer_desc& d0 = descs[0];
+    const int M = rows.cu_seqlens != nullptr ? rows.total : d0.batch * d0.seq;
+    VB_TRY(det_require(layer_bwd_det_bytes(M, d0.hidden, d0.inter), "layer backward"));
+    for (int l = 0; l < n; ++l) {
+        VB_TRY(check_grads(&grads[l]));
+        VB_REQUIRE(descs[l].hidden_dropout <= 0.f || w->d_pre_drop, "encoder_bwd_ckpt: d_pre_drop scratch required when hidden_dropout > 0");
+    }
+    void* const carry = dx != nullptr ? dx : w->d_x1;
+    const void* g_in = dy;
+    for (int l = n - 1; l >= 0; --l) {
+        vb_layer_acts a;
+        void* y;
+        const void* xl = x_in;
+        if (l > 0) {
+            vb_layer_acts ap;
+            void* yp;
+            ckpt_acts(&descs[l - 1], ckpt, slot, l - 1, &ap, &yp, rows);
+            xl = yp;
+        }
+        if (l == n - 1) {
+            arena_acts(&descs[l], slot, 0, &a, &y, rows);
+        } else {
+            ckpt_acts(&descs[l], ckpt, slot, l, &a, &y, rows);
+            VB_TRY(layer_fwd(&descs[l], xl, nullptr, &a, st, rows, true, false));
+        }
+        VB_TRY(layer_bwd(&descs[l], xl, &a, g_in, l > 0 ? carry : dx, &grads[l], w, st, rows));
+        g_in = carry;
+    }
+    return 0;
+}
+
 static int check_embed(const vb_embed_desc* d) {
     VB_REQUIRE(d != nullptr, "embed: null descriptor");
     VB_REQUIRE(d->batch > 0 && d->text_len > 0 && d->num_regions >= 0, "embed: bad shape");
@@ -533,6 +640,41 @@ int vb_encoder_bwd_varlen(const vb_layer_desc* descs, int32_t n_layers, const in
     if (total <= 0) { vb::set_error("vb_encoder_bwd_varlen: total (%d) must be > 0", total); return 2; }
     const vb::LayerRows rows = {cu_seqlens, total};
     return vb::encoder_bwd(descs, n_layers, x_in, arena, dy, dx, grads, scratch, static_cast<cudaStream_t>(stream), rows);
+}
+int64_t vb_encoder_ckpt_layout(int32_t batch, int32_t seq, int32_t hidden, int32_t heads, int32_t inter, int64_t packed_rows,
+                               int64_t* offsets) {
+    if (batch <= 0 || seq <= 0 || hidden <= 0 || heads <= 0 || inter <= 0 || packed_rows == 0 || packed_rows >= (1LL << 31)) {
+        vb::set_error("vb_encoder_ckpt_layout: bad shape (batch %d, seq %d, hidden %d, heads %d, inter %d, packed_rows %lld)", batch,
+                      seq, hidden, heads, inter, static_cast<long long>(packed_rows));
+        return -1;
+    }
+    long long off[vb::kCkBuffers];
+    const long long stride = vb::ckpt_layout(packed_rows >= 0 ? packed_rows : static_cast<long long>(batch) * seq, hidden, off);
+    if (offsets) for (int i = 0; i < vb::kCkBuffers; ++i) offsets[i] = off[i];
+    return stride;
+}
+int vb_encoder_fwd_ckpt(const vb_layer_desc* descs, int32_t n_layers, const void* x_in, void* ckpt, void* slot, float* probs,
+                        void* stream) {
+    return vb::encoder_fwd_ckpt(descs, n_layers, x_in, ckpt, slot, probs, static_cast<cudaStream_t>(stream));
+}
+int vb_encoder_bwd_ckpt(const vb_layer_desc* descs, int32_t n_layers, const void* x_in, void* ckpt, void* slot, const void* dy,
+                        void* dx, const vb_layer_grads* grads, const vb_layer_scratch* scratch, void* stream) {
+    return vb::encoder_bwd_ckpt(descs, n_layers, x_in, ckpt, slot, dy, dx, grads, scratch, static_cast<cudaStream_t>(stream));
+}
+int vb_encoder_fwd_ckpt_varlen(const vb_layer_desc* descs, int32_t n_layers, const int32_t* cu_seqlens, int32_t total,
+                               const void* x_in, void* ckpt, void* slot, void* stream) {
+    if (cu_seqlens == nullptr) { vb::set_error("vb_encoder_fwd_ckpt_varlen: cu_seqlens is NULL"); return 2; }
+    if (total <= 0) { vb::set_error("vb_encoder_fwd_ckpt_varlen: total (%d) must be > 0", total); return 2; }
+    const vb::LayerRows rows = {cu_seqlens, total};
+    return vb::encoder_fwd_ckpt(descs, n_layers, x_in, ckpt, slot, nullptr, static_cast<cudaStream_t>(stream), rows);
+}
+int vb_encoder_bwd_ckpt_varlen(const vb_layer_desc* descs, int32_t n_layers, const int32_t* cu_seqlens, int32_t total,
+                               const void* x_in, void* ckpt, void* slot, const void* dy, void* dx, const vb_layer_grads* grads,
+                               const vb_layer_scratch* scratch, void* stream) {
+    if (cu_seqlens == nullptr) { vb::set_error("vb_encoder_bwd_ckpt_varlen: cu_seqlens is NULL"); return 2; }
+    if (total <= 0) { vb::set_error("vb_encoder_bwd_ckpt_varlen: total (%d) must be > 0", total); return 2; }
+    const vb::LayerRows rows = {cu_seqlens, total};
+    return vb::encoder_bwd_ckpt(descs, n_layers, x_in, ckpt, slot, dy, dx, grads, scratch, static_cast<cudaStream_t>(stream), rows);
 }
 int vb_embed_fwd(const vb_embed_desc* d, void* y, const vb_embed_acts* acts, void* stream) {
     return vb::embed_fwd_api(d, y, acts, static_cast<cudaStream_t>(stream));

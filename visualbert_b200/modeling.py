@@ -157,7 +157,8 @@ def _encoder_meta(owner, layers, seed, **more):
     return dict(heads=l0.attention.self.num_attention_heads, layer_index0=l0.layer_index,
                 hidden_dropout=l0.hidden_dropout_prob if train else 0.0,
                 attn_dropout=l0.attention_probs_dropout_prob if train else 0.0, seed=int(seed), train=train,
-                caches=[l._weights for l in layers], plan=plan, seed_offset=ops.current_seed_offset() if train else None, **more)
+                caches=[l._weights for l in layers], plan=plan, seed_offset=ops.current_seed_offset() if train else None,
+                checkpoint=bool(owner.__dict__.get("activation_checkpointing", False)), **more)
 
 
 class BertLayer(nn.Module):
@@ -206,6 +207,7 @@ class BertEncoder(nn.Module):
         super().__init__()
         self.layer = nn.ModuleList([BertLayer(config, i) for i in range(config.num_hidden_layers)])
         self.output_attention_weights = getattr(config, "output_attention_weights", False)
+        self.activation_checkpointing = False   # BertVisualModel.set_activation_checkpointing
 
     def forward(self, hidden_states, attention_mask, output_all_encoded_layers=True, seed=0, varlen=None,
                 output_attention_weights=None):
@@ -531,6 +533,21 @@ class BertVisualModel(PreTrainedBertModel):
             del self._vb_step
             self._seed_offset = None
         self._capturable = flag
+        return self
+
+    def set_activation_checkpointing(self, flag=True):
+        """Opt-in activation checkpointing of the encoder, off by default.
+
+        When on, a training forward of the whole-encoder call keeps ONE layer's activations (an arena slot) plus each lower
+        layer's output and LayerNorm-2 statistics, instead of every layer's activations; the backward call recomputes each lower
+        layer into the slot before running its backward (vb_encoder_fwd_ckpt / vb_encoder_bwd_ckpt). The recompute draws the
+        same dropout masks, so the loss, the outputs and, in deterministic mode, every gradient are bit for bit those of the
+        default path; a step costs about one more forward of the lower layers. Read at every forward; works with set_unpadded,
+        set_graph_capturable (GraphedStep captures a new graph when the flag changes), deterministic mode, frozen parameters,
+        output_attention_weights and bypass_transformer (its text encoder call). The padded per-layer route
+        (output_all_encoded_layers=True in training mode under grad) keeps one single-layer arena per layer, as without the
+        flag."""
+        self.encoder.activation_checkpointing = bool(flag)
         return self
 
     def set_unpadded(self, flag=True):

@@ -486,7 +486,12 @@ class _EncoderFn(torch.autograd.Function):
     (vb_encoder_fwd_varlen / vb_encoder_bwd_varlen).
 
     With meta["attn_maps"] (dense calls only) the L layer outputs are followed by the L attention maps, fp32 [B, A, S, S] views
-    of one [L, B, A, S, S] tensor written by vb_encoder_attention_probs right after the forward; they are not differentiable."""
+    of one [L, B, A, S, S] tensor written by vb_encoder_attention_probs right after the forward; they are not differentiable.
+
+    With meta["checkpoint"] (activation checkpointing) the call keeps one arena slot and L - 1 checkpoint regions (each lower
+    layer's output and LayerNorm-2 statistics) instead of L slots: vb_encoder_fwd_ckpt / vb_encoder_bwd_ckpt (and their _varlen
+    forms) recompute each lower layer inside the backward call. Outputs l < L - 1 are views of the checkpoint buffer, the last one
+    a view of the slot; the attention maps come from the forward call itself. Same bits as the arena call."""
 
     @staticmethod
     def _shape(x, meta):
@@ -507,6 +512,14 @@ class _EncoderFn(torch.autograd.Function):
         x = x.contiguous()
         with torch.cuda.device(x.device), deterministic(x.device, M, H, I), dropout_offset(meta.get("seed_offset")):
             descs, weights, stride, off = meta["plan"].prepare(meta["caches"], params, B, S, H, A, I, mbias, meta, x.device, vl)
+            if meta.get("checkpoint"):
+                outs, maps, arena, ckpt = _EncoderFn._forward_ckpt(x, descs, B, S, H, A, I, L, M, oshape, vl, stride, off, meta)
+                ctx.meta, ctx.descs, ctx.arena, ctx.ckpt, ctx.params, ctx.weights = meta, descs, arena, ckpt, params, weights
+                ctx.shape = (B, S, H, A, I, L, M, oshape)
+                ctx.save_for_backward(x, mbias)
+                ctx.mark_non_differentiable(*outs[:-1], *maps)
+                ctx.set_materialize_grads(False)
+                return outs + maps
             arena = torch.empty(L * stride, device=x.device, dtype=torch.uint8)
             if vl is None:
                 _lib.check(_lib.lib().vb_encoder_fwd(descs, L, ctypes.c_void_p(x.data_ptr()), ctypes.c_void_p(arena.data_ptr()),
@@ -524,12 +537,37 @@ class _EncoderFn(torch.autograd.Function):
                 maps = tuple(probs.unbind(0))
         n = M * H * 2
         outs = tuple(arena[l * stride + off[13]: l * stride + off[13] + n].view(_BF16).view(oshape) for l in range(L))
-        ctx.meta, ctx.descs, ctx.arena, ctx.params, ctx.weights = meta, descs, arena, params, weights
+        ctx.meta, ctx.descs, ctx.arena, ctx.ckpt, ctx.params, ctx.weights = meta, descs, arena, None, params, weights
         ctx.shape = (B, S, H, A, I, L, M, oshape)
         ctx.save_for_backward(x, mbias)
         ctx.mark_non_differentiable(*outs[:-1], *maps)
         ctx.set_materialize_grads(False)   # or autograd hands backward a 64 MB zero tensor for each of the L - 1 unused outputs
         return outs + maps
+
+    @staticmethod
+    def _forward_ckpt(x, descs, B, S, H, A, I, L, M, oshape, vl, stride, off, meta):
+        """vb_encoder_fwd_ckpt(_varlen) -> (outputs, maps, slot, ckpt); ckpt is None for one layer."""
+        coff = (ctypes.c_int64 * len(_lib.CKPT_NAMES))()
+        cs = int(_lib.lib().vb_encoder_ckpt_layout(B, S, H, A, I, -1 if vl is None else M, coff))
+        if cs < 0:
+            _lib.check(1, "vb_encoder_ckpt_layout")
+        slot = torch.empty(stride, device=x.device, dtype=torch.uint8)
+        ckpt = torch.empty((L - 1) * cs, device=x.device, dtype=torch.uint8) if L > 1 else None
+        probs = None
+        if meta.get("attn_maps"):
+            if vl is not None:
+                raise ValueError("bert_encoder: attention maps need a dense (padded) call")
+            probs = torch.empty(L, B, A, S, S, device=x.device, dtype=torch.float32)
+        if vl is None:
+            _lib.check(_lib.lib().vb_encoder_fwd_ckpt(descs, L, x.data_ptr(), _ptr(ckpt), slot.data_ptr(), _ptr(probs), _stream()),
+                       "vb_encoder_fwd_ckpt")
+        else:
+            _lib.check(_lib.lib().vb_encoder_fwd_ckpt_varlen(descs, L, vl["cu_seqlens"].data_ptr(), M, x.data_ptr(), _ptr(ckpt),
+                                                             slot.data_ptr(), _stream()), "vb_encoder_fwd_ckpt_varlen")
+        n = M * H * 2
+        outs = tuple(ckpt[l * cs + coff[0]: l * cs + coff[0] + n].view(_BF16).view(oshape) for l in range(L - 1))
+        outs += (slot[off[13]: off[13] + n].view(_BF16).view(oshape),)
+        return outs, (() if probs is None else tuple(probs.unbind(0))), slot, ckpt
 
     @staticmethod
     def backward(ctx, *douts):
@@ -551,7 +589,14 @@ class _EncoderFn(torch.autograd.Function):
             sc = _lib.LayerScratch(**{k: _ptr(t) for k, t in w.items()})
             dx = torch.empty(oshape, device=dev, dtype=_BF16) if ctx.needs_input_grad[0] else None
             _stamp(descs, L, meta, mbias)   # a later forward with the same plan key has stamped its own step since
-            if vl is None:
+            if meta.get("checkpoint") and vl is None:
+                _lib.check(_lib.lib().vb_encoder_bwd_ckpt(descs, L, x.data_ptr(), _ptr(ctx.ckpt), ctx.arena.data_ptr(), dy.data_ptr(),
+                                                          _ptr(dx), grads, ctypes.byref(sc), _stream()), "vb_encoder_bwd_ckpt")
+            elif meta.get("checkpoint"):
+                _lib.check(_lib.lib().vb_encoder_bwd_ckpt_varlen(descs, L, vl["cu_seqlens"].data_ptr(), M, x.data_ptr(), _ptr(ctx.ckpt),
+                                                                 ctx.arena.data_ptr(), dy.data_ptr(), _ptr(dx), grads, ctypes.byref(sc),
+                                                                 _stream()), "vb_encoder_bwd_ckpt_varlen")
+            elif vl is None:
                 _lib.check(_lib.lib().vb_encoder_bwd(descs, L, ctypes.c_void_p(x.data_ptr()), ctypes.c_void_p(ctx.arena.data_ptr()),
                                                      ctypes.c_void_p(dy.data_ptr()), ctypes.c_void_p(_ptr(dx)), grads,
                                                      ctypes.byref(sc), _stream()), "vb_encoder_bwd")
@@ -559,7 +604,7 @@ class _EncoderFn(torch.autograd.Function):
                 _lib.check(_lib.lib().vb_encoder_bwd_varlen(descs, L, vl["cu_seqlens"].data_ptr(), M, x.data_ptr(),
                                                             ctx.arena.data_ptr(), dy.data_ptr(), _ptr(dx), grads, ctypes.byref(sc),
                                                             _stream()), "vb_encoder_bwd_varlen")
-        ctx.arena = None
+        ctx.arena = ctx.ckpt = None
         out = [None] * (16 * L)
         for i, g in pieces:
             if plan[i // 16][0]:
@@ -609,7 +654,8 @@ def _encoder_infer(x, mbias, meta, params):
 
 def bert_encoder(x, mbias, meta, params):
     """All layers at once. meta: dict(heads, layer_index0, hidden_dropout, attn_dropout, seed, train, caches=[LayerWeights],
-    plan=EncoderPlan, optional varlen=unpad_plan(...), optional attn_maps=True, optional all_layers=False); params: 16 tensors
+    plan=EncoderPlan, optional varlen=unpad_plan(...), optional attn_maps=True, optional all_layers=False, optional
+    checkpoint=True: activation checkpointing of the _EncoderFn part); params: 16 tensors
     per layer in bert_layer order. Returns the tuple of all layer outputs (only the last one is differentiable: a caller that
     needs gradients through intermediate outputs calls bert_layer once per layer) — with all_layers=False only the last
     layer's — followed, with attn_maps, by the L detached fp32 [B, A, S, S] attention maps.
