@@ -81,6 +81,16 @@ def gelu_prime64(u):
     return 0.5 * (1.0 + torch.erf(u / math.sqrt(2.0))) + u * torch.exp(-0.5 * u * u) / math.sqrt(2.0 * math.pi)
 
 
+def gp_tiled_ok(M, N):
+    """Restatement of vb_gemm.cu::gemm_gp_tiled_ok: the shapes whose gelu'(u) can be stored tile-native."""
+    return M >= 256 and M % 256 == 0 and N % 256 == 0
+
+
+def untile(t, M, N):
+    """tile-native gelu'(u) (vbert_b200.h, vb_gemm_args.gp_tiled) -> row-major [M, N]"""
+    return t.reshape(M // 256, N // 256, 2, 2, 4, 8, 32, 16).permute(0, 2, 4, 6, 1, 3, 5, 7).reshape(M, N)
+
+
 def tile_n(N):
     """vb_gemm's tile width: 256 unless N is small or padding N to a multiple of 256 wastes more than 1/8 of the columns."""
     pad = (N + 255) // 256 * 256 - N

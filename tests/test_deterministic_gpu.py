@@ -16,6 +16,7 @@ import ctypes
 import os
 import subprocess
 import sys
+import time
 
 import pytest
 import torch
@@ -52,12 +53,20 @@ def _sms():
     return torch.cuda.get_device_properties(0).multi_processor_count
 
 
+# torch.profiler can lose the kernel records nearest the edges of its capture window (the first kernel of a short window,
+# or the whole of one): each counted window starts after the device is idle and leaves host time at both ends
+PROFILE_PAD_S = 0.05
+
+
 def _kernels(fn):
     """The names of the CUDA kernels fn launches, in launch order (copies and memsets left out)."""
     from torch.profiler import ProfilerActivity, profile
+    torch.cuda.synchronize()
     with profile(activities=[ProfilerActivity.CUDA]) as prof:
+        time.sleep(PROFILE_PAD_S)
         fn()
         torch.cuda.synchronize()
+        time.sleep(PROFILE_PAD_S)
     out = []
     for e in prof.events():
         if e.device_type == torch.autograd.DeviceType.CUDA and "memset" not in e.name.lower() and "memcpy" not in e.name.lower():

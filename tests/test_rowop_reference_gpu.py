@@ -14,6 +14,7 @@ No call here passes a misaligned pointer or stride; those refusals are checked w
 import ctypes
 import json
 import re
+import time
 
 import numpy as np
 import pytest
@@ -96,6 +97,11 @@ def _vec(n, fill=None):
     return Guarded(1, n, F32, fill=fill)
 
 
+# torch.profiler can lose the kernel records nearest the edges of its capture window (the first kernel of a short window,
+# or the whole of one): each counted window starts after the device is idle and leaves host time at both ends
+PROFILE_PAD_S = 0.05
+
+
 class Launches:
     """Profiles a block of calls and checks, in launch order, every row kernel (KERNELS) against `expected`."""
 
@@ -108,12 +114,15 @@ class Launches:
 
     def __enter__(self):
         from torch.profiler import ProfilerActivity, profile
+        torch.cuda.synchronize()
         self.prof = profile(activities=[ProfilerActivity.CUDA])
         self.prof.__enter__()
+        time.sleep(PROFILE_PAD_S)
         return self
 
     def __exit__(self, *exc):
         torch.cuda.synchronize()
+        time.sleep(PROFILE_PAD_S)
         self.prof.__exit__(*exc)
         if exc[0] is not None:
             return False
