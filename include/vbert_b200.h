@@ -355,6 +355,35 @@ int vb_encoder_fwd_ckpt_varlen(const vb_layer_desc* descs, int32_t n_layers, con
 int vb_encoder_bwd_ckpt_varlen(const vb_layer_desc* descs, int32_t n_layers, const int32_t* cu_seqlens, int32_t total,
                                const void* x_in, void* ckpt, void* slot, const void* dy, void* dx, const vb_layer_grads* grads,
                                const vb_layer_scratch* scratch, void* stream);
+/* Selective recomputation of the FFN intermediates: the arena calls with every layer's gelu'(u) (buffer 7, u) and g = gelu(u)
+ * (buffer 8) moved out of the arena into ONE caller-owned buffer `ffn` that all layers share, instead of 2 * M * inter bf16 per
+ * slot. ffn holds gelu'(u) at byte 0, in the order vb_encoder_fwd keeps it (tile-native whenever vb_gemm_gp_tiled_ok(M, inter)),
+ * and g at byte ffn_bytes / 2.
+ * vb_encoder_arena_layout_ffnrc(_varlen): the arguments, offsets and slot stride of vb_encoder_arena_layout(_varlen), with u and g
+ * of size 0 in the slot (offsets[7] == offsets[8] == offsets[9]); *ffn_bytes (if not NULL) receives the size of ffn. -1 on a bad
+ * shape.
+ * vb_encoder_fwd_ffnrc: the launches and arguments of vb_encoder_fwd, except that each layer's FFN-up GEMM writes gelu'(u) and g
+ * into ffn and its FFN-down GEMM reads g from there; on return ffn holds the top layer's.
+ * vb_encoder_bwd_ffnrc: vb_encoder_bwd on that arena and the same ffn, as the forward left it. The top layer's backward reads ffn as
+ * it is; before the backward of each lower layer l the FFN-up GEMM of its forward (VB_EPI_GELU from slot l's x1, same weights,
+ * same tiling) rewrites ffn. That is n_layers - 1 extra GEMMs, and every output and gradient bit equals the arena calls' (in
+ * deterministic mode for the gradients). Every descriptor and gradient entry is checked before the first launch.
+ * vb_encoder_attention_probs reads only each slot's qkv (offset 0 in both layouts) and mask_bias: on an arena of these calls, give
+ * it one layer at a time (n_layers = 1, descs + l, arena + l * stride of vb_encoder_arena_layout_ffnrc). */
+int64_t vb_encoder_arena_layout_ffnrc(int32_t batch, int32_t seq, int32_t hidden, int32_t heads, int32_t inter,
+                                      int32_t attn_dropout_on, int64_t* offsets /* [VB_ENCODER_ARENA_BUFFERS] */,
+                                      int64_t* ffn_bytes);
+int64_t vb_encoder_arena_layout_ffnrc_varlen(int32_t batch, int32_t max_seq, int32_t total, int32_t hidden, int32_t heads,
+                                             int32_t inter, int32_t attn_dropout_on,
+                                             int64_t* offsets /* [VB_ENCODER_ARENA_BUFFERS] */, int64_t* ffn_bytes);
+int vb_encoder_fwd_ffnrc(const vb_layer_desc* descs, int32_t n_layers, const void* x_in, void* arena, void* ffn, void* stream);
+int vb_encoder_bwd_ffnrc(const vb_layer_desc* descs, int32_t n_layers, const void* x_in, void* arena, void* ffn, const void* dy,
+                         void* dx, const vb_layer_grads* grads, const vb_layer_scratch* scratch, void* stream);
+int vb_encoder_fwd_ffnrc_varlen(const vb_layer_desc* descs, int32_t n_layers, const int32_t* cu_seqlens, int32_t total,
+                                const void* x_in, void* arena, void* ffn, void* stream);
+int vb_encoder_bwd_ffnrc_varlen(const vb_layer_desc* descs, int32_t n_layers, const int32_t* cu_seqlens, int32_t total,
+                                const void* x_in, void* arena, void* ffn, const void* dy, void* dx, const vb_layer_grads* grads,
+                                const vb_layer_scratch* scratch, void* stream);
 
 /* ---- BertEmbeddingsWithVisualEmbedding (M.py:1169-1257) ----------------------------------- */
 typedef struct {

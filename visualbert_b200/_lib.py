@@ -89,6 +89,8 @@ EXPORTS = [
     "vb_set_deterministic", "vb_deterministic_workspace_bytes", "vb_set_dropout_offset",
     "vb_bert_adam_step_sched", "vb_bert_adam_sched_check",
     "vb_encoder_ckpt_layout", "vb_encoder_fwd_ckpt", "vb_encoder_bwd_ckpt", "vb_encoder_fwd_ckpt_varlen", "vb_encoder_bwd_ckpt_varlen",
+    "vb_encoder_arena_layout_ffnrc", "vb_encoder_arena_layout_ffnrc_varlen", "vb_encoder_fwd_ffnrc", "vb_encoder_bwd_ffnrc",
+    "vb_encoder_fwd_ffnrc_varlen", "vb_encoder_bwd_ffnrc_varlen",
 ]
 VB_ENCODER_ARENA_BUFFERS = 14
 ARENA_NAMES = ("qkv", "ctx", "lse", "pre1", "mean1", "rstd1", "x1", "u", "g", "pre2", "mean2", "rstd2", "keep_mask", "y")
@@ -142,6 +144,14 @@ def lib():
         h.vb_encoder_bwd_ckpt.argtypes = [_P, _I, _P, _P, _P, _P, _P, _P, _P, _P]
         h.vb_encoder_fwd_ckpt_varlen.argtypes = [_P, _I, _P, _I, _P, _P, _P, _P]
         h.vb_encoder_bwd_ckpt_varlen.argtypes = [_P, _I, _P, _I, _P, _P, _P, _P, _P, _P, _P, _P]
+        h.vb_encoder_arena_layout_ffnrc.restype = ctypes.c_int64
+        h.vb_encoder_arena_layout_ffnrc.argtypes = [_I, _I, _I, _I, _I, _I, _P, _P]
+        h.vb_encoder_arena_layout_ffnrc_varlen.restype = ctypes.c_int64
+        h.vb_encoder_arena_layout_ffnrc_varlen.argtypes = [_I, _I, _I, _I, _I, _I, _I, _P, _P]
+        h.vb_encoder_fwd_ffnrc.argtypes = [_P, _I, _P, _P, _P, _P]
+        h.vb_encoder_bwd_ffnrc.argtypes = [_P, _I, _P, _P, _P, _P, _P, _P, _P, _P]
+        h.vb_encoder_fwd_ffnrc_varlen.argtypes = [_P, _I, _P, _I, _P, _P, _P, _P]
+        h.vb_encoder_bwd_ffnrc_varlen.argtypes = [_P, _I, _P, _I, _P, _P, _P, _P, _P, _P, _P, _P]
         _lib = h
     return _lib
 

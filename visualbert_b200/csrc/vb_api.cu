@@ -71,6 +71,15 @@ static int check_layer(const vb_layer_desc* d, const LayerRows& r) {
     return 0;
 }
 
+// step 5 of a training forward: s->u = gelu'(x1 W1^T + b), s->g = gelu(x1 W1^T + b). acts.u is private to the library, so
+// gelu' is kept tile-native whenever the shape allows. The backward of vb_encoder_bwd_ffnrc calls it again to rebuild both.
+static int ffn_up(const vb_layer_desc* d, const vb_layer_acts* s, int M, cudaStream_t st) {
+    vb_gemm_args a = fwd_args(s->x1, d->w_inter, s->u, M, d->inter, d->hidden);
+    a.bias = d->b_inter; a.epilogue = VB_EPI_GELU; a.aux_out = s->g; a.ld_aux = d->inter;
+    a.gp_tiled = gemm_gp_tiled_ok(M, d->inter) ? 1 : 0;
+    return gemm(a, st);
+}
+
 // for_bwd = false (vb_encoder_infer): the same launches with the same arguments, but nothing only a backward reads is stored —
 // s->u is not touched (the FFN-up epilogue writes gelu(u) alone) and s->lse, s->mean1/2, s->rstd1/2 may be NULL.
 // ln2 = false (the recompute of vb_encoder_bwd_ckpt): stop after step 6; the LN2 output and statistics are already kept, and
@@ -96,14 +105,12 @@ int layer_fwd(const vb_layer_desc* d, const void* x_in, void* x_out, const vb_la
     VB_TRY(gemm(a, st));
     VB_TRY(ln_fwd(s->pre1, H, d->ln1_gamma, d->ln1_beta, s->x1, H, s->mean1, s->rstd1, M, H, kLnEps, st));
     if (for_bwd) {
-        a = fwd_args(s->x1, d->w_inter, s->u, M, I, H);
-        a.bias = d->b_inter; a.epilogue = VB_EPI_GELU; a.aux_out = s->g; a.ld_aux = I;
-        a.gp_tiled = gemm_gp_tiled_ok(M, I) ? 1 : 0;   // acts.u is private to the library: tile-native whenever the shape allows
+        VB_TRY(ffn_up(d, s, M, st));
     } else {
         a = fwd_args(s->x1, d->w_inter, s->g, M, I, H);
         a.bias = d->b_inter; a.epilogue = VB_EPI_GELU_FWD;
+        VB_TRY(gemm(a, st));
     }
-    VB_TRY(gemm(a, st));
     a = fwd_args(s->g, d->w_out, s->pre2, M, H, I);
     a.bias = d->b_out; a.addend = s->x1; a.ld_add = H;
     a.dropout_p = d->hidden_dropout; a.dropout_seed = d->seed; a.dropout_stream = drop_stream(d->layer_index, kSiteFfnOut);
@@ -191,11 +198,14 @@ int layer_bwd(const vb_layer_desc* d, const void* x_in, const vb_layer_acts* s, 
 static long long align256(long long x) { return (x + 255) / 256 * 256; }
 
 // M rows per layer (B * S dense, total varlen); lse holds A * M floats either way ([B, A, S] or [A, total]); the keep bits are
-// laid out for (B, S) with S the longest sequence
-long long encoder_arena_layout(int B, int S, int H, int A, int I, int attn_drop, long long* off, long long packed_rows = -1) {
+// laid out for (B, S) with S the longest sequence. shared_ffn (vb_encoder_fwd_ffnrc): u and g live in the shared FFN buffer and
+// take no room in the slot.
+long long encoder_arena_layout(int B, int S, int H, int A, int I, int attn_drop, long long* off, long long packed_rows = -1,
+                               bool shared_ffn = false) {
     const long long M = packed_rows >= 0 ? packed_rows : static_cast<long long>(B) * S;
+    const long long ffn = shared_ffn ? 0 : M * I * 2;
     const long long sizes[VB_ENCODER_ARENA_BUFFERS] = {
-        M * 3 * H * 2, M * H * 2, static_cast<long long>(A) * M * 4, M * H * 2, M * 4, M * 4, M * H * 2, M * I * 2, M * I * 2,
+        M * 3 * H * 2, M * H * 2, static_cast<long long>(A) * M * 4, M * H * 2, M * 4, M * 4, M * H * 2, ffn, ffn,
         M * H * 2, M * 4, M * 4, attn_drop ? attn_keep_bytes(B, S, A) : 0, M * H * 2};
     long long o = 0;
     for (int i = 0; i < VB_ENCODER_ARENA_BUFFERS; ++i) {
@@ -205,20 +215,33 @@ long long encoder_arena_layout(int B, int S, int H, int A, int I, int attn_drop,
     return o;
 }
 
-static void arena_acts(const vb_layer_desc* d, void* arena, int l, vb_layer_acts* a, void** y, const LayerRows& rows) {
+// the shared FFN buffer of vb_encoder_fwd_ffnrc: gelu'(u) at byte 0 (tile-native when gemm_gp_tiled_ok), g at half its size
+static long long shared_ffn_bytes(long long M, int I) { return 2 * align256(M * I * 2); }
+
+// ffn: nullptr for an arena of vb_encoder_arena_layout; else the shared FFN buffer, with the slot stride of the _ffnrc layout
+static void arena_acts(const vb_layer_desc* d, void* arena, int l, vb_layer_acts* a, void** y, const LayerRows& rows,
+                       void* ffn = nullptr) {
     long long off[VB_ENCODER_ARENA_BUFFERS];
-    const long long stride = encoder_arena_layout(d->batch, d->seq, d->hidden, d->heads, d->inter, d->attn_dropout > 0.f, off,
-                                                  rows.cu_seqlens != nullptr ? rows.total : -1);
+    const long long packed = rows.cu_seqlens != nullptr ? rows.total : -1;
+    const long long stride = encoder_arena_layout(d->batch, d->seq, d->hidden, d->heads, d->inter, d->attn_dropout > 0.f, off, packed,
+                                                  ffn != nullptr);
     char* base = static_cast<char*>(arena) + l * stride;
     a->qkv = base + off[0]; a->ctx = base + off[1]; a->lse = reinterpret_cast<float*>(base + off[2]);
     a->pre1 = base + off[3]; a->mean1 = reinterpret_cast<float*>(base + off[4]); a->rstd1 = reinterpret_cast<float*>(base + off[5]);
     a->x1 = base + off[6]; a->u = base + off[7]; a->g = base + off[8]; a->pre2 = base + off[9];
+    if (ffn != nullptr) {
+        const long long M = packed >= 0 ? packed : static_cast<long long>(d->batch) * d->seq;
+        a->u = ffn;
+        a->g = static_cast<char*>(ffn) + shared_ffn_bytes(M, d->inter) / 2;
+    }
     a->mean2 = reinterpret_cast<float*>(base + off[10]); a->rstd2 = reinterpret_cast<float*>(base + off[11]);
     a->keep_mask = d->attn_dropout > 0.f ? base + off[12] : nullptr;
     *y = base + off[13];
 }
 
-int encoder_fwd(const vb_layer_desc* descs, int n, const void* x_in, void* arena, cudaStream_t st, const LayerRows& rows = kDenseRows) {
+// ffn (vb_encoder_fwd_ffnrc): every layer's u and g go to that one buffer instead of the layer's slot
+int encoder_fwd(const vb_layer_desc* descs, int n, const void* x_in, void* arena, cudaStream_t st, const LayerRows& rows = kDenseRows,
+                void* ffn = nullptr) {
     VB_REQUIRE(descs && n > 0 && x_in && arena, "encoder_fwd: null pointer / no layers");
     const void* x = x_in;
     for (int l = 0; l < n; ++l) {
@@ -227,15 +250,18 @@ int encoder_fwd(const vb_layer_desc* descs, int n, const void* x_in, void* arena
                    (descs[l].attn_dropout > 0.f) == (descs[0].attn_dropout > 0.f), "encoder_fwd: layers differ in shape");
         vb_layer_acts a;
         void* y;
-        arena_acts(&descs[l], arena, l, &a, &y, rows);
+        arena_acts(&descs[l], arena, l, &a, &y, rows, ffn);
         VB_TRY(layer_fwd(&descs[l], x, y, &a, st, rows));
         x = y;
     }
     return 0;
 }
 
+// ffn (vb_encoder_bwd_ffnrc): the shared FFN buffer as vb_encoder_fwd_ffnrc left it, holding the top layer's u and g; below the
+// top layer, the FFN-up GEMM of layer l's forward rebuilds them from slot l's x1 before its backward
 int encoder_bwd(const vb_layer_desc* descs, int n, const void* x_in, void* arena, const void* dy, void* dx,
-                const vb_layer_grads* grads, const vb_layer_scratch* w, cudaStream_t st, const LayerRows& rows = kDenseRows) {
+                const vb_layer_grads* grads, const vb_layer_scratch* w, cudaStream_t st, const LayerRows& rows = kDenseRows,
+                void* ffn = nullptr) {
     VB_REQUIRE(descs && n > 0 && x_in && arena && dy && grads && w, "encoder_bwd: null pointer / no layers");
     for (int l = 0; l < n; ++l) VB_TRY(check_grads(&grads[l]));   // a refused call launches nothing
     // the gradient between layers ping-pongs inside `dx` (vb_layer_bwd allows dx to alias dy). Without dx it travels in
@@ -246,14 +272,16 @@ int encoder_bwd(const vb_layer_desc* descs, int n, const void* x_in, void* arena
     for (int l = n - 1; l >= 0; --l) {
         vb_layer_acts a;
         void* y;
-        arena_acts(&descs[l], arena, l, &a, &y, rows);
+        arena_acts(&descs[l], arena, l, &a, &y, rows, ffn);
         const void* xl = x_in;
         if (l > 0) {
             vb_layer_acts ap;
             void* yp;
-            arena_acts(&descs[l - 1], arena, l - 1, &ap, &yp, rows);
+            arena_acts(&descs[l - 1], arena, l - 1, &ap, &yp, rows, ffn);
             xl = yp;
         }
+        if (ffn != nullptr && l < n - 1)
+            VB_TRY(ffn_up(&descs[l], &a, rows.cu_seqlens != nullptr ? rows.total : descs[l].batch * descs[l].seq, st));
         VB_TRY(layer_bwd(&descs[l], xl, &a, g_in, l > 0 ? carry : dx, &grads[l], w, st, rows));
         g_in = carry;
     }
@@ -347,10 +375,9 @@ long long ckpt_layout(long long M, int H, long long* off) {
     return o;
 }
 
-// every descriptor and gradient entry of a checkpointed call, before its first launch: a refused call launches nothing
-static int check_ckpt_call(const vb_layer_desc* descs, int n, const void* ckpt, const LayerRows& rows, const char* what) {
+// every descriptor of a checkpointed or _ffnrc call, before its first launch: a refused call launches nothing
+static int check_stack(const vb_layer_desc* descs, int n, const LayerRows& rows, const char* what) {
     VB_REQUIRE(descs && n > 0, "%s: null descriptors / no layers", what);
-    VB_REQUIRE(n == 1 || ckpt != nullptr, "%s: ckpt is NULL with %d layers", what, n);
     const vb_layer_desc& d0 = descs[0];
     for (int l = 0; l < n; ++l) {
         VB_TRY(check_layer(&descs[l], rows));
@@ -359,6 +386,25 @@ static int check_ckpt_call(const vb_layer_desc* descs, int n, const void* ckpt, 
                    "%s: layers differ in shape", what);
     }
     return 0;
+}
+
+// and, for a backward, every gradient entry and the scratch its layers need
+static int check_stack_bwd(const vb_layer_desc* descs, int n, const vb_layer_grads* grads, const vb_layer_scratch* w,
+                           const LayerRows& rows, const char* what) {
+    VB_REQUIRE(grads && w, "%s: null pointer", what);
+    const int M = rows.cu_seqlens != nullptr ? rows.total : descs[0].batch * descs[0].seq;
+    VB_TRY(det_require(layer_bwd_det_bytes(M, descs[0].hidden, descs[0].inter), "layer backward"));
+    for (int l = 0; l < n; ++l) {
+        VB_TRY(check_grads(&grads[l]));
+        VB_REQUIRE(descs[l].hidden_dropout <= 0.f || w->d_pre_drop, "%s: d_pre_drop scratch required when hidden_dropout > 0", what);
+    }
+    return 0;
+}
+
+static int check_ckpt_call(const vb_layer_desc* descs, int n, const void* ckpt, const LayerRows& rows, const char* what) {
+    VB_REQUIRE(descs && n > 0, "%s: null descriptors / no layers", what);
+    VB_REQUIRE(n == 1 || ckpt != nullptr, "%s: ckpt is NULL with %d layers", what, n);
+    return check_stack(descs, n, rows, what);
 }
 
 // the slot's activations with LN2's statistics taken from checkpoint l, and the checkpointed output y of layer l
@@ -408,13 +454,7 @@ int encoder_bwd_ckpt(const vb_layer_desc* descs, int n, const void* x_in, void* 
                      const vb_layer_grads* grads, const vb_layer_scratch* w, cudaStream_t st, const LayerRows& rows = kDenseRows) {
     VB_TRY(check_ckpt_call(descs, n, ckpt, rows, "encoder_bwd_ckpt"));
     VB_REQUIRE(x_in && slot && dy && grads && w, "encoder_bwd_ckpt: null pointer");
-    const vb_layer_desc& d0 = descs[0];
-    const int M = rows.cu_seqlens != nullptr ? rows.total : d0.batch * d0.seq;
-    VB_TRY(det_require(layer_bwd_det_bytes(M, d0.hidden, d0.inter), "layer backward"));
-    for (int l = 0; l < n; ++l) {
-        VB_TRY(check_grads(&grads[l]));
-        VB_REQUIRE(descs[l].hidden_dropout <= 0.f || w->d_pre_drop, "encoder_bwd_ckpt: d_pre_drop scratch required when hidden_dropout > 0");
-    }
+    VB_TRY(check_stack_bwd(descs, n, grads, w, rows, "encoder_bwd_ckpt"));
     void* const carry = dx != nullptr ? dx : w->d_x1;
     const void* g_in = dy;
     for (int l = n - 1; l >= 0; --l) {
@@ -437,6 +477,27 @@ int encoder_bwd_ckpt(const vb_layer_desc* descs, int n, const void* x_in, void* 
         g_in = carry;
     }
     return 0;
+}
+
+// ---- selective recomputation: every layer's FFN intermediates in one shared buffer, rebuilt before each lower layer's backward ----
+long long ffnrc_layout(int B, int S, int H, int A, int I, int attn_drop, long long packed_rows, long long* off, long long* ffn) {
+    if (ffn) *ffn = shared_ffn_bytes(packed_rows >= 0 ? packed_rows : static_cast<long long>(B) * S, I);
+    return encoder_arena_layout(B, S, H, A, I, attn_drop, off, packed_rows, true);
+}
+
+int encoder_fwd_ffnrc(const vb_layer_desc* descs, int n, const void* x_in, void* arena, void* ffn, cudaStream_t st,
+                      const LayerRows& rows = kDenseRows) {
+    VB_TRY(check_stack(descs, n, rows, "encoder_fwd_ffnrc"));
+    VB_REQUIRE(x_in && arena && ffn, "encoder_fwd_ffnrc: null x_in / arena / ffn");
+    return encoder_fwd(descs, n, x_in, arena, st, rows, ffn);
+}
+
+int encoder_bwd_ffnrc(const vb_layer_desc* descs, int n, const void* x_in, void* arena, void* ffn, const void* dy, void* dx,
+                      const vb_layer_grads* grads, const vb_layer_scratch* w, cudaStream_t st, const LayerRows& rows = kDenseRows) {
+    VB_TRY(check_stack(descs, n, rows, "encoder_bwd_ffnrc"));
+    VB_REQUIRE(x_in && arena && ffn && dy, "encoder_bwd_ffnrc: null pointer");
+    VB_TRY(check_stack_bwd(descs, n, grads, w, rows, "encoder_bwd_ffnrc"));
+    return encoder_bwd(descs, n, x_in, arena, dy, dx, grads, w, st, rows, ffn);
 }
 
 static int check_embed(const vb_embed_desc* d) {
@@ -675,6 +736,54 @@ int vb_encoder_bwd_ckpt_varlen(const vb_layer_desc* descs, int32_t n_layers, con
     if (total <= 0) { vb::set_error("vb_encoder_bwd_ckpt_varlen: total (%d) must be > 0", total); return 2; }
     const vb::LayerRows rows = {cu_seqlens, total};
     return vb::encoder_bwd_ckpt(descs, n_layers, x_in, ckpt, slot, dy, dx, grads, scratch, static_cast<cudaStream_t>(stream), rows);
+}
+int64_t vb_encoder_arena_layout_ffnrc(int32_t batch, int32_t seq, int32_t hidden, int32_t heads, int32_t inter,
+                                      int32_t attn_dropout_on, int64_t* offsets, int64_t* ffn_bytes) {
+    if (batch <= 0 || seq <= 0 || hidden <= 0 || heads <= 0 || inter <= 0) {
+        vb::set_error("vb_encoder_arena_layout_ffnrc: bad shape (batch %d, seq %d, hidden %d, heads %d, inter %d)", batch, seq,
+                      hidden, heads, inter);
+        return -1;
+    }
+    long long off[VB_ENCODER_ARENA_BUFFERS], ffn;
+    const long long stride = vb::ffnrc_layout(batch, seq, hidden, heads, inter, attn_dropout_on, -1, off, &ffn);
+    if (offsets) for (int i = 0; i < VB_ENCODER_ARENA_BUFFERS; ++i) offsets[i] = off[i];
+    if (ffn_bytes) *ffn_bytes = ffn;
+    return stride;
+}
+int64_t vb_encoder_arena_layout_ffnrc_varlen(int32_t batch, int32_t max_seq, int32_t total, int32_t hidden, int32_t heads,
+                                             int32_t inter, int32_t attn_dropout_on, int64_t* offsets, int64_t* ffn_bytes) {
+    if (batch <= 0 || max_seq <= 0 || total < 0 || hidden <= 0 || heads <= 0 || inter <= 0) {
+        vb::set_error("vb_encoder_arena_layout_ffnrc_varlen: bad shape (batch %d, max_seq %d, total %d, hidden %d, heads %d, inter %d)",
+                      batch, max_seq, total, hidden, heads, inter);
+        return -1;
+    }
+    long long off[VB_ENCODER_ARENA_BUFFERS], ffn;
+    const long long stride = vb::ffnrc_layout(batch, max_seq, hidden, heads, inter, attn_dropout_on, total, off, &ffn);
+    if (offsets) for (int i = 0; i < VB_ENCODER_ARENA_BUFFERS; ++i) offsets[i] = off[i];
+    if (ffn_bytes) *ffn_bytes = ffn;
+    return stride;
+}
+int vb_encoder_fwd_ffnrc(const vb_layer_desc* descs, int32_t n_layers, const void* x_in, void* arena, void* ffn, void* stream) {
+    return vb::encoder_fwd_ffnrc(descs, n_layers, x_in, arena, ffn, static_cast<cudaStream_t>(stream));
+}
+int vb_encoder_bwd_ffnrc(const vb_layer_desc* descs, int32_t n_layers, const void* x_in, void* arena, void* ffn, const void* dy,
+                         void* dx, const vb_layer_grads* grads, const vb_layer_scratch* scratch, void* stream) {
+    return vb::encoder_bwd_ffnrc(descs, n_layers, x_in, arena, ffn, dy, dx, grads, scratch, static_cast<cudaStream_t>(stream));
+}
+int vb_encoder_fwd_ffnrc_varlen(const vb_layer_desc* descs, int32_t n_layers, const int32_t* cu_seqlens, int32_t total,
+                                const void* x_in, void* arena, void* ffn, void* stream) {
+    if (cu_seqlens == nullptr) { vb::set_error("vb_encoder_fwd_ffnrc_varlen: cu_seqlens is NULL"); return 2; }
+    if (total <= 0) { vb::set_error("vb_encoder_fwd_ffnrc_varlen: total (%d) must be > 0", total); return 2; }
+    const vb::LayerRows rows = {cu_seqlens, total};
+    return vb::encoder_fwd_ffnrc(descs, n_layers, x_in, arena, ffn, static_cast<cudaStream_t>(stream), rows);
+}
+int vb_encoder_bwd_ffnrc_varlen(const vb_layer_desc* descs, int32_t n_layers, const int32_t* cu_seqlens, int32_t total,
+                                const void* x_in, void* arena, void* ffn, const void* dy, void* dx, const vb_layer_grads* grads,
+                                const vb_layer_scratch* scratch, void* stream) {
+    if (cu_seqlens == nullptr) { vb::set_error("vb_encoder_bwd_ffnrc_varlen: cu_seqlens is NULL"); return 2; }
+    if (total <= 0) { vb::set_error("vb_encoder_bwd_ffnrc_varlen: total (%d) must be > 0", total); return 2; }
+    const vb::LayerRows rows = {cu_seqlens, total};
+    return vb::encoder_bwd_ffnrc(descs, n_layers, x_in, arena, ffn, dy, dx, grads, scratch, static_cast<cudaStream_t>(stream), rows);
 }
 int vb_embed_fwd(const vb_embed_desc* d, void* y, const vb_embed_acts* acts, void* stream) {
     return vb::embed_fwd_api(d, y, acts, static_cast<cudaStream_t>(stream));

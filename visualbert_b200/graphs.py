@@ -52,9 +52,9 @@ class GraphedStep:
     (load_state_dict, a new set of tensors) or whose (b1, b2, e, max_grad_norm) changed is dropped and captured again. With
     gradient accumulation the optimizer must stay outside (it steps once per several calls).
 
-    The set of trainable parameters (requires_grad) and the activation-checkpointing flag (set_activation_checkpointing) are part
-    of the signature: after a parameter is frozen or unfrozen, or the flag changes, the next calls warm up and capture again, as
-    for a new input shape."""
+    The set of trainable parameters (requires_grad) and the activation-checkpointing and FFN-recompute flags
+    (set_activation_checkpointing, set_ffn_recompute) are part of the signature: after a parameter is frozen or unfrozen, or a
+    flag changes, the next calls warm up and capture again, as for a new input shape."""
 
     def __init__(self, model, sync, loss_scale=None, warmup=1, max_graphs=4, optimizer=None):
         if not model.training:
@@ -112,9 +112,10 @@ class GraphedStep:
 
     def __call__(self, batch):
         # which parameters train is part of the signature: a graph writes the gradients of the set it was captured with; so is
-        # activation checkpointing, which changes the calls (and the memory) of the step
-        sig = (_signature(batch), tuple(p.requires_grad for p in self.model.parameters()),
-               self.model.bert.encoder.activation_checkpointing)
+        # activation checkpointing and FFN recomputation, which change the calls (and the memory) of the step
+        enc = self.model.bert.encoder
+        sig = (_signature(batch), tuple(p.requires_grad for p in self.model.parameters()), enc.activation_checkpointing,
+               enc.ffn_recompute)
         entry = self.graphs.get(sig)
         if entry is not None and self.optimizer is not None:
             if entry.opt_signature != self.optimizer._graph_signature():   # the graph holds stale pointers or arguments

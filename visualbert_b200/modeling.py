@@ -151,6 +151,8 @@ def _encoder_meta(owner, layers, seed, **more):
     """meta of one ops.bert_encoder / ops.bert_layer call over `layers`, for the module that makes the call. Each such
     module keeps its own ops.EncoderPlan: a plan shared between callers would be rebuilt at every call."""
     l0, train = layers[0], owner.training
+    # full checkpointing keeps no FFN intermediate either, so it governs when both switches are on
+    ckpt = bool(owner.__dict__.get("activation_checkpointing", False))
     plan = owner.__dict__.get("_plan")
     if plan is None:
         plan = owner.__dict__["_plan"] = ops.EncoderPlan()
@@ -158,7 +160,7 @@ def _encoder_meta(owner, layers, seed, **more):
                 hidden_dropout=l0.hidden_dropout_prob if train else 0.0,
                 attn_dropout=l0.attention_probs_dropout_prob if train else 0.0, seed=int(seed), train=train,
                 caches=[l._weights for l in layers], plan=plan, seed_offset=ops.current_seed_offset() if train else None,
-                checkpoint=bool(owner.__dict__.get("activation_checkpointing", False)), **more)
+                checkpoint=ckpt, ffn_recompute=bool(owner.__dict__.get("ffn_recompute", False)) and not ckpt, **more)
 
 
 class BertLayer(nn.Module):
@@ -208,6 +210,7 @@ class BertEncoder(nn.Module):
         self.layer = nn.ModuleList([BertLayer(config, i) for i in range(config.num_hidden_layers)])
         self.output_attention_weights = getattr(config, "output_attention_weights", False)
         self.activation_checkpointing = False   # BertVisualModel.set_activation_checkpointing
+        self.ffn_recompute = False              # BertVisualModel.set_ffn_recompute
 
     def forward(self, hidden_states, attention_mask, output_all_encoded_layers=True, seed=0, varlen=None,
                 output_attention_weights=None):
@@ -548,6 +551,21 @@ class BertVisualModel(PreTrainedBertModel):
         (output_all_encoded_layers=True in training mode under grad) keeps one single-layer arena per layer, as without the
         flag."""
         self.encoder.activation_checkpointing = bool(flag)
+        return self
+
+    def set_ffn_recompute(self, flag=True):
+        """Opt-in selective recomputation of the encoder's FFN intermediates, off by default.
+
+        When on, a training forward of the whole-encoder call keeps every layer's activations except gelu(u) and gelu'(u) of its
+        FFN (2 * rows * intermediate_size bf16, half of a layer's activation memory): one buffer shared by all layers holds them
+        for the layer being run, and the backward call rebuilds them for each layer below the top one with the FFN-up GEMM of
+        its forward (vb_encoder_fwd_ffnrc / vb_encoder_bwd_ffnrc). That GEMM has the forward's weights, epilogue and tiling, so
+        the loss, the outputs and, in deterministic mode, every gradient are bit for bit those of the default path; a step costs
+        L - 1 more GEMMs. Read at every forward; works with set_unpadded, set_graph_capturable (GraphedStep captures a new graph
+        when the flag changes), deterministic mode, frozen parameters, output_attention_weights and bypass_transformer (its
+        text encoder call). With set_activation_checkpointing also on, full checkpointing governs. The padded per-layer route
+        (output_all_encoded_layers=True in training mode under grad) and forward-only calls are not changed."""
+        self.encoder.ffn_recompute = bool(flag)
         return self
 
     def set_unpadded(self, flag=True):

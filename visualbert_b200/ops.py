@@ -491,7 +491,13 @@ class _EncoderFn(torch.autograd.Function):
     With meta["checkpoint"] (activation checkpointing) the call keeps one arena slot and L - 1 checkpoint regions (each lower
     layer's output and LayerNorm-2 statistics) instead of L slots: vb_encoder_fwd_ckpt / vb_encoder_bwd_ckpt (and their _varlen
     forms) recompute each lower layer inside the backward call. Outputs l < L - 1 are views of the checkpoint buffer, the last one
-    a view of the slot; the attention maps come from the forward call itself. Same bits as the arena call."""
+    a view of the slot; the attention maps come from the forward call itself. Same bits as the arena call.
+
+    With meta["ffn_recompute"] (selective recomputation; meta["checkpoint"] wins when both are set) the arena slots keep no FFN
+    intermediate: every layer's gelu'(u) and gelu(u) go to one shared buffer, kept on ctx until the backward, and
+    vb_encoder_bwd_ffnrc rebuilds them for each lower layer with one FFN-up GEMM (vb_encoder_fwd_ffnrc / vb_encoder_bwd_ffnrc and
+    their _varlen forms). The attention maps are read from the slots one layer at a time. Same launches as the arena call plus
+    L - 1 GEMMs in the backward, same bits."""
 
     @staticmethod
     def _shape(x, meta):
@@ -515,29 +521,48 @@ class _EncoderFn(torch.autograd.Function):
             if meta.get("checkpoint"):
                 outs, maps, arena, ckpt = _EncoderFn._forward_ckpt(x, descs, B, S, H, A, I, L, M, oshape, vl, stride, off, meta)
                 ctx.meta, ctx.descs, ctx.arena, ctx.ckpt, ctx.params, ctx.weights = meta, descs, arena, ckpt, params, weights
+                ctx.ffn = None
                 ctx.shape = (B, S, H, A, I, L, M, oshape)
                 ctx.save_for_backward(x, mbias)
                 ctx.mark_non_differentiable(*outs[:-1], *maps)
                 ctx.set_materialize_grads(False)
                 return outs + maps
+            ffn = None
+            if meta.get("ffn_recompute"):
+                stride, off, ffn_bytes = _ffnrc_layout(B, S, H, A, I, M, vl, meta)
+                ffn = torch.empty(ffn_bytes, device=x.device, dtype=torch.uint8)
             arena = torch.empty(L * stride, device=x.device, dtype=torch.uint8)
-            if vl is None:
+            if vl is None and ffn is None:
                 _lib.check(_lib.lib().vb_encoder_fwd(descs, L, ctypes.c_void_p(x.data_ptr()), ctypes.c_void_p(arena.data_ptr()),
                                                      _stream()), "vb_encoder_fwd")
-            else:
+            elif vl is None:
+                _lib.check(_lib.lib().vb_encoder_fwd_ffnrc(descs, L, x.data_ptr(), arena.data_ptr(), ffn.data_ptr(), _stream()),
+                           "vb_encoder_fwd_ffnrc")
+            elif ffn is None:
                 _lib.check(_lib.lib().vb_encoder_fwd_varlen(descs, L, vl["cu_seqlens"].data_ptr(), M, x.data_ptr(),
                                                             arena.data_ptr(), _stream()), "vb_encoder_fwd_varlen")
+            else:
+                _lib.check(_lib.lib().vb_encoder_fwd_ffnrc_varlen(descs, L, vl["cu_seqlens"].data_ptr(), M, x.data_ptr(),
+                                                                  arena.data_ptr(), ffn.data_ptr(), _stream()),
+                           "vb_encoder_fwd_ffnrc_varlen")
             maps = ()
             if meta.get("attn_maps"):
                 if vl is not None:
                     raise ValueError("bert_encoder: attention maps need a dense (padded) call")
                 probs = torch.empty(L, B, A, S, S, device=x.device, dtype=torch.float32)
-                _lib.check(_lib.lib().vb_encoder_attention_probs(descs, L, arena.data_ptr(), probs.data_ptr(), _stream()),
-                           "vb_encoder_attention_probs")
+                if ffn is None:
+                    _lib.check(_lib.lib().vb_encoder_attention_probs(descs, L, arena.data_ptr(), probs.data_ptr(), _stream()),
+                               "vb_encoder_attention_probs")
+                else:   # the call knows the default slot stride only; qkv sits at offset 0 of a slot in both layouts
+                    for l in range(L):
+                        _lib.check(_lib.lib().vb_encoder_attention_probs(ctypes.addressof(descs) + l * ctypes.sizeof(_lib.LayerDesc), 1,
+                                                                         arena.data_ptr() + l * stride, probs[l].data_ptr(), _stream()),
+                                   "vb_encoder_attention_probs")
                 maps = tuple(probs.unbind(0))
         n = M * H * 2
         outs = tuple(arena[l * stride + off[13]: l * stride + off[13] + n].view(_BF16).view(oshape) for l in range(L))
         ctx.meta, ctx.descs, ctx.arena, ctx.ckpt, ctx.params, ctx.weights = meta, descs, arena, None, params, weights
+        ctx.ffn = ffn
         ctx.shape = (B, S, H, A, I, L, M, oshape)
         ctx.save_for_backward(x, mbias)
         ctx.mark_non_differentiable(*outs[:-1], *maps)
@@ -596,6 +621,13 @@ class _EncoderFn(torch.autograd.Function):
                 _lib.check(_lib.lib().vb_encoder_bwd_ckpt_varlen(descs, L, vl["cu_seqlens"].data_ptr(), M, x.data_ptr(), _ptr(ctx.ckpt),
                                                                  ctx.arena.data_ptr(), dy.data_ptr(), _ptr(dx), grads, ctypes.byref(sc),
                                                                  _stream()), "vb_encoder_bwd_ckpt_varlen")
+            elif ctx.ffn is not None and vl is None:
+                _lib.check(_lib.lib().vb_encoder_bwd_ffnrc(descs, L, x.data_ptr(), ctx.arena.data_ptr(), ctx.ffn.data_ptr(), dy.data_ptr(),
+                                                           _ptr(dx), grads, ctypes.byref(sc), _stream()), "vb_encoder_bwd_ffnrc")
+            elif ctx.ffn is not None:
+                _lib.check(_lib.lib().vb_encoder_bwd_ffnrc_varlen(descs, L, vl["cu_seqlens"].data_ptr(), M, x.data_ptr(),
+                                                                  ctx.arena.data_ptr(), ctx.ffn.data_ptr(), dy.data_ptr(), _ptr(dx),
+                                                                  grads, ctypes.byref(sc), _stream()), "vb_encoder_bwd_ffnrc_varlen")
             elif vl is None:
                 _lib.check(_lib.lib().vb_encoder_bwd(descs, L, ctypes.c_void_p(x.data_ptr()), ctypes.c_void_p(ctx.arena.data_ptr()),
                                                      ctypes.c_void_p(dy.data_ptr()), ctypes.c_void_p(_ptr(dx)), grads,
@@ -604,7 +636,7 @@ class _EncoderFn(torch.autograd.Function):
                 _lib.check(_lib.lib().vb_encoder_bwd_varlen(descs, L, vl["cu_seqlens"].data_ptr(), M, x.data_ptr(),
                                                             ctx.arena.data_ptr(), dy.data_ptr(), _ptr(dx), grads, ctypes.byref(sc),
                                                             _stream()), "vb_encoder_bwd_varlen")
-        ctx.arena = ctx.ckpt = None
+        ctx.arena = ctx.ckpt = ctx.ffn = None
         out = [None] * (16 * L)
         for i, g in pieces:
             if plan[i // 16][0]:
@@ -612,6 +644,20 @@ class _EncoderFn(torch.autograd.Function):
             else:
                 out[i] = g
         return (dx, None, None) + tuple(out)
+
+
+def _ffnrc_layout(B, S, H, A, I, M, vl, meta):
+    """vb_encoder_arena_layout_ffnrc(_varlen) -> (slot stride, the 14 buffer offsets, bytes of the shared FFN buffer)."""
+    off = (ctypes.c_int64 * _lib.VB_ENCODER_ARENA_BUFFERS)()
+    ffn_bytes = ctypes.c_int64()
+    drop = 1 if meta["attn_dropout"] > 0 else 0
+    if vl is None:
+        stride = int(_lib.lib().vb_encoder_arena_layout_ffnrc(B, S, H, A, I, drop, off, ctypes.byref(ffn_bytes)))
+    else:
+        stride = int(_lib.lib().vb_encoder_arena_layout_ffnrc_varlen(B, S, M, H, A, I, drop, off, ctypes.byref(ffn_bytes)))
+    if stride < 0:
+        _lib.check(1, "vb_encoder_arena_layout_ffnrc")
+    return stride, list(off), ffn_bytes.value
 
 
 def _encoder_infer(x, mbias, meta, params):
@@ -655,7 +701,8 @@ def _encoder_infer(x, mbias, meta, params):
 def bert_encoder(x, mbias, meta, params):
     """All layers at once. meta: dict(heads, layer_index0, hidden_dropout, attn_dropout, seed, train, caches=[LayerWeights],
     plan=EncoderPlan, optional varlen=unpad_plan(...), optional attn_maps=True, optional all_layers=False, optional
-    checkpoint=True: activation checkpointing of the _EncoderFn part); params: 16 tensors
+    checkpoint=True: activation checkpointing of the _EncoderFn part, optional ffn_recompute=True: selective recomputation of
+    its FFN intermediates); params: 16 tensors
     per layer in bert_layer order. Returns the tuple of all layer outputs (only the last one is differentiable: a caller that
     needs gradients through intermediate outputs calls bert_layer once per layer) — with all_layers=False only the last
     layer's — followed, with attn_maps, by the L detached fp32 [B, A, S, S] attention maps.
